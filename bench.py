@@ -2,6 +2,7 @@
 """bench.py — the reference's headline metric on its named configurations, one JSON line on rank 0.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload mel|cluster] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 Main line (BASELINE.json configs[1], the configuration the metric is quoted on):
     log-mel of 1 h of synthetic 16 kHz mono audio, 25 ms / 10 ms frames, 512-point FFT, 80 mels -> [360 001 x 80].
@@ -20,6 +21,11 @@ Attached sub-objects, each with its own parity field:
     `streaming`: p50 / p99 latency of small `.prePadded` calls (the production callers' shape).
 With N > 1 (torchrun) units are independent: no data-path collective; NCCL carries the barrier, the MAX-reduction of
 times and the gather of labels / checksums.  Timing: barrier + device sync on both sides, MAX over ranks.
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the timed path returned in its last step as DIR/<name>.npy
+(float32 / float64): for `mel` a fixed, seeded sample of the hour's log-mel rows (`mel.npy`, with their row indices in
+`mel_rows.npy`) and the labels of the attached `cluster` run; for `cluster` its labels.  Inputs are synthetic and seeded,
+so two builds run with the same arguments can be compared output for output.
 
 --impl reference: the reference's CPU implementation of the path on the host cores, rank 0 only — for `mel` the
 float32-FFT port of AudioMelSpectrogram vectorised across frames (oracle/oracle_mel_fast.cpp; no Swift toolchain
@@ -50,6 +56,7 @@ AHC_BYTES = 8.0 * CLUSTER_D * CLUSTER_N * CLUSTER_N                       # 2.04
 C4_CLIPS, C4_SAMPLES = 512, 480_000
 C5_MEETINGS, C5_N = 64, 5_000
 MEL_TOL = 1e-4
+DUMP_MEL_ROWS = 131_072      # seeded sample of the hour's 360 001 log-mel rows: 42 MB, under the 64 MB --dump-outputs budget
 
 
 def measured_peaks():
@@ -59,7 +66,7 @@ def measured_peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not measured)"
 
 
 class ClockSampler:
@@ -207,7 +214,7 @@ def bench_mel(args, dist, clocks):
     d_out = _lib.DeviceBuffer(MEL_FRAMES * N_MELS * 4)
     d_in.upload(audio)
     K, W = args.steps, args.warmup
-    # ---- kernel-only: inputs resident in HBM (345.6 MB touched per step > 126 MB L2: nothing survives a step) ----
+    # ---- kernel-only: inputs resident in HBM (345.6 MB touched per step > 50 MB L2: nothing survives a step) ----
     step = lambda: mel.compute_device(d_in, MEL_SAMPLES, d_out)
     step64 = lambda: mel64.compute_device(d_in, MEL_SAMPLES, d_out)
     for _ in range(W):
@@ -281,13 +288,11 @@ def bench_mel(args, dist, clocks):
                     "copy_floor_ms": floor["i16"], "of_copy_floor": floor["i16"] / (e2e16_s / K * 1e3)},
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": 316.8e6, "traffic_source": "ncu --set full, profiles/r02_summary.txt: dram read 230.5 MB + write "
-                     "86.3 MB per launch (the tail of the output is still in L2 at kernel end)",
                      "kernel": "mel512_kernel<8, f32x2>", "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": MEL_BYTES_PER_HOUR},
         "config": {"workload": "log-mel STFT, 1 h synthetic 16 kHz mono, 25 ms/10 ms frames, nFFT 512, 80 mels, per GPU",
                    "samples": MEL_SAMPLES, "frames": MEL_FRAMES, "n_mels": N_MELS, "transform": "float32 (FA_MEL_PRECISION_F32)",
-                   "l2": "inputs+outputs 345.6 MB per step exceed the 126 MB L2 (no flush needed)",
+                   "l2": "inputs+outputs 345.6 MB per step exceed the 50 MB L2 (no flush needed)",
                    "parallelism": f"dp{dist.world}: one process per GPU, independent clips, no data-path collective"},
     }
     out["parity"]["ok"] = bool(diff <= MEL_TOL)
@@ -360,8 +365,6 @@ def bench_cluster(args, dist, steps=None):
                 "host_buffers": "pinned (fa_host_alloc)", "api": "fa_diarize_cluster"},
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": 42.3e6, "traffic_source": "ncu --set full, profiles/r01c_summary.txt: ahc_merge_kernel dram "
-                     "read 41.3 MB + write 1.0 MB per launch (+ 20.5 MB read by ahc_init_nn_kernel)",
                      "kernel": "ahc_merge_kernel (+ ahc_init_nn_kernel)", "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": AHC_BYTES,
                      "note": "node vectors are resident in shared memory, so algorithmic bytes are served on-chip; "
@@ -383,6 +386,20 @@ def bench_cluster(args, dist, steps=None):
     out["labels_equal_ref"] = bool(sharding.all_reduce_sum(dist, ok if dist.rank == 0 else 0.0) == 1.0)
     out["labels_deterministic_all_ranks"] = bool(sharding.all_reduce_sum(dist, same) == dist.world)
     return out, (emb, rho, psi, res)
+
+
+def dump_outputs(path, mel=None, labels=None):
+    """--dump-outputs: the last timed step's results as float32 / float64 .npy files (mel: a fixed, seeded row sample
+    that always includes the first and last 16 frames)."""
+    os.makedirs(path, exist_ok=True)
+    if mel is not None:
+        n = mel.shape[0]
+        sample = np.random.default_rng(0).choice(n, DUMP_MEL_ROWS - 32, replace=False)
+        rows = np.union1d(np.r_[0:16, n - 16:n], sample)
+        np.save(os.path.join(path, "mel_rows.npy"), rows.astype(np.float64))
+        np.save(os.path.join(path, "mel.npy"), np.ascontiguousarray(mel[rows], np.float32))
+    if labels is not None:
+        np.save(os.path.join(path, "cluster_labels.npy"), np.asarray(labels, np.float64))
 
 
 def _stats(ts):
@@ -486,6 +503,7 @@ def main():
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--only-main", action="store_true", help="skip the c4 / c5 / streaming sub-objects (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -533,7 +551,7 @@ def main():
     from fluidaudio_b200 import _lib
     dist = sharding.init_distributed()
     if _lib.device_count() < 1:
-        raise SystemExit("bench.py needs a B200: " + "no sm_100a device visible (there is no CPU fallback)")
+        raise SystemExit("bench.py needs an H100: no sm_90a device visible (there is no CPU fallback)")
     _lib.set_device(dist.local_rank)
     all_cpus = os.sched_getaffinity(0)
     numa = sharding.bind_to_gpu_numa(dist.local_rank)
@@ -557,6 +575,8 @@ def main():
         line, cluster_data = bench_cluster(args, dist)
         audio = None
     line["clocks"] = clocks.summary()
+    if args.dump_outputs and dist.is_root:
+        dump_outputs(args.dump_outputs, got32, cluster_data[3].labels)
 
     os.sched_setaffinity(0, all_cpus)      # the CPU baseline may use every host core again
     if dist.is_root and world == 1 and not args.no_cpu_baseline:

@@ -1,7 +1,7 @@
 """ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h``).
 
 The library is the product: it is built in-tree by ``__graft_entry__.build()`` / ``make -C fluidaudio_b200/csrc``.
-There is no Python or CPU fallback — if the shared object is missing, or no sm_100a device is visible, every
+There is no Python or CPU fallback — if the shared object is missing, or no sm_90a device is visible, every
 compute entry point raises.  This module never imports anything from ``oracle/``.
 """
 from __future__ import annotations

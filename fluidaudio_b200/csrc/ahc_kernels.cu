@@ -1,4 +1,4 @@
-// Centroid-linkage agglomerative clustering on one B200, bit-compatible with the reference's
+// Centroid-linkage agglomerative clustering on one H100, bit-compatible with the reference's
 // fastcluster_compute_centroid_linkage (Sources/FastClusterWrapper/FastClusterWrapper.cpp:196-244 driving
 // fastcluster_internal.hpp:1625-1800).
 //
@@ -312,10 +312,10 @@ __global__ void __launch_bounds__(256) ahc_filter_tile_kernel(int N, int D, int 
     }
 }
 
-// Pass 1 at full SIMT rate: 128 x 128 tiles of the lower triangle, 8 x 8 inner products per thread held as packed
-// float pairs (FFMA2: one issue slot per two FMAs), k in chunks of eight through double-buffered shared memory with the
+// Pass 1 at full SIMT rate: 128 x 128 tiles of the lower triangle, 8 x 8 inner products per thread held as
+// float pairs (two FFMA per pair on sm_90), k in chunks of eight through double-buffered shared memory with the
 // next chunk's two float4 global loads in flight during the arithmetic.  Rows / columns of a thread: {ty*4..+3, 64+ty*4..+3}
-// x {tx*4..+3, 64+tx*4..+3}, so the per-k operand loads are four LDS.128 (two of them warp-wide broadcasts) for 32 FFMA2.
+// x {tx*4..+3, 64+tx*4..+3}, so the per-k operand loads are four LDS.128 (two of them warp-wide broadcasts) for 64 FFMA.
 // The bounds keep the 64-column granularity of pass 2: a tile feeds column tiles 2*TJ and 2*TJ+1.
 constexpr int kGT = 128, kGK = 8;
 
@@ -326,7 +326,7 @@ __device__ __forceinline__ void cp_async16_zfill(void *smem, const void *gmem, b
 }
 
 __device__ __forceinline__ float2 ffma2_bcast(float a, float2 b, float2 c) {
-    return __ffma2_rn(make_float2(a, a), b, c);
+    return ffma2_rn(make_float2(a, a), b, c);
 }
 
 __global__ void __launch_bounds__(256, 2) ahc_filter_tile128_kernel(int N, int D, int Ns, FilterBufs F) {
@@ -1198,8 +1198,8 @@ int Solver::init(cudaStream_t s, int worker_limit) {
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
     FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 10) {
-        fa::set_error("fluidaudio_b200 requires an sm_100a device, found sm_%d%d", prop.major, prop.minor);
+    if (prop.major != 9) {
+        fa::set_error("fluidaudio_b200 requires an sm_90a device, found sm_%d%d", prop.major, prop.minor);
         return FA_NO_DEVICE;
     }
     int coop = 0;

@@ -1,4 +1,4 @@
-// Host-side solver for centroid-linkage agglomerative clustering on one B200 (see ahc_kernels.cu).
+// Host-side solver for centroid-linkage agglomerative clustering on one H100 (see ahc_kernels.cu).
 #pragma once
 
 #include "ahc_core.cuh"

@@ -57,7 +57,7 @@ static int usable_device_count() {
     int ok = 0;
     for (int i = 0; i < n; ++i) {
         cudaDeviceProp p;
-        if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 10) ++ok;
+        if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 9) ++ok;
     }
     return ok;
 }
@@ -70,7 +70,7 @@ static int require_device() {
         cached.store(c);
     }
     if (c <= 0) {
-        set_error("no sm_100a (B200) device visible; fluidaudio_b200 has no CPU fallback");
+        set_error("no sm_90a (H100) device visible; fluidaudio_b200 has no CPU fallback");
         return FA_NO_DEVICE;
     }
     return FA_OK;
@@ -479,7 +479,7 @@ using namespace fa;
     }
 
 // ------------------------------------------------------------------------------------------------ runtime
-FA_API const char *fa_version(void) { return "fluidaudio_b200 0.1.0 (sm_100a)"; }
+FA_API const char *fa_version(void) { return "fluidaudio_b200 0.1.0 (sm_90a)"; }
 FA_API const char *fa_last_error(void) { return fa::last_error(); }
 FA_API int32_t fa_device_count(void) { return usable_device_count(); }
 
@@ -1418,7 +1418,7 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
     API_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
     // Concurrency: as many sets at a time as still leaves each of them enough SMs to keep its node vectors in shared
     // memory (the merge loop is ~3x slower when they are streamed from L2): 5 000 x 256 needs 46 workers + 1 master,
-    // so three sets run side by side on 148 SMs; small sets run four at a time.
+    // so two sets run side by side on an H100's 132 SMs; small sets run four at a time.
     long long n_max = 0;
     for (int m = 0; m < set_count; ++m) n_max = std::max<long long>(n_max, set_offsets[m + 1] - set_offsets[m]);
     int lanes = std::max(1, std::min(set_count, 4));

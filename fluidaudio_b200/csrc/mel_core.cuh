@@ -25,10 +25,10 @@
 // TWO value types run through the SAME code (template parameter V):
 //   V = double  one frame per warp, transform in FP64 (the parity default, see above);
 //   V = f32x2   TWO frames per warp, each value a pair (frame A, frame B) of float32 in one 64-bit register pair,
-//               every butterfly one packed Blackwell instruction (FADD2 / FMUL2 / FFMA2: negation, half swap and the
-//               broadcast of a scalar register are free operand modifiers), twiddles exact-rounded per-lane scalars
+//               every butterfly a pair of independent float32 operations (fa_common.cuh: FADD / FMUL / FFMA per frame on
+//               sm_90), twiddles exact-rounded per-lane scalars
 //               held in registers.  Same element size (16 bytes), same layouts, same index math as the FP64 path;
-//               half the instructions per frame.  This is what the reference's own float32 vDSP_DFT does numerically
+//               FP32 instead of FP64 arithmetic per frame.  This is what the reference's own float32 vDSP_DFT does numerically
 //               (float32 noise floor: up to ~1e-4 on weak log-mel bins against the exactly rounded transform).
 //
 // Shared-memory layouts of the 256 complex values (16-byte elements; a warp-wide 16-byte access is 4 wavefronts
@@ -59,7 +59,7 @@ constexpr int kFftPad = 304;      // complex values per warp buffer (max layout 
 constexpr int kTileFrames = 16;   // frames per CTA tile; the mel stage maps 32 / kTileFrames mel bins onto one warp
 // Power tile: one row per frame PAIR, the two frames' values of a bin side by side: row[2 * bin + slot], slot = frame & 1.
 // The float32-pair transform stores both frames of a bin with ONE 64-bit store, and the filterbank stage runs two frames
-// per lane on packed FFMA2 with the weight as a broadcast scalar.  Row stride 524 floats = 2 x 260 bins + 4: 16-byte
+// per lane, both multiplied by the same weight.  Row stride 524 floats = 2 x 260 bins + 4: 16-byte
 // aligned and = 12 (mod 32) banks, so the 8 lanes (pairs) of a quarter-warp reading the same bin quad hit disjoint banks.
 constexpr int kPairStride = 524;
 // Inside a pair row bin b sits at position pow_pos(b) = b ^ ((b >> 4) & 3): the two low bits are XORed with bits 4-5, a
@@ -105,15 +105,15 @@ FA_HD f32x2 vneg(f32x2 x) {
     return r;
 }
 #if defined(__CUDA_ARCH__)
-// SASS: FADD2 / FMUL2 / FFMA2 with -R (negate) and R.F32 (scalar broadcast) operand modifiers, no extra instruction
-__device__ __forceinline__ f32x2 vadd(f32x2 x, f32x2 y) { return as_v(__fadd2_rn(as_f2(x), as_f2(y))); }
-__device__ __forceinline__ f32x2 vsub(f32x2 x, f32x2 y) { return as_v(__fadd2_rn(as_f2(x), as_f2(vneg(y)))); }
-__device__ __forceinline__ f32x2 vmul_s(f32x2 x, float s) { return as_v(__fmul2_rn(as_f2(x), make_float2(s, s))); }
+// each one FADD / FMUL / FFMA per frame, rounded exactly as the host emulator's scalar expressions below
+__device__ __forceinline__ f32x2 vadd(f32x2 x, f32x2 y) { return as_v(fadd2_rn(as_f2(x), as_f2(y))); }
+__device__ __forceinline__ f32x2 vsub(f32x2 x, f32x2 y) { return as_v(fadd2_rn(as_f2(x), as_f2(vneg(y)))); }
+__device__ __forceinline__ f32x2 vmul_s(f32x2 x, float s) { return as_v(fmul2_rn(as_f2(x), make_float2(s, s))); }
 __device__ __forceinline__ f32x2 vfma_s(f32x2 a, float s, f32x2 c) {
-    return as_v(__ffma2_rn(as_f2(a), make_float2(s, s), as_f2(c)));
+    return as_v(ffma2_rn(as_f2(a), make_float2(s, s), as_f2(c)));
 }
 __device__ __forceinline__ f32x2 vfnma_s(f32x2 a, float s, f32x2 c) {
-    return as_v(__ffma2_rn(as_f2(vneg(a)), make_float2(s, s), as_f2(c)));
+    return as_v(ffma2_rn(as_f2(vneg(a)), make_float2(s, s), as_f2(c)));
 }
 #else
 inline f32x2 vadd(f32x2 x, f32x2 y) { return f32x2{x.a + y.a, x.b + y.b}; }
@@ -431,8 +431,8 @@ FA_HD void pair_power(f32x2 zbx, f32x2 zby, f32x2 zcx, f32x2 zcy, float wx, floa
     const f32x2 xr = vadd(sr, tr), xi = vadd(si, ti);
     const f32x2 yr = vsub(sr, tr), yi = vsub(si, ti);
 #if defined(__CUDA_ARCH__)
-    const float2 pb = __ffma2_rn(as_f2(xr), as_f2(xr), __fmul2_rn(as_f2(xi), as_f2(xi)));
-    const float2 pc = __ffma2_rn(as_f2(yr), as_f2(yr), __fmul2_rn(as_f2(yi), as_f2(yi)));
+    const float2 pb = ffma2_rn(as_f2(xr), as_f2(xr), fmul2_rn(as_f2(xi), as_f2(xi)));
+    const float2 pc = ffma2_rn(as_f2(yr), as_f2(yr), fmul2_rn(as_f2(yi), as_f2(yi)));
     *reinterpret_cast<float2 *>(prow + 2 * ib) = pb;   // (frame A, frame B) of bin ib: one 64-bit store
     *reinterpret_cast<float2 *>(prow + 2 * ic) = pc;
 #else
@@ -517,16 +517,16 @@ FA_HD float mel_dot(const float *prow, const float *w, int lo, int hi) {
 }
 #if defined(__CUDACC__)
 // Two frames at once out of a pair row: p4 -> (bin, slot) interleaved values of the band's first quad (two float4 per bin
-// quad), w4 -> packed weights; four FFMA2 per quad with the weight as a broadcast scalar operand.
+// quad), w4 -> packed weights; four FFMA pairs per quad, the weight shared by both frames.
 __device__ __forceinline__ float2 mel_dot_pairs(const float4 *p4, const float4 *w4, int nq) {
     float2 acc = make_float2(0.0f, 0.0f);
 #pragma unroll 1
     for (int b = 0; b < nq; ++b) {
         const float4 x01 = p4[2 * b], x23 = p4[2 * b + 1], c = w4[b];
-        acc = __ffma2_rn(make_float2(x01.x, x01.y), make_float2(c.x, c.x), acc);
-        acc = __ffma2_rn(make_float2(x01.z, x01.w), make_float2(c.y, c.y), acc);
-        acc = __ffma2_rn(make_float2(x23.x, x23.y), make_float2(c.z, c.z), acc);
-        acc = __ffma2_rn(make_float2(x23.z, x23.w), make_float2(c.w, c.w), acc);
+        acc = ffma2_rn(make_float2(x01.x, x01.y), make_float2(c.x, c.x), acc);
+        acc = ffma2_rn(make_float2(x01.z, x01.w), make_float2(c.y, c.y), acc);
+        acc = ffma2_rn(make_float2(x23.x, x23.y), make_float2(c.z, c.z), acc);
+        acc = ffma2_rn(make_float2(x23.z, x23.w), make_float2(c.w, c.w), acc);
     }
     return acc;
 }

@@ -1,4 +1,4 @@
-// Fused log-mel frontend for sm_100a:  pre-emphasis -> Hann window -> 512-point real FFT -> |.|^2 ->
+// Fused log-mel frontend for sm_90a:  pre-emphasis -> Hann window -> 512-point real FFT -> |.|^2 ->
 // Slaney mel filterbank -> log, one persistent CTA per SM.
 //
 // Re-implements Sources/FluidAudio/Shared/AudioMelSpectrogram.swift:325-456 (computeFlatTransposed),
@@ -293,7 +293,7 @@ __global__ void __launch_bounds__(kWarps * 32, 2) mel512_kernel(const MelLaunch 
             // warp with the widest (highest) filters does not hold the block barrier; md.w = the slot's mel bin, -1 = empty
             for (int slot = warp * kGroup + mg; slot < P.n_slots; slot += kWarps * kGroup) {
                 const int4 md = fbmeta[slot];
-                // two frames per lane on packed FFMA2; rows beyond the tile's last frame hold finite leftovers: computed and
+                // two frames per lane; rows beyond the tile's last frame hold finite leftovers: computed and
                 // dropped, no divergent branch
                 const float2 a2 = mel_dot_pairs(reinterpret_cast<const float4 *>(prow + 2 * md.x),
                                                 reinterpret_cast<const float4 *>(fbw + md.z), md.y);
@@ -516,7 +516,7 @@ int MelPlan::init(const MelConfig &c) {
     }
     const bool pow2 = cfg.n_fft >= 32 && cfg.n_fft <= 4096 && (cfg.n_fft & (cfg.n_fft - 1)) == 0;
     if (!pow2 || cfg.win_length > cfg.n_fft || cfg.n_mels > 512 || cfg.hop_length > 65536) {
-        fa::set_error("mel config unsupported by the sm_100a kernels: need nFFT a power of two in 32..4096, win <= nFFT, "
+        fa::set_error("mel config unsupported by the sm_90a kernels: need nFFT a power of two in 32..4096, win <= nFFT, "
                       "nMels <= 512 (got nFFT=%d hop=%d win=%d nMels=%d)",
                       cfg.n_fft, cfg.hop_length, cfg.win_length, cfg.n_mels);
         return FA_UNSUPPORTED;
@@ -595,8 +595,8 @@ int MelPlan::init(const MelConfig &c) {
     cudaDeviceProp prop;
     FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
     num_sms = prop.multiProcessorCount;
-    if (prop.major != 10) {
-        fa::set_error("fluidaudio_b200 requires an sm_100a device, found sm_%d%d", prop.major, prop.minor);
+    if (prop.major != 9) {
+        fa::set_error("fluidaudio_b200 requires an sm_90a device, found sm_%d%d", prop.major, prop.minor);
         return FA_NO_DEVICE;
     }
 

@@ -80,10 +80,10 @@ struct MelPlan {
     size_t smem_bytes = 0;
     int num_sms = 0;
     long long launches = 0;          // kernels launched through this plan (bench.py reports it)
-    int precision = 0;               // transform arithmetic: 0 = FP64 (one frame per warp), 1 = packed float32 pairs
+    int precision = 0;               // transform arithmetic: 0 = FP64 (one frame per warp), 1 = float32 frame pairs
     int pipeline_chunks = 24;        // units a long host-buffer call is cut into (H2D / kernel / D2H overlap)
     bool zero_copy_out = false;      // time-major output in a pinned host buffer: the kernel stores straight into it
-                                     // (measured SLOWER than the staged copy on B200 + PCIe 5: 4.72 vs 4.53 ms per hour; opt-in)
+                                     // (opt-in: the staged copy is the default)
     bool inline_unit = false;        // next launch() passes its (single) unit in the kernel parameters
     bool generic = false;            // nFFT != 512 or odd hop: mel_generic_kernel (FP64 transform whatever `precision`)
     int generic_warps = 0, generic_prow = 0, generic_log2n = 0;

@@ -1,4 +1,4 @@
-// VBx refinement, gamma-weighted centroids and cosine assignment in FP64 on sm_100a.
+// VBx refinement, gamma-weighted centroids and cosine assignment in FP64 on sm_90a.
 //
 // Re-implements
 //   Sources/FluidAudio/Diarizer/Offline/Clustering/VBxClustering.swift:167-664   (runVBx)

@@ -4,7 +4,7 @@ Reference: OfflineDiarizerManager.exportEmbeddings (Sources/FluidAudio/Diarizer/
 writes `[TimedEmbedding + cluster]` as JSON when `OfflineDiarizerConfig.embeddingExportPath` is set; `PreparedDiarization`
 (PreparedDiarization.swift:8-26) is the in-memory cache that `OfflineDiarizerManager.cluster(_:)` consumes so that
 clustering can be re-run without model inference.  Here the file is the wire format between a Mac running the CoreML
-models and the B200 clustering backend: parsing is native (`fa_export_*` in libfluidaudio_b200.so).
+models and the GPU clustering backend: parsing is native (`fa_export_*` in libfluidaudio_b200.so).
 """
 from __future__ import annotations
 

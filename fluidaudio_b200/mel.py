@@ -2,7 +2,7 @@
 
 Same constructor parameters, same three entry points (``compute`` :132, ``compute_flat`` :185,
 ``compute_flat_transposed`` :299/:325), same return tuples, same "empty" guards, same non-thread-safety
-(one instance per stream of calls).  All arithmetic happens in the sm_100a kernel behind ``fa_mel_*``.
+(one instance per stream of calls).  All arithmetic happens in the sm_90a kernel behind ``fa_mel_*``.
 """
 from __future__ import annotations
 
@@ -26,7 +26,7 @@ class LogFloorMode(enum.IntEnum):
 
 class Precision(enum.IntEnum):
     f64 = 0           # FA_MEL_PRECISION_F64: transform in FP64, rounded once (default; parity with the oracle ~5e-6)
-    f32 = 1           # FA_MEL_PRECISION_F32: float32 transform like vDSP_DFT, packed two frames per warp
+    f32 = 1           # FA_MEL_PRECISION_F32: float32 transform like vDSP_DFT, two frames per warp
 
 
 _TIME_MAJOR, _MEL_MAJOR = 0, 1

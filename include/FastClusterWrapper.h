@@ -2,7 +2,7 @@
  *
  * Replaces Sources/FastClusterWrapper/include/FastClusterWrapper.h:11-40 of FluidAudio: same symbol, same status
  * values, same buffer contract, so AHCClustering.swift:40-50 links against libfluidaudio_b200.so unchanged
- * (module map: swift/FastClusterWrapper/module.modulemap).  The body runs on an sm_100a GPU; there is no CPU
+ * (module map: swift/FastClusterWrapper/module.modulemap).  The body runs on an sm_90a GPU; there is no CPU
  * fallback — without a device the call returns FASTCLUSTER_WRAPPER_RUNTIME_ERROR, which the Swift caller already
  * maps to "every point its own cluster" (AHCClustering.swift:52-55).
  */

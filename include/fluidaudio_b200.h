@@ -1,9 +1,9 @@
-/* fluidaudio_b200 — C ABI of the B200-native (sm_100a) implementation of FluidAudio's two CPU hot paths.
+/* fluidaudio_b200 — C ABI of the H100-native (sm_90a) implementation of FluidAudio's two CPU hot paths.
  *
  * Every entry point is what a Swift/cgo/ctypes FFI binding for that piece of the reference would bind:
  * plain pointers and sizes, caller-owned buffers, an int status, no exception ever crosses the boundary
  * (same conventions as the reference's only C boundary, Sources/FastClusterWrapper/include/FastClusterWrapper.h).
- * There is NO CPU fallback: without an sm_100a device every compute call returns FA_NO_DEVICE.
+ * There is NO CPU fallback: without an sm_90a device every compute call returns FA_NO_DEVICE.
  *
  * Reference interfaces replaced (paths relative to the FluidAudio repository):
  *   fa_mel_*             Sources/FluidAudio/Shared/AudioMelSpectrogram.swift:18-121 (class + init),
@@ -46,7 +46,7 @@ typedef enum {
     FA_STATUS_OUTPUT_TOO_SMALL = 3,
     FA_STATUS_ALLOCATION_FAILURE = 4,
     FA_STATUS_RUNTIME_ERROR = 5,   /* e.g. NaN distance, as the reference's nan_error */
-    FA_STATUS_NO_DEVICE = 6,       /* no sm_100a GPU visible: there is deliberately no CPU fallback */
+    FA_STATUS_NO_DEVICE = 6,       /* no sm_90a GPU visible: there is deliberately no CPU fallback */
     FA_STATUS_CUDA_ERROR = 7,
     FA_STATUS_UNSUPPORTED = 8,
     FA_STATUS_UNKNOWN_ERROR = 255
@@ -55,7 +55,7 @@ typedef enum {
 /* ---- runtime ------------------------------------------------------------------------------------------- */
 const char *fa_version(void);
 const char *fa_last_error(void);            /* thread-local text of the last failure */
-int32_t fa_device_count(void);              /* sm_100a devices visible */
+int32_t fa_device_count(void);              /* sm_90a devices visible */
 fa_status fa_set_device(int32_t ordinal);   /* binds the calling thread; one process per GPU is the intended use */
 fa_status fa_device_synchronize(void);
 int64_t fa_kernel_launch_count(void);       /* kernels this library has launched in this process */
@@ -109,7 +109,7 @@ int64_t fa_mel_frame_count(const fa_mel *mel, int64_t sample_count, int32_t padd
  *   FA_MEL_PRECISION_F64  (default) DFT evaluated in FP64 and rounded once — the implementation-independent value,
  *                         reproduces the oracle to ~5e-6 in the log domain whatever the signal's dynamic range;
  *   FA_MEL_PRECISION_F32  DFT in float32 like the reference's own vDSP_DFT_zop (AudioMelSpectrogram.swift:459-481), two
- *                         frames per warp on packed FFMA2/FADD2: ~2x the throughput; carries the float32 noise floor of
+ *                         frames per warp in float32 arithmetic instead of FP64; carries the float32 noise floor of
  *                         any float32 FFT (measured max |delta log-mel| 6e-5 over BASELINE's hour of audio). */
 enum { FA_MEL_PRECISION_F64 = 0, FA_MEL_PRECISION_F32 = 1 };
 fa_status fa_mel_set_precision(fa_mel *mel, int32_t precision);
@@ -118,8 +118,8 @@ int32_t fa_mel_get_precision(const fa_mel *mel);
  * streams (default 24; 1 = no overlap).  Results do not depend on it. */
 fa_status fa_mel_set_pipeline_chunks(fa_mel *mel, int32_t chunks);
 /* When the caller's time-major output buffer is pinned host memory (fa_host_alloc / cudaHostAlloc), the kernel stores its rows
- * straight into it over PCIe instead of staging them in HBM and copying.  Default OFF: on B200 + PCIe 5 the SM-issued posted writes
- * measured slower than the copy engine (4.72 vs 4.53 ms per audio-hour, profiles/r02_mel.md); pageable buffers always take the copy. */
+ * straight into it over PCIe instead of staging them in HBM and copying.  Default OFF: the copy engine is the
+ * measured default; pageable buffers always take the copy. */
 fa_status fa_mel_set_zero_copy_output(fa_mel *mel, int32_t enabled);
 
 /* Host buffers in and out (the drop-in call).  On return *mel_length = valid frames, *num_frames = padded frames;

@@ -683,7 +683,7 @@ void oracle_build_chunk_assignments(const int32_t *chunk, const int32_t *speaker
 //   KMeansClustering.clusterWithCentroids / clusterWithCentroidsNInit   Diarizer/Offline/Clustering/KMeansClustering.swift:39-130
 //   SeededRNG (LCG)                                                     KMeansClustering.swift:212-223
 //   SpeakerCountConstraints.resolve / needsAdjustment / targetCount     SpeakerCountConstraints.swift:27-85
-// Third-party semantics this depends on and that are NOT in /root/reference: the Swift standard library's
+// Third-party semantics this depends on and that are NOT in the reference repository: the Swift standard library's
 // `MutableCollection.shuffle(using:)`, `Collection.randomElement(using:)`, `Int.random(in:using:)` and
 // `RandomNumberGenerator.next(upperBound:)` (swift/stdlib/public/core/{CollectionAlgorithms,Random,Integers}.swift,
 // Swift 5.9+/6.x as required by the package's tools version).  Published algorithm, restated here:

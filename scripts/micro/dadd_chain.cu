@@ -1,6 +1,6 @@
 // Microbenchmark: latency of a dependent FP64 add chain on one SM, alone and with the scan's two independent FP64
 // operations per step (d = x - v, p = d * d), at 1 / 2 / 4 warps per SM sub-partition.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dadd_chain dadd_chain.cu && ./dadd_chain
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dadd_chain dadd_chain.cu && ./dadd_chain
 #include <cstdio>
 #include <cuda_runtime.h>
 constexpr int kSteps = 4096;

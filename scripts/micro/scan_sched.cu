@@ -1,7 +1,7 @@
 // Microbenchmark of the AHC scan step's instruction schedule: 128 threads of one CTA, each a sequential chain
 // sum = sum + (x_k - v_k)^2 over D = 256 with x in a k-major shared-memory tile (stride SP) and v broadcast — the loop
 // of ahc_merge_kernel — in several source forms.  Reports cycles per element (clock64, one SM).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scan_sched scan_sched.cu && ./scan_sched
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scan_sched scan_sched.cu && ./scan_sched
 #include <cstdio>
 #include <cuda_runtime.h>
 constexpr int D = 256, SP = 112, kReps = 16;

@@ -1,6 +1,6 @@
 // Drop-in for the conversion core of Sources/FluidAudio/Shared/AudioConverter.swift (same public surface for the
 // array / buffer entry points: resample(_:from:) :60-71, resampleBuffer(_:) :77-85).  Mixdown, int16 widening and the
-// sample-rate conversion run on an sm_100a GPU behind fa_audio_resample; file decoding (AVAudioFile, :91-130) and
+// sample-rate conversion run on an sm_90a GPU behind fa_audio_resample; file decoding (AVAudioFile, :91-130) and
 // CMSampleBuffer handling (:134-297) stay where they are and hand their PCM to `resampleBuffer`.
 // One or two channels: the library's documented Kaiser-windowed-sinc filter replaces Apple's closed AVAudioConverter
 // ("parity unpinned" for sample values; the output length follows Int(n / ratio), inside the reference tests' 1 %).

@@ -1,6 +1,6 @@
 // Drop-in for Sources/FluidAudio/Shared/AudioMelSpectrogram.swift (same public surface: init :59-70,
 // compute :132, computeFlat :185, computeFlatTransposed :299/:325, getFilterbank/getHannWindow :486-493, nFFT).
-// All arithmetic happens in libfluidaudio_b200.so on an sm_100a GPU; this file only marshals buffers.
+// All arithmetic happens in libfluidaudio_b200.so on an sm_90a GPU; this file only marshals buffers.
 // NOT compiled in this repository (no Swift toolchain in the build image) — see INTEGRATION.md.
 import CFluidAudioB200
 import Foundation

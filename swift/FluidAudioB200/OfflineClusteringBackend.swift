@@ -114,7 +114,7 @@ struct OfflineClusteringBackend {
 
 
 /// Reads the JSON that OfflineDiarizerManager.exportEmbeddings writes (OfflineDiarizerManager.swift:913-955) — the
-/// wire format between a Mac running the CoreML models and the B200 clustering backend.
+/// wire format between a Mac running the CoreML models and the GPU clustering backend.
 struct EmbeddingExportFile {
     var chunkIndex: [Int32] = [], speakerIndex: [Int32] = [], startFrame: [Int32] = [], endFrame: [Int32] = []
     var startTime: [Double] = [], endTime: [Double] = [], embedding256: [Float] = [], rho128: [Double] = []

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu on a machine that has one")
 
 
 @pytest.fixture(scope="session")
@@ -28,8 +28,8 @@ def golden_dir():
 
 @pytest.fixture(scope="session")
 def gpu_lib():
-    """The CUDA library on a box that has a B200; GPU tests fail (not skip) if it is unusable."""
+    """The CUDA library on a machine that has an H100; GPU tests fail (not skip) if it is unusable."""
     from fluidaudio_b200 import _lib
     L = _lib.load()
-    assert _lib.device_count() >= 1, "no sm_100a device visible: GPU tests must run on the B200 box"
+    assert _lib.device_count() >= 1, "no sm_90a device visible: GPU tests must run on a machine with an H100"
     return L

@@ -1,10 +1,13 @@
-"""Generates the committed golden fixtures.  Run HERE (the container that has /root/reference):
+"""Generates the committed golden fixtures.  Run where oracle/_ref/liboracle_fc.so could be built (the reference sources
+are present; see oracle/Makefile):
 
     python tests/golden/make_golden.py
 
 * ahc_*.npz   inputs + dendrograms produced by the UNMODIFIED reference FastClusterWrapper.cpp
               (oracle/_ref/liboracle_fc.so, built by `make -C oracle ref`) — these pin both the oracle
               restatement (CPU tests) and the CUDA path (GPU tests).
+* ahc_reference_fresh.npz  the reference's dendrograms of the seeded inputs test_oracle_golden.py regenerates (only the
+              outputs are stored; `python tests/golden/make_golden.py fresh` regenerates only these).
 * ahc_large.json  SHA-256 of the reference dendrogram bytes for the BASELINE-size problems (N = 5 000 / 10 000),
               whose inputs are regenerated from seeds (fluidaudio_b200/synth.py) instead of being stored.
 * next_rows.npz  the rows either side of the hot path (SURVEY 8f): seeded K-Means runs, UnifiedMelExtractor and LS-EEND
@@ -55,11 +58,29 @@ def next_rows():
     print("next_rows.npz written:", sorted(out))
 
 
+def fresh_inputs():
+    """Seeded inputs of test_restatement_equals_compiled_reference_on_fresh_inputs (the test regenerates them)."""
+    rng = np.random.default_rng(7)
+    cases = {f"random_{n}x{d}": rng.standard_normal((n, d)) for n, d in ((2, 3), (3, 1), (17, 4), (200, 16), (600, 256))}
+    cases["ties_150x6"] = np.repeat(rng.standard_normal((30, 6)), 5, axis=0)[rng.permutation(150)]
+    return cases
+
+
+def fresh():
+    out = {name + "__z": ref_linkage(x) for name, x in fresh_inputs().items()}
+    bad = np.array([[0.0, 1.0], [np.nan, 0.0], [1.0, 1.0]])
+    out["nan_row__status"] = np.array([O.centroid_linkage(bad, use_ref=True)[0]], np.int32)
+    np.savez_compressed(os.path.join(HERE, "ahc_reference_fresh.npz"), **out)
+    print("ahc_reference_fresh.npz written:", sorted(out))
+
+
 def main():
     O.build()
     if len(sys.argv) > 1 and sys.argv[1] == "next":
         return next_rows()
-    assert O.ref_available(), "oracle/_ref/liboracle_fc.so missing: run `make -C oracle ref` where /root/reference exists"
+    assert O.ref_available(), "oracle/_ref/liboracle_fc.so missing: run `make -C oracle ref` where the reference sources are"
+    if len(sys.argv) > 1 and sys.argv[1] == "fresh":
+        return fresh()
     rng = np.random.default_rng(2024)
     cases = {}
     # BASELINE config 1: 100 x 256, 4 speakers
@@ -113,6 +134,7 @@ def main():
     mel["filterbank_80"] = O.mel_filterbank(512, 80)
     np.savez_compressed(os.path.join(HERE, "mel_oracle.npz"), **mel)
     next_rows()
+    fresh()
     print("golden fixtures written to", HERE)
 
 

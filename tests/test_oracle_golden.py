@@ -29,17 +29,19 @@ def test_restatement_reproduces_reference_goldens_bit_exact(oracle, golden_dir):
         assert np.array_equal(z, z_ref), f"{name}: restatement differs from the reference dendrogram"
 
 
-def test_restatement_equals_compiled_reference_on_fresh_inputs(oracle):
-    if not oracle.ref_available():
-        pytest.skip("oracle/_ref not built on this box (needs /root/reference)")
+def test_restatement_equals_compiled_reference_on_fresh_inputs(oracle, golden_dir):
+    """Seeded inputs against the reference's dendrograms stored in ahc_reference_fresh.npz (make_golden.py fresh), and
+    against the compiled reference itself where oracle/_ref was built."""
+    g = np.load(os.path.join(golden_dir, "ahc_reference_fresh.npz"))
     rng = np.random.default_rng(7)
-    for n, d in ((2, 3), (3, 1), (17, 4), (200, 16), (600, 256)):
-        x = rng.standard_normal((n, d))
+    cases = {f"random_{n}x{d}": rng.standard_normal((n, d)) for n, d in ((2, 3), (3, 1), (17, 4), (200, 16), (600, 256))}
+    cases["ties_150x6"] = np.repeat(rng.standard_normal((30, 6)), 5, axis=0)[rng.permutation(150)]   # exact ties
+    for name, x in cases.items():
         st1, z1 = oracle.centroid_linkage(x)
-        st2, z2 = oracle.centroid_linkage(x, use_ref=True)
-        assert st1 == st2 == 0 and np.array_equal(z1, z2)
-    x = np.repeat(rng.standard_normal((30, 6)), 5, axis=0)[rng.permutation(150)]   # exact ties
-    assert np.array_equal(oracle.centroid_linkage(x)[1], oracle.centroid_linkage(x, use_ref=True)[1])
+        assert st1 == 0 and np.array_equal(z1, g[name + "__z"]), f"{name}: restatement differs from the reference"
+        if oracle.ref_available():
+            st2, z2 = oracle.centroid_linkage(x, use_ref=True)
+            assert st2 == 0 and np.array_equal(z1, z2)
 
 
 def test_large_reference_hashes_match_restatement(oracle, golden_dir):
@@ -55,7 +57,7 @@ def test_large_reference_hashes_match_restatement(oracle, golden_dir):
     assert labels.max() + 1 == m["clusters"]
 
 
-def test_status_codes_match_reference_contract(oracle):
+def test_status_codes_match_reference_contract(oracle, golden_dir):
     import ctypes as C
     L = oracle.lib()
     x = np.ones((3, 2))
@@ -68,6 +70,7 @@ def test_status_codes_match_reference_contract(oracle):
     assert L.oracle_centroid_linkage(x.ctypes.data, 2 ** 31, 2, z.ctypes.data, 8) == 2
     bad = np.array([[0.0, 1.0], [np.nan, 0.0], [1.0, 1.0]])
     assert oracle.centroid_linkage(bad)[0] == 5
+    assert int(np.load(os.path.join(golden_dir, "ahc_reference_fresh.npz"))["nan_row__status"][0]) == 5
     if oracle.ref_available():
         assert oracle.centroid_linkage(bad, use_ref=True)[0] == 5
 
