@@ -36,15 +36,6 @@
 namespace fa {
 namespace ahc {
 
-#define FA_CUDA_TRY(expr)                                                                               \
-    do {                                                                                                \
-        cudaError_t e__ = (expr);                                                                       \
-        if (e__ != cudaSuccess) {                                                                       \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            return e__ == cudaErrorMemoryAllocation ? FA_ALLOCATION_FAILURE : FA_CUDA_ERROR;            \
-        }                                                                                               \
-    } while (0)
-
 // ------------------------------------------------------------------------------------------------ sync helpers
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) {
     unsigned v;
@@ -1189,7 +1180,7 @@ void Solver::release() {
     d_pool = nullptr;
     d_input = nullptr;
     h_pool = nullptr;
-    pool_bytes = h_pool_bytes = input_cap = 0;
+    pool_bytes = h_pool_bytes = input_bytes = 0;
 }
 
 int Solver::init(cudaStream_t s, int worker_limit) {
@@ -1197,11 +1188,8 @@ int Solver::init(cudaStream_t s, int worker_limit) {
     int dev = 0;
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
-    FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 9) {
-        fa::set_error("fluidaudio_b200 requires an sm_90a device, found sm_%d%d", prop.major, prop.minor);
-        return FA_NO_DEVICE;
-    }
+    const int st = sm90_device_props(dev, prop);
+    if (st != FA_OK) return st;
     int coop = 0;
     FA_CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
     if (!coop) {
@@ -1214,15 +1202,6 @@ int Solver::init(cudaStream_t s, int worker_limit) {
 }
 
 namespace {
-struct Carver {
-    size_t off = 0;
-    template <typename T> size_t take(size_t count) {
-        off = (off + 255) & ~size_t(255);
-        const size_t at = off;
-        off += count * sizeof(T);
-        return at;
-    }
-};
 struct Layout {
     size_t rows, cols, node_weight, key, nn, heap_at, heap_where, node_of, slot_of, live_bits, merge_a, merge_b, merge_d,
         cmd, threshold, results, error, trace, init_partial, problem, total;
@@ -1233,42 +1212,42 @@ struct Layout {
 Layout make_layout(int N, int D, int Ns, int workers) {
     Layout L{};
     Carver c;
-    L.rows = c.take<double>((size_t)(2 * N - 1) * D);
-    L.cols = c.take<double>((size_t)D * Ns);
-    L.node_weight = c.take<int>((size_t)2 * N);
-    L.key = c.take<double>((size_t)N + 2);
-    L.nn = c.take<int>((size_t)N + 2);
-    L.heap_at = c.take<int>((size_t)N + 2);
-    L.heap_where = c.take<int>((size_t)N + 2);
-    L.node_of = c.take<int>((size_t)N + 2);
-    L.slot_of = c.take<int>((size_t)2 * N);
-    L.live_bits = c.take<unsigned>((size_t)(2 * N + 31) / 32 + 2);
-    L.merge_a = c.take<int>((size_t)N);
-    L.merge_b = c.take<int>((size_t)N);
-    L.merge_d = c.take<double>((size_t)N);
-    L.cmd = c.take<unsigned long long>(32);         // own 256-byte line
-    L.threshold = c.take<unsigned long long>(32);   // own 256-byte line
-    L.results = c.take<ResultSlot>(2 * 8 * ((size_t)workers + 1));
-    L.error = c.take<int>(64);
-    L.trace = c.take<unsigned long long>((size_t)kTraceSteps * 16);
+    L.rows = c.at<double>((size_t)(2 * N - 1) * D);
+    L.cols = c.at<double>((size_t)D * Ns);
+    L.node_weight = c.at<int>((size_t)2 * N);
+    L.key = c.at<double>((size_t)N + 2);
+    L.nn = c.at<int>((size_t)N + 2);
+    L.heap_at = c.at<int>((size_t)N + 2);
+    L.heap_where = c.at<int>((size_t)N + 2);
+    L.node_of = c.at<int>((size_t)N + 2);
+    L.slot_of = c.at<int>((size_t)2 * N);
+    L.live_bits = c.at<unsigned>((size_t)(2 * N + 31) / 32 + 2);
+    L.merge_a = c.at<int>((size_t)N);
+    L.merge_b = c.at<int>((size_t)N);
+    L.merge_d = c.at<double>((size_t)N);
+    L.cmd = c.at<unsigned long long>(32);         // own 256-byte line
+    L.threshold = c.at<unsigned long long>(32);   // own 256-byte line
+    L.results = c.at<ResultSlot>(2 * 8 * ((size_t)workers + 1));
+    L.error = c.at<int>(64);
+    L.trace = c.at<unsigned long long>((size_t)kTraceSteps * 16);
     L.ranges = (N + kJR - 1) / kJR;
-    L.init_partial = c.take<Cand>((size_t)L.ranges * N);
-    L.problem = c.take<Problem>(1);
+    L.init_partial = c.at<Cand>((size_t)L.ranges * N);
+    L.problem = c.at<Problem>(1);
     // float32 filter of the initial nearest-neighbour pass (N >= kFilterMinN only, but sized unconditionally: small)
     L.filter_cap = (int)std::min<long long>(64LL * N, 1 << 24);
-    L.f_cf = c.take<float>((size_t)((D + 7) & ~7) * Ns);   // rows rounded up to the GEMM's k-chunk (zero rows)
-    L.f_nrm2 = c.take<double>((size_t)N);
-    L.f_rn = c.take<float>((size_t)N);
-    L.f_U = c.take<unsigned long long>((size_t)N);
-    L.f_best_d = c.take<unsigned long long>((size_t)N);
-    L.f_best_j = c.take<int>((size_t)N);
-    L.f_cand = c.take<int2>((size_t)L.filter_cap);
-    L.f_cand_d = c.take<double>((size_t)L.filter_cap);
-    L.f_counters = c.take<int>(64);
+    L.f_cf = c.at<float>((size_t)((D + 7) & ~7) * Ns);   // rows rounded up to the GEMM's k-chunk (zero rows)
+    L.f_nrm2 = c.at<double>((size_t)N);
+    L.f_rn = c.at<float>((size_t)N);
+    L.f_U = c.at<unsigned long long>((size_t)N);
+    L.f_best_d = c.at<unsigned long long>((size_t)N);
+    L.f_best_j = c.at<int>((size_t)N);
+    L.f_cand = c.at<int2>((size_t)L.filter_cap);
+    L.f_cand_d = c.at<double>((size_t)L.filter_cap);
+    L.f_counters = c.at<int>(64);
     {
         const long long nt = (N + 63) / 64;
         L.f_keep_tmin = (long long)N * nt <= (16LL << 20);   // <= 64 MB
-        L.f_tmin = c.take<float>(L.f_keep_tmin ? (size_t)((long long)N * nt) : 1);
+        L.f_tmin = c.at<float>(L.f_keep_tmin ? (size_t)((long long)N * nt) : 1);
     }
     L.total = (c.off + 255) & ~size_t(255);
     return L;
@@ -1298,22 +1277,10 @@ int resident_workers_needed(int N, int D) {
 int Solver::ensure_pool(int N, int D) {
     const int Ns = (N + 31) & ~31;
     const Layout L = make_layout(N, D, Ns, max_workers);
-    if (L.total > pool_bytes) {
-        if (d_pool) cudaFree(d_pool);
-        d_pool = nullptr;
-        pool_bytes = 0;
-        FA_CUDA_TRY(cudaMalloc(&d_pool, L.total));
-        pool_bytes = L.total;
-    }
+    const int st = grow_buffer(d_pool, pool_bytes, L.total);
+    if (st != FA_OK) return st;
     const size_t hneed = sizeof(double) * (size_t)(2 * N + 16) + sizeof(int) * (size_t)(4 * N + 64);
-    if (hneed > h_pool_bytes) {
-        if (h_pool) cudaFreeHost(h_pool);
-        h_pool = nullptr;
-        h_pool_bytes = 0;
-        FA_CUDA_TRY(cudaMallocHost(&h_pool, hneed));
-        h_pool_bytes = hneed;
-    }
-    return FA_OK;
+    return grow_buffer(h_pool, h_pool_bytes, hneed, true);
 }
 
 // FA_AHC_* environment hooks (test / tuning only: fall-back placements at small N, trace, candidate spacing), read once.
@@ -1610,13 +1577,8 @@ int Solver::linkage_host(const double *rows_host, size_t N, size_t D, double *Z,
     if (z_len < (N > 1 ? (N - 1) * 4 : 0)) return FA_OUTPUT_TOO_SMALL;
     if (N == 1) return FA_OK;
     const size_t count = N * D;
-    if (count > input_cap) {
-        if (d_input) cudaFree(d_input);
-        d_input = nullptr;
-        input_cap = 0;
-        FA_CUDA_TRY(cudaMalloc(&d_input, count * sizeof(double)));
-        input_cap = count;
-    }
+    const int st = grow_buffer(d_input, input_bytes, count * sizeof(double));
+    if (st != FA_OK) return st;
     FA_CUDA_TRY(cudaMemcpyAsync(d_input, rows_host, count * sizeof(double), cudaMemcpyHostToDevice, stream));
     return linkage_device(d_input, (int)N, (int)D, Z);
 }

@@ -68,7 +68,7 @@ struct Solver {
     size_t pool_bytes = 0;
     Problem *d_problem = nullptr;
     double *d_input = nullptr;   // staging of the caller's [N x D] rows when they come from the host
-    size_t input_cap = 0;
+    size_t input_bytes = 0;
     // pinned host mirrors
     void *h_pool = nullptr;
     size_t h_pool_bytes = 0;

@@ -39,15 +39,6 @@ const char *last_error() { return g_error; }
 
 static std::atomic<long long> g_launches{0};
 
-#define FA_CUDA_TRY(expr)                                                                               \
-    do {                                                                                                \
-        cudaError_t e__ = (expr);                                                                       \
-        if (e__ != cudaSuccess) {                                                                       \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            return e__ == cudaErrorMemoryAllocation ? FA_ALLOCATION_FAILURE : FA_CUDA_ERROR;            \
-        }                                                                                               \
-    } while (0)
-
 static int usable_device_count() {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) {
@@ -57,7 +48,7 @@ static int usable_device_count() {
     int ok = 0;
     for (int i = 0; i < n; ++i) {
         cudaDeviceProp p;
-        if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 9) ++ok;
+        if (sm90_device_props(i, p) == FA_OK) ++ok;
     }
     return ok;
 }
@@ -110,21 +101,8 @@ struct ClusterContext {
         if (stream) cudaStreamDestroy(stream);
     }
     int reserve(size_t dbytes, size_t hbytes) {
-        if (dbytes > d_bytes) {
-            if (d_buf) cudaFree(d_buf);
-            d_buf = nullptr;
-            d_bytes = 0;
-            FA_CUDA_TRY(cudaMalloc(&d_buf, dbytes));
-            d_bytes = dbytes;
-        }
-        if (hbytes > h_bytes) {
-            if (h_buf) cudaFreeHost(h_buf);
-            h_buf = nullptr;
-            h_bytes = 0;
-            FA_CUDA_TRY(cudaMallocHost(&h_buf, hbytes));
-            h_bytes = hbytes;
-        }
-        return FA_OK;
+        const int st = grow_buffer(d_buf, d_bytes, dbytes);
+        return st != FA_OK ? st : grow_buffer(h_buf, h_bytes, hbytes, true);
     }
 };
 
@@ -160,17 +138,6 @@ struct Lease {
             std::lock_guard<std::mutex> lock(g_pool_mutex);
             g_pool.push_back(std::move(ctx));
         }
-    }
-};
-
-struct Carver {
-    char *base;
-    size_t off = 0;
-    template <typename T> T *take(size_t count) {
-        off = (off + 255) & ~size_t(255);
-        T *p = reinterpret_cast<T *>(base + off);
-        off += count * sizeof(T);
-        return p;
     }
 };
 
@@ -483,14 +450,8 @@ FA_API const char *fa_version(void) { return "fluidaudio_b200 0.1.0 (sm_90a)"; }
 FA_API const char *fa_last_error(void) { return fa::last_error(); }
 FA_API int32_t fa_device_count(void) { return usable_device_count(); }
 
-#define API_CUDA_TRY(expr)                                                                              \
-    do {                                                                                                \
-        cudaError_t e__ = (expr);                                                                       \
-        if (e__ != cudaSuccess) {                                                                       \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            return e__ == cudaErrorMemoryAllocation ? FA_STATUS_ALLOCATION_FAILURE : FA_STATUS_CUDA_ERROR; \
-        }                                                                                               \
-    } while (0)
+static_assert(FA_STATUS_ALLOCATION_FAILURE == FA_ALLOCATION_FAILURE && FA_STATUS_CUDA_ERROR == FA_CUDA_ERROR,
+              "FA_CUDA_TRY's status is returned as fa_status by value");
 #define API_REQUIRE_DEVICE()                                       \
     do {                                                           \
         if (require_device() != FA_OK) return FA_STATUS_NO_DEVICE; \
@@ -498,13 +459,13 @@ FA_API int32_t fa_device_count(void) { return usable_device_count(); }
 
 FA_API fa_status fa_set_device(int32_t ordinal) {
     API_REQUIRE_DEVICE();
-    API_CUDA_TRY(cudaSetDevice(ordinal));
+    FA_CUDA_TRY(cudaSetDevice(ordinal));
     return FA_STATUS_OK;
 }
 
 FA_API fa_status fa_device_synchronize(void) {
     API_REQUIRE_DEVICE();
-    API_CUDA_TRY(cudaDeviceSynchronize());
+    FA_CUDA_TRY(cudaDeviceSynchronize());
     return FA_STATUS_OK;
 }
 
@@ -513,31 +474,31 @@ FA_API int64_t fa_kernel_launch_count(void) { return g_launches.load(); }
 FA_API fa_status fa_host_alloc(size_t bytes, void **out) {
     if (!out) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
-    API_CUDA_TRY(cudaMallocHost(out, bytes ? bytes : 1));
+    FA_CUDA_TRY(cudaMallocHost(out, bytes ? bytes : 1));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_host_free(void *p) {
-    if (p) API_CUDA_TRY(cudaFreeHost(p));
+    if (p) FA_CUDA_TRY(cudaFreeHost(p));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_device_alloc(size_t bytes, void **out) {
     if (!out) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
-    API_CUDA_TRY(cudaMalloc(out, bytes ? bytes : 1));
+    FA_CUDA_TRY(cudaMalloc(out, bytes ? bytes : 1));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_device_free(void *p) {
-    if (p) API_CUDA_TRY(cudaFree(p));
+    if (p) FA_CUDA_TRY(cudaFree(p));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_memcpy_h2d(void *dst, const void *src, size_t bytes) {
     API_REQUIRE_DEVICE();
-    API_CUDA_TRY(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+    FA_CUDA_TRY(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_memcpy_d2h(void *dst, const void *src, size_t bytes) {
     API_REQUIRE_DEVICE();
-    API_CUDA_TRY(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+    FA_CUDA_TRY(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
     return FA_STATUS_OK;
 }
 
@@ -558,17 +519,17 @@ FA_API fa_status fa_memcpy_probe(const void *host_src, size_t h2d_bytes, void *h
                 if (x) cudaStreamDestroy(x);
         }
     } r;
-    API_CUDA_TRY(cudaMalloc(&r.a, h2d_bytes + 16));
-    API_CUDA_TRY(cudaMalloc(&r.b, d2h_bytes + 16));
-    API_CUDA_TRY(cudaMemset(r.b, 0, d2h_bytes + 16));
-    for (auto &x : r.s) API_CUDA_TRY(cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking));
-    API_CUDA_TRY(cudaDeviceSynchronize());
+    FA_CUDA_TRY(cudaMalloc(&r.a, h2d_bytes + 16));
+    FA_CUDA_TRY(cudaMalloc(&r.b, d2h_bytes + 16));
+    FA_CUDA_TRY(cudaMemset(r.b, 0, d2h_bytes + 16));
+    for (auto &x : r.s) FA_CUDA_TRY(cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking));
+    FA_CUDA_TRY(cudaDeviceSynchronize());
     const auto t0 = std::chrono::steady_clock::now();
     for (int i = 0; i < reps; ++i) {
-        if (h2d_bytes) API_CUDA_TRY(cudaMemcpyAsync(r.a, host_src, h2d_bytes, cudaMemcpyHostToDevice, r.s[0]));
-        if (d2h_bytes) API_CUDA_TRY(cudaMemcpyAsync(host_dst, r.b, d2h_bytes, cudaMemcpyDeviceToHost, r.s[1]));
-        API_CUDA_TRY(cudaStreamSynchronize(r.s[0]));
-        API_CUDA_TRY(cudaStreamSynchronize(r.s[1]));
+        if (h2d_bytes) FA_CUDA_TRY(cudaMemcpyAsync(r.a, host_src, h2d_bytes, cudaMemcpyHostToDevice, r.s[0]));
+        if (d2h_bytes) FA_CUDA_TRY(cudaMemcpyAsync(host_dst, r.b, d2h_bytes, cudaMemcpyDeviceToHost, r.s[1]));
+        FA_CUDA_TRY(cudaStreamSynchronize(r.s[0]));
+        FA_CUDA_TRY(cudaStreamSynchronize(r.s[1]));
     }
     const auto t1 = std::chrono::steady_clock::now();
     *ms_per_round = (float)(std::chrono::duration<double, std::milli>(t1 - t0).count() / reps);
@@ -581,19 +542,19 @@ FA_API fa_status fa_memcpy_probe(const void *host_src, size_t h2d_bytes, void *h
 FA_API fa_status fa_timer_start(void) {
     API_REQUIRE_DEVICE();
     if (!t_ev0) {
-        API_CUDA_TRY(cudaEventCreate(&t_ev0));
-        API_CUDA_TRY(cudaEventCreate(&t_ev1));
+        FA_CUDA_TRY(cudaEventCreate(&t_ev0));
+        FA_CUDA_TRY(cudaEventCreate(&t_ev1));
     }
-    API_CUDA_TRY(cudaDeviceSynchronize());
-    API_CUDA_TRY(cudaEventRecord(t_ev0, 0));
+    FA_CUDA_TRY(cudaDeviceSynchronize());
+    FA_CUDA_TRY(cudaEventRecord(t_ev0, 0));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_timer_stop_ms(float *elapsed_ms) {
     if (!elapsed_ms || !t_ev0) return FA_STATUS_INVALID_ARGUMENT;
-    API_CUDA_TRY(cudaDeviceSynchronize());
-    API_CUDA_TRY(cudaEventRecord(t_ev1, 0));
-    API_CUDA_TRY(cudaEventSynchronize(t_ev1));
-    API_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, t_ev0, t_ev1));
+    FA_CUDA_TRY(cudaDeviceSynchronize());
+    FA_CUDA_TRY(cudaEventRecord(t_ev1, 0));
+    FA_CUDA_TRY(cudaEventSynchronize(t_ev1));
+    FA_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, t_ev0, t_ev1));
     return FA_STATUS_OK;
 }
 
@@ -620,7 +581,7 @@ FA_API fa_status fa_mel_create(const fa_mel_config *cfg, fa_mel **out) {
     std::unique_ptr<MelHandle> h(new MelHandle());
     mel::MelConfig c{cfg->sample_rate, cfg->n_mels, cfg->n_fft, cfg->hop_length, cfg->win_length, cfg->preemph,
                      cfg->pad_to, cfg->log_floor, cfg->log_floor_mode, cfg->window_periodic};
-    API_CUDA_TRY(cudaGetDevice(&h->device));
+    FA_CUDA_TRY(cudaGetDevice(&h->device));
     const int st = h->plan.init(c);
     if (st != FA_OK) return (fa_status)st;
     *out = reinterpret_cast<fa_mel *>(h.release());
@@ -688,7 +649,10 @@ FA_API fa_status fa_mel_compute(fa_mel *mel, const float *audio, size_t n, float
     auto *h = reinterpret_cast<MelHandle *>(mel);
     long long ml = 0, nf = 0;
     const long long before = h->plan.launches;
-    const int st = h->plan.compute_host(audio, (long long)n, last, mode, expected, layout, out, (long long)out_len, &ml, &nf);
+    const double rate = h->plan.cfg.sample_rate;
+    const resample::AudioFormat mono_f32{rate, rate, 1, resample::kPcmF32, 1, resample::kAlgoAuto};
+    const int st = h->plan.compute_host(audio, (long long)n, mono_f32, last, mode, expected, layout, out,
+                                        (long long)out_len, &ml, &nf, nullptr);
     g_launches += h->plan.launches - before;
     if (mel_length) *mel_length = ml;
     if (num_frames) *num_frames = nf;
@@ -753,20 +717,20 @@ FA_API fa_status fa_mel_timer_start(fa_mel *mel) {
     if (!mel) return FA_STATUS_INVALID_ARGUMENT;
     auto *h = reinterpret_cast<MelHandle *>(mel);
     if (!h->plan.timer[0]) {
-        API_CUDA_TRY(cudaEventCreate(&h->plan.timer[0]));
-        API_CUDA_TRY(cudaEventCreate(&h->plan.timer[1]));
+        FA_CUDA_TRY(cudaEventCreate(&h->plan.timer[0]));
+        FA_CUDA_TRY(cudaEventCreate(&h->plan.timer[1]));
     }
-    API_CUDA_TRY(cudaStreamSynchronize(h->plan.streams[1]));
-    API_CUDA_TRY(cudaEventRecord(h->plan.timer[0], h->plan.streams[1]));
+    FA_CUDA_TRY(cudaStreamSynchronize(h->plan.streams[1]));
+    FA_CUDA_TRY(cudaEventRecord(h->plan.timer[0], h->plan.streams[1]));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_mel_timer_stop_ms(fa_mel *mel, float *elapsed_ms) {
     if (!mel || !elapsed_ms) return FA_STATUS_INVALID_ARGUMENT;
     auto *h = reinterpret_cast<MelHandle *>(mel);
     if (!h->plan.timer[0]) return FA_STATUS_INVALID_ARGUMENT;
-    API_CUDA_TRY(cudaEventRecord(h->plan.timer[1], h->plan.streams[1]));
-    API_CUDA_TRY(cudaEventSynchronize(h->plan.timer[1]));
-    API_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, h->plan.timer[0], h->plan.timer[1]));
+    FA_CUDA_TRY(cudaEventRecord(h->plan.timer[1], h->plan.streams[1]));
+    FA_CUDA_TRY(cudaEventSynchronize(h->plan.timer[1]));
+    FA_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, h->plan.timer[0], h->plan.timer[1]));
     return FA_STATUS_OK;
 }
 
@@ -875,20 +839,20 @@ FA_API fa_status fa_audio_resample(const void *pcm, int64_t frames, const fa_aud
             if (s) cudaStreamDestroy(s);
         }
     } b;
-    API_CUDA_TRY(cudaStreamCreateWithFlags(&b.s, cudaStreamNonBlocking));
-    API_CUDA_TRY(cudaMalloc(&b.pcm, bytes + 16));
-    API_CUDA_TRY(cudaMalloc(&b.out, (size_t)n * sizeof(float)));
+    FA_CUDA_TRY(cudaStreamCreateWithFlags(&b.s, cudaStreamNonBlocking));
+    FA_CUDA_TRY(cudaMalloc(&b.pcm, bytes + 16));
+    FA_CUDA_TRY(cudaMalloc(&b.out, (size_t)n * sizeof(float)));
     if (!d.table.empty()) {
-        API_CUDA_TRY(cudaMalloc(&b.tab, d.table.size() * sizeof(float)));
-        API_CUDA_TRY(cudaMemcpyAsync(b.tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice, b.s));
+        FA_CUDA_TRY(cudaMalloc(&b.tab, d.table.size() * sizeof(float)));
+        FA_CUDA_TRY(cudaMemcpyAsync(b.tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice, b.s));
     }
-    API_CUDA_TRY(cudaMemcpyAsync(b.pcm, pcm, bytes, cudaMemcpyHostToDevice, b.s));
+    FA_CUDA_TRY(cudaMemcpyAsync(b.pcm, pcm, bytes, cudaMemcpyHostToDevice, b.s));
     long long launches = 0;
     const int st = resample::launch_convert(b.pcm, frames, f, d, b.tab, b.out, 0, n, b.s, &launches);
     g_launches += launches;
     if (st != FA_OK) return (fa_status)st;
-    API_CUDA_TRY(cudaMemcpyAsync(out, b.out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, b.s));
-    API_CUDA_TRY(cudaStreamSynchronize(b.s));
+    FA_CUDA_TRY(cudaMemcpyAsync(out, b.out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, b.s));
+    FA_CUDA_TRY(cudaStreamSynchronize(b.s));
     return FA_STATUS_OK;
     FA_GUARD_END
 }
@@ -907,15 +871,8 @@ FA_API fa_status fa_audio_to_mel(fa_mel *mel, const void *pcm, int64_t frames, c
     }
     long long ml = 0, nf = 0, rs = 0;
     const long long before = h->plan.launches;
-    const resample::AudioFormat f = to_format(fmt);
-    int st;
-    if (resample::is_identity(f)) {   // mono float32 at the model rate: AudioConverter returns the samples as they are (:66-68)
-        rs = frames;
-        st = h->plan.compute_host(static_cast<const float *>(pcm), (long long)frames, last, mode, -1, layout, out,
-                                  (long long)out_len, &ml, &nf);
-    } else {
-        st = h->plan.compute_host_pcm(pcm, (long long)frames, f, last, mode, layout, out, (long long)out_len, &ml, &nf, &rs);
-    }
+    const int st = h->plan.compute_host(pcm, (long long)frames, to_format(fmt), last, mode, -1, layout, out,
+                                        (long long)out_len, &ml, &nf, &rs);
     g_launches += h->plan.launches - before;
     if (mel_length) *mel_length = ml;
     if (num_frames) *num_frames = nf;
@@ -1000,12 +957,12 @@ FA_API fa_status fa_l2_normalize_rows(const double *x, size_t rows, size_t dim, 
     if (st != FA_OK) return (fa_status)st;
     double *d_in = static_cast<double *>(C.d_buf);
     double *d_out = d_in + rows * dim;
-    API_CUDA_TRY(cudaMemcpyAsync(d_in, x, rows * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_in, x, rows * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     st = ahc::launch_normalize_rows(d_in, d_out, (int)rows, (int)dim, C.stream);
     if (st != FA_OK) return (fa_status)st;
     g_launches += 1;
-    API_CUDA_TRY(cudaMemcpyAsync(out, d_out, rows * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, rows * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     return FA_STATUS_OK;
     FA_GUARD_END
 }
@@ -1041,7 +998,7 @@ FA_API fa_status fa_ahc_cluster(const double *features, size_t count, size_t dim
     double *d_in = static_cast<double *>(C.d_buf);
     double *d_norm = d_in + count * dim;
     double *h_Z = static_cast<double *>(C.h_buf);
-    API_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     st = ahc::launch_normalize_rows(d_in, d_norm, (int)count, (int)dim, C.stream);
     if (st != FA_OK) return (fa_status)st;
     const long long before = C.solver.launches;
@@ -1169,16 +1126,16 @@ FA_API fa_status fa_kmeans_cluster(const double *emb, size_t N, size_t D, int32_
     double *d_emb = c.take<double>(N * D);
     double *d_cent = c.take<double>((size_t)rows_needed * D);
     int *d_labels = c.take<int>(N);
-    API_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     long long lc = 0;
     int rows = 0, best = 0;
     st = kmeans::cluster_ninit_device(C.vbx_ws, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
                                       d_labels, d_cent, &rows, &best, C.stream, &lc);
     g_launches += lc;
     if (st != FA_OK) return (fa_status)st;
-    API_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)rows * D * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)rows * D * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     if (centroid_rows) *centroid_rows = rows;
     if (best_init) *best_init = best;
     return FA_STATUS_OK;
@@ -1213,8 +1170,8 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
     int *d_hard = c.take<int>(T);
     std::vector<double> psi_eff(D, 1.0);
     if (psi && psi_len == D) std::memcpy(psi_eff.data(), psi, D * sizeof(double));
-    API_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    if (initial) API_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    if (initial) FA_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
     vbx::Config vc;
     vc.Fa = cfg->Fa;
     vc.Fb = cfg->Fb;
@@ -1227,11 +1184,11 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
                             d_pi, d_elbos, d_hard, &its, C.stream, &lc);
     g_launches += lc;
     if (st != FA_OK) return (fa_status)st;
-    API_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(pi, d_pi, S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(elbos, d_elbos, cap * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(hard, d_hard, T * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(pi, d_pi, S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(elbos, d_elbos, cap * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(hard, d_hard, T * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     if (iterations) *iterations = its;
     return FA_STATUS_OK;
     FA_GUARD_END
@@ -1262,20 +1219,20 @@ FA_API fa_status fa_compute_centroids(const double *emb, size_t T, size_t dim, c
     double *d_cent = c.take<double>((size_t)S * dim);
     double *d_cent_n = c.take<double>((size_t)S * dim);
     int *d_count = c.take<int>(64);
-    API_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     long long lc = 0;
     st = vbx::centroids_device(C.vbx_ws, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream, &lc);
     g_launches += lc;
     if (st != FA_OK) return (fa_status)st;
     int K = 0;
-    API_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     *centroid_count = K;
     if (K > 0) {
-        API_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)K * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        API_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)K * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     }
     return FA_STATUS_OK;
     FA_GUARD_END
@@ -1308,8 +1265,8 @@ FA_API fa_status fa_assign_embeddings(const double *emb, size_t N, size_t dim, c
     double *d_cn = c.take<double>((size_t)K * dim);
     int *d_labels = c.take<int>(N);
     double *d_scores = c.take<double>(scores ? N * (size_t)K : 1);
-    API_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    API_CUDA_TRY(cudaMemcpyAsync(d_craw, centroids, (size_t)K * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_craw, centroids, (size_t)K * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     // centroid normalisation (:793, :824-860; zero rows kept) with the same kernel the pipeline uses
     st = ahc::launch_normalize_rows_keep(d_craw, d_cn, K, (int)dim, C.stream);
     if (st != FA_OK) return (fa_status)st;
@@ -1318,9 +1275,9 @@ FA_API fa_status fa_assign_embeddings(const double *emb, size_t N, size_t dim, c
     st = vbx::assign_device(d_emb, (int)N, (int)dim, d_cn, nullptr, K, d_labels, scores ? d_scores : nullptr, C.stream, &lc);
     g_launches += lc;
     if (st != FA_OK) return (fa_status)st;
-    API_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    if (scores) API_CUDA_TRY(cudaMemcpyAsync(scores, d_scores, N * (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    API_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+    if (scores) FA_CUDA_TRY(cudaMemcpyAsync(scores, d_scores, N * (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     return FA_STATUS_OK;
     FA_GUARD_END
 }
@@ -1413,9 +1370,9 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
     int dev = 0;
-    API_CUDA_TRY(cudaGetDevice(&dev));
+    FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
-    API_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
+    FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
     // Concurrency: as many sets at a time as still leaves each of them enough SMs to keep its node vectors in shared
     // memory (the merge loop is ~3x slower when they are streamed from L2): 5 000 x 256 needs 46 workers + 1 master,
     // so two sets run side by side on an H100's 132 SMs; small sets run four at a time.

@@ -5,6 +5,7 @@
 #include <cstdint>
 
 #if defined(__CUDACC__)
+#include <cuda_runtime.h>
 #define FA_HD __host__ __device__ __forceinline__
 #else
 #define FA_HD inline
@@ -31,7 +32,61 @@ namespace fa {
 void set_error(const char *fmt, ...);
 const char *last_error();
 
+// Slices one allocation into 256-byte aligned arrays.  Carver{nullptr} is a dry run: `off` then holds the bytes the
+// arrays need, and at<T>() returns offsets for layouts computed before the allocation exists.
+struct Carver {
+    char *base = nullptr;
+    size_t off = 0;
+    template <typename T> size_t at(size_t count) {
+        off = (off + 255) & ~size_t(255);
+        const size_t p = off;
+        off += count * sizeof(T);
+        return p;
+    }
+    template <typename T> T *take(size_t count) { return reinterpret_cast<T *>(base + at<T>(count)); }
+};
+
 #if defined(__CUDACC__)
+// Status of a failed CUDA call: FA_ALLOCATION_FAILURE when memory ran out, FA_CUDA_ERROR otherwise.  It converts to
+// the int codes used inside the library and to fa_status at the C ABI (the same numbers).
+struct CudaStatus {
+    int code;
+    template <typename T> operator T() const { return static_cast<T>(code); }
+};
+inline CudaStatus cuda_failure(cudaError_t e, const char *expr, const char *file, int line) {
+    set_error("%s failed: %s (%s:%d)", expr, cudaGetErrorString(e), file, line);
+    return CudaStatus{e == cudaErrorMemoryAllocation ? FA_ALLOCATION_FAILURE : FA_CUDA_ERROR};
+}
+#define FA_CUDA_TRY(expr)                                                                 \
+    do {                                                                                  \
+        const cudaError_t e__ = (expr);                                                   \
+        if (e__ != cudaSuccess) return fa::cuda_failure(e__, #expr, __FILE__, __LINE__); \
+    } while (0)
+
+// Grow-only device (or pinned host) buffer: keeps `p` when it already holds `bytes`, otherwise replaces it.  It never
+// shrinks, and a failed allocation leaves `p` null and `cap` zero.
+template <typename T> int grow_buffer(T *&p, size_t &cap, size_t bytes, bool pinned = false) {
+    if (bytes <= cap) return FA_OK;
+    if (p) pinned ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    void *q = nullptr;
+    FA_CUDA_TRY(pinned ? cudaMallocHost(&q, bytes) : cudaMalloc(&q, bytes));
+    p = static_cast<T *>(q);
+    cap = bytes;
+    return FA_OK;
+}
+
+// Properties of device `dev`, which must be sm_90: the library carries sm_90a code only.
+inline int sm90_device_props(int dev, cudaDeviceProp &prop) {
+    FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
+    if (prop.major != 9) {
+        set_error("fluidaudio_b200 requires an sm_90a device, found sm_%d%d", prop.major, prop.minor);
+        return FA_NO_DEVICE;
+    }
+    return FA_OK;
+}
+
 // Float pairs (two frames, two columns) with every lane an independent round-to-nearest IEEE operation.  sm_90 has no
 // packed FP32 instructions: each is two FADD / FMUL / FFMA, and the __f*_rn intrinsics keep the compiler from fusing a
 // separate multiply and add, so results equal the scalar expressions bit for bit.

@@ -23,15 +23,6 @@
 namespace fa {
 namespace kmeans {
 
-#define FA_CUDA_TRY(expr)                                                                      \
-    do {                                                                                       \
-        cudaError_t e_ = (expr);                                                               \
-        if (e_ != cudaSuccess) {                                                               \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e_), __FILE__, __LINE__); \
-            return FA_CUDA_ERROR;                                                              \
-        }                                                                                      \
-    } while (0)
-
 struct Lcg {
     unsigned long long state;
     __host__ __device__ unsigned long long next() {
@@ -213,16 +204,6 @@ unsigned long long host_next_below(Lcg &g, unsigned long long upper) {
     }
     return (unsigned long long)(m >> 64);
 }
-struct Carver {
-    char *base;
-    size_t off = 0;
-    template <typename T> T *take(size_t count) {
-        off = (off + 255) & ~size_t(255);
-        T *p = reinterpret_cast<T *>(base + off);
-        off += sizeof(T) * count;
-        return p;
-    }
-};
 } // namespace
 
 void resolve_constraints(long long num_embeddings, long long num_speakers, long long min_speakers, long long max_speakers,

@@ -22,15 +22,6 @@
 namespace fa {
 namespace mel {
 
-#define FA_CUDA_TRY(expr)                                                                      \
-    do {                                                                                       \
-        cudaError_t e_ = (expr);                                                               \
-        if (e_ != cudaSuccess) {                                                               \
-            fa::set_error("CUDA error %s at %s:%d", cudaGetErrorString(e_), __FILE__, __LINE__); \
-            return FA_CUDA_ERROR;                                                              \
-        }                                                                                      \
-    } while (0)
-
 constexpr int kBinsPerCta = 128;
 constexpr int kTile = 32;
 

@@ -28,6 +28,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <vector>
 
 namespace fa {
@@ -456,15 +457,6 @@ void build_filterbank(int n_fft, int n_mels, int sample_rate, std::vector<float>
     }
 }
 
-#define FA_CUDA_TRY(expr)                                                                   \
-    do {                                                                                    \
-        cudaError_t e__ = (expr);                                                           \
-        if (e__ != cudaSuccess) {                                                           \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            return FA_CUDA_ERROR;                                                           \
-        }                                                                                   \
-    } while (0)
-
 static constexpr int kWarpsPerCta = 8;
 static constexpr int kCtasPerSm = 2;
 
@@ -492,12 +484,10 @@ void MelPlan::release() {
     fr(d_pcm);
     fr(d_rs_tab);
     fr(d_generic_tw);
-    d_pcm_cap = 0;
     rs_in = rs_out = 0.0;
-    d_audio_cap = d_out_cap = 0;
+    d_units_bytes = h_units_bytes = d_audio_bytes = d_out_bytes = d_pcm_bytes = rs_tab_bytes = 0;
     if (h_units) cudaFreeHost(h_units);
     h_units = nullptr;
-    units_cap = 0;
     for (auto &s : streams)
         if (s) cudaStreamDestroy(s), s = nullptr;
     for (auto &e : events)
@@ -593,12 +583,9 @@ int MelPlan::init(const MelConfig &c) {
     int dev = 0;
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
-    FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
+    const int st = sm90_device_props(dev, prop);
+    if (st != FA_OK) return st;
     num_sms = prop.multiProcessorCount;
-    if (prop.major != 9) {
-        fa::set_error("fluidaudio_b200 requires an sm_90a device, found sm_%d%d", prop.major, prop.minor);
-        return FA_NO_DEVICE;
-    }
 
     std::vector<float> win_tab(n_fft, 0.0f);
     std::vector<uint8_t> in_tab(n_fft, 0);
@@ -614,16 +601,7 @@ int MelPlan::init(const MelConfig &c) {
         FA_CUDA_TRY(cudaMalloc(&d_in_tab_mode[mode], n_fft));
         FA_CUDA_TRY(cudaMemcpy(d_win_tab_mode[mode], win_tab.data(), n_fft * sizeof(float), cudaMemcpyHostToDevice));
         FA_CUDA_TRY(cudaMemcpy(d_in_tab_mode[mode], in_tab.data(), n_fft, cudaMemcpyHostToDevice));
-    }
-    if (!generic) {
-        for (int mode = 0; mode < 2; ++mode) {
-            const int off_w = mode == 0 ? (cfg.n_fft - cfg.win_length) / 2 : 0;
-            std::fill(win_tab.begin(), win_tab.end(), 0.0f);
-            std::fill(in_tab.begin(), in_tab.end(), 0);
-            for (int j = 0; j < cfg.win_length; ++j) {
-                win_tab[off_w + j] = window[j];
-                in_tab[off_w + j] = 1;
-            }
+        if (!generic) {
             std::vector<LaneTables<double>> t64(32);
             std::vector<LaneTables<f32x2>> t32(32);
             for (int l = 0; l < 32; ++l) {
@@ -699,33 +677,14 @@ long long MelPlan::frame_count(long long n, int mode, long long expected) const 
 }
 
 int MelPlan::ensure_units(int count) {
-    if (count <= units_cap) return FA_OK;
-    if (d_units) cudaFree(d_units);
-    if (h_units) cudaFreeHost(h_units);
-    d_units = nullptr;
-    h_units = nullptr;
-    units_cap = std::max(count, 64);
-    FA_CUDA_TRY(cudaMalloc(&d_units, units_cap * sizeof(MelUnit)));
-    FA_CUDA_TRY(cudaMallocHost(&h_units, units_cap * sizeof(MelUnit)));
-    return FA_OK;
+    const size_t bytes = (size_t)std::max(count, 64) * sizeof(MelUnit);
+    const int st = grow_buffer(d_units, d_units_bytes, bytes);
+    return st != FA_OK ? st : grow_buffer(h_units, h_units_bytes, bytes, true);
 }
 
 int MelPlan::ensure_staging(size_t audio_floats, size_t out_floats) {
-    if (audio_floats > d_audio_cap) {
-        if (d_audio) cudaFree(d_audio);
-        d_audio = nullptr;
-        d_audio_cap = 0;
-        FA_CUDA_TRY(cudaMalloc(&d_audio, audio_floats * sizeof(float)));
-        d_audio_cap = audio_floats;
-    }
-    if (out_floats > d_out_cap) {
-        if (d_out) cudaFree(d_out);
-        d_out = nullptr;
-        d_out_cap = 0;
-        FA_CUDA_TRY(cudaMalloc(&d_out, out_floats * sizeof(float)));
-        d_out_cap = out_floats;
-    }
-    return FA_OK;
+    const int st = grow_buffer(d_audio, d_audio_bytes, audio_floats * sizeof(float));
+    return st != FA_OK ? st : grow_buffer(d_out, d_out_bytes, out_floats * sizeof(float));
 }
 
 int MelPlan::ensure_events(size_t count) {
@@ -812,26 +771,35 @@ static bool shape_of(const MelPlan &p, long long n, int mode, long long expected
     return true;
 }
 
+// Output shape of one clip, reported through mel_length / num_frames: T frames computed, Tp rows returned.  Empty input
+// gives T = 0 and one pad row (none in mode 2), which the caller zeroes.  Fails when out_len floats cannot hold Tp rows.
+static int clip_shape(const MelPlan &p, long long n, int mode, long long expected, long long out_len, long long &T,
+                      long long &Tp, long long *mel_length, long long *num_frames) {
+    if (!shape_of(p, n, mode, expected, T, Tp)) {
+        T = 0;
+        Tp = mode == 2 ? 0 : 1;
+    }
+    if (mel_length) *mel_length = T;
+    if (num_frames) *num_frames = Tp;
+    if (out_len < Tp * p.cfg.n_mels) {
+        fa::set_error("mel output needs %lld floats, buffer has %lld", Tp * p.cfg.n_mels, out_len);
+        return FA_OUTPUT_TOO_SMALL;
+    }
+    return FA_OK;
+}
+static constexpr long long kUnchecked = std::numeric_limits<long long>::max();   // batch calls take no output lengths
+
 int MelPlan::compute_device(const float *d_in, long long n, float last, int mode, long long expected, int layout,
                             float *d_out_buf, long long out_len, long long *mel_length, long long *num_frames,
                             cudaStream_t stream) {
     long long T, Tp;
-    if (!shape_of(*this, n, mode, expected, T, Tp)) {
-        if (mel_length) *mel_length = 0;
-        if (num_frames) *num_frames = mode == 2 ? 0 : 1;
-        if (mode != 2) {
-            if (out_len < cfg.n_mels) return FA_OUTPUT_TOO_SMALL;
-            FA_CUDA_TRY(cudaMemsetAsync(d_out_buf, 0, cfg.n_mels * sizeof(float), stream));
-        }
+    int st = clip_shape(*this, n, mode, expected, out_len, T, Tp, mel_length, num_frames);
+    if (st != FA_OK) return st;
+    if (T == 0) {
+        if (Tp) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf, 0, cfg.n_mels * sizeof(float), stream));
         return FA_OK;
     }
-    if (mel_length) *mel_length = T;
-    if (num_frames) *num_frames = Tp;
-    if (out_len < Tp * cfg.n_mels) {
-        fa::set_error("mel output needs %lld floats, buffer has %lld", Tp * cfg.n_mels, out_len);
-        return FA_OUTPUT_TOO_SMALL;
-    }
-    int st = ensure_units(1);
+    st = ensure_units(1);
     if (st != FA_OK) return st;
     if (Tp > T) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf, 0, Tp * cfg.n_mels * sizeof(float), stream));
     h_units[0] = MelUnit{0, n, 0, Tp, 0, T, last, 0};
@@ -850,14 +818,12 @@ int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, i
     for (int i = 0; i < count; ++i) {
         const long long n = offsets[i + 1] - offsets[i];
         long long T, Tp;
-        if (!shape_of(*this, n, mode, -1, T, Tp)) {
-            if (mel_lengths) mel_lengths[i] = 0;
-            if (num_frames) num_frames[i] = mode == 2 ? 0 : 1;
-            if (mode != 2) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf + out_offsets[i], 0, cfg.n_mels * sizeof(float), stream));
+        clip_shape(*this, n, mode, -1, kUnchecked, T, Tp, mel_lengths ? mel_lengths + i : nullptr,
+                   num_frames ? num_frames + i : nullptr);
+        if (T == 0) {
+            if (Tp) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf + out_offsets[i], 0, cfg.n_mels * sizeof(float), stream));
             continue;
         }
-        if (mel_lengths) mel_lengths[i] = T;
-        if (num_frames) num_frames[i] = Tp;
         if (Tp > T) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf + out_offsets[i], 0, Tp * cfg.n_mels * sizeof(float), stream));
         if (offsets[i] & 3) aligned = false;
         h_units[used] = MelUnit{offsets[i], n, out_offsets[i], Tp, 0, T, last ? last[i] : 0.0f, tiles};
@@ -881,10 +847,8 @@ static float *device_alias_if_pinned(float *host) {
     return (a.type == cudaMemoryTypeHost && a.devicePointer) ? static_cast<float *>(a.devicePointer) : nullptr;
 }
 
-// Host buffers in, host buffers out.  A long clip is cut into units of `chunk` frames: unit c's samples are copied
-// on the H2D stream while unit c-1 runs on the compute stream and unit c-2's rows return on the D2H stream.
-// FA_MEL_TRACE_PIPELINE=1: device timestamps (timing events) at the end of every unit's H2D, kernels and D2H, printed to
-// stderr after the call — the tool behind profiles/r02_mel.md's pipeline timeline.  Off: no events, no cost.
+// FA_MEL_TRACE_PIPELINE=1: device timestamps (timing events) at the end of every unit's H2D, kernels and D2H of the
+// host-buffer pipeline (MelPlan::compute_host), printed to stderr after the call.  Off: no events, no cost.
 struct PipelineTrace {
     bool on = false;
     cudaEvent_t t0 = nullptr;
@@ -950,96 +914,14 @@ static std::vector<long long> unit_bounds(long long T, long long max_units, long
     return b;
 }
 
-int MelPlan::compute_host(const float *audio, long long n, float last, int mode, long long expected, int layout,
-                          float *out, long long out_len, long long *mel_length, long long *num_frames) {
-    long long T, Tp;
-    if (!shape_of(*this, n, mode, expected, T, Tp)) {
-        if (mel_length) *mel_length = 0;
-        if (num_frames) *num_frames = mode == 2 ? 0 : 1;
-        if (mode != 2) {
-            if (out_len < cfg.n_mels) return FA_OUTPUT_TOO_SMALL;
-            for (int m = 0; m < cfg.n_mels; ++m) out[m] = 0.0f;   // padValue
-        }
-        return FA_OK;
-    }
-    if (mel_length) *mel_length = T;
-    if (num_frames) *num_frames = Tp;
-    const long long need = Tp * cfg.n_mels;
-    if (out_len < need) {
-        fa::set_error("mel output needs %lld floats, buffer has %lld", need, out_len);
-        return FA_OUTPUT_TOO_SMALL;
-    }
-    int st = ensure_staging((size_t)n + 8, (size_t)need);
-    if (st != FA_OK) return st;
-    const std::vector<long long> bounds = unit_bounds(T, pipeline_chunks, 4096);
-    const int chunks = (int)bounds.size() - 1;
-    float *out_alias = (zero_copy_out && layout == 0 && chunks > 1) ? device_alias_if_pinned(out) : nullptr;
-    float *k_out = out_alias ? out_alias : d_out;   // where the kernel writes
-    if (out_alias && Tp > T) std::memset(out + T * cfg.n_mels, 0, (size_t)(Tp - T) * cfg.n_mels * sizeof(float));
-    st = ensure_units(chunks);
-    if (st != FA_OK) return st;
-    cudaStream_t s_in = streams[0], s_k = streams[1], s_out = streams[2];
-    if (chunks == 1) {
-        // the streaming callers' shape (a few thousand samples, SortformerDiarizer.swift:857-905): nothing to overlap, so
-        // one stream, no events, the unit descriptor passed in the kernel parameters, one synchronisation
-        FA_CUDA_TRY(cudaMemcpyAsync(d_audio, audio, n * sizeof(float), cudaMemcpyHostToDevice, s_k));
-        if (Tp > T) FA_CUDA_TRY(cudaMemsetAsync(d_out, 0, need * sizeof(float), s_k));
-        h_units[0] = MelUnit{0, n, 0, Tp, 0, T, last, 0};
-        inline_unit = true;
-        st = launch(d_audio, d_out, 0, 1, tiles_of(T), mode, layout, s_k, true);
-        inline_unit = false;
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, need * sizeof(float), cudaMemcpyDeviceToHost, s_k));
-        FA_CUDA_TRY(cudaStreamSynchronize(s_k));
-        return FA_OK;
-    }
-    st = ensure_events(2 * (size_t)chunks);
-    if (st != FA_OK) return st;
-    for (int c = 0; c < chunks; ++c) h_units[c] = MelUnit{0, n, 0, Tp, bounds[c], bounds[c + 1] - bounds[c], last, 0};
-    FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, chunks * sizeof(MelUnit), cudaMemcpyHostToDevice, s_k));
-    if (Tp > T && !out_alias) FA_CUDA_TRY(cudaMemsetAsync(d_out, 0, need * sizeof(float), s_k));
-    const long long pad = mode == 0 ? cfg.n_fft / 2 : 0;
-    long long copied = 0;
-    for (int c = 0; c < chunks; ++c) {
-        const long long f_end = h_units[c].frame_begin + h_units[c].frame_count;            // exclusive
-        long long s_end = std::min(n, (f_end - 1) * cfg.hop_length + cfg.n_fft - pad);          // samples needed so far
-        if (c == chunks - 1) s_end = n;
-        if (s_end > copied) {
-            FA_CUDA_TRY(cudaMemcpyAsync(d_audio + copied, audio + copied, (s_end - copied) * sizeof(float),
-                                        cudaMemcpyHostToDevice, s_in));
-            copied = s_end;
-        }
-        FA_CUDA_TRY(cudaEventRecord(events[2 * c], s_in));
-        FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * c], 0));
-        st = launch(d_audio, k_out, c, 1, tiles_of(h_units[c].frame_count), mode, layout, s_k, true);
-        if (st != FA_OK) return st;
-        if (out_alias) continue;   // the kernel stored its rows in the caller's pinned buffer: no D2H stage
-        FA_CUDA_TRY(cudaEventRecord(events[2 * c + 1], s_k));
-        FA_CUDA_TRY(cudaStreamWaitEvent(s_out, events[2 * c + 1], 0));
-        const long long fb = h_units[c].frame_begin, fc = h_units[c].frame_count;
-        if (layout == 0) {
-            const long long rows = (c == chunks - 1) ? (Tp - fb) : fc;   // last unit also returns the zero pad rows
-            FA_CUDA_TRY(cudaMemcpyAsync(out + fb * cfg.n_mels, d_out + fb * cfg.n_mels, rows * cfg.n_mels * sizeof(float),
-                                        cudaMemcpyDeviceToHost, s_out));
-        } else {
-            const long long cols = (c == chunks - 1) ? (Tp - fb) : fc;
-            FA_CUDA_TRY(cudaMemcpy2DAsync(out + fb, Tp * sizeof(float), d_out + fb, Tp * sizeof(float),
-                                          cols * sizeof(float), cfg.n_mels, cudaMemcpyDeviceToHost, s_out));
-        }
-    }
-    FA_CUDA_TRY(cudaStreamSynchronize(s_out));
-    FA_CUDA_TRY(cudaStreamSynchronize(s_k));
-    return FA_OK;
-}
-
 int MelPlan::ensure_resampler(double in_rate, double out_rate) {
     if (in_rate == out_rate || (in_rate == rs_in && out_rate == rs_out && d_rs_tab)) return FA_OK;
     resample::Design d;
-    const int st = resample::make_design(in_rate, out_rate, d);
+    int st = resample::make_design(in_rate, out_rate, d);
     if (st != FA_OK) return st;
-    if (d_rs_tab) cudaFree(d_rs_tab);
-    d_rs_tab = nullptr;
-    FA_CUDA_TRY(cudaMalloc(&d_rs_tab, d.table.size() * sizeof(float)));
+    rs_in = rs_out = 0.0;   // the table is being replaced
+    st = grow_buffer(d_rs_tab, rs_tab_bytes, d.table.size() * sizeof(float));
+    if (st != FA_OK) return st;
     FA_CUDA_TRY(cudaMemcpy(d_rs_tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice));
     rs_design = std::move(d);
     rs_in = in_rate;
@@ -1047,61 +929,58 @@ int MelPlan::ensure_resampler(double in_rate, double out_rate) {
     return FA_OK;
 }
 
-// AudioConverter.resample + computeFlatTransposed as one device pipeline.  The PCM is copied in chunks; as soon as a
-// chunk has landed the compute stream converts the samples it completes (mixdown + polyphase / linear, see
-// resample_kernels.cu) into the float buffer the mel kernel reads, runs the frames those samples complete, and the D2H
-// stream returns their rows — H2D of chunk c+1, kernels of chunk c and D2H of chunk c-1 overlap.
-int MelPlan::compute_host_pcm(const void *pcm, long long frames, const resample::AudioFormat &f, float last, int mode,
-                              int layout, float *out, long long out_len, long long *mel_length, long long *num_frames,
-                              long long *resampled) {
+// Host buffers in, host buffers out: AudioConverter.resample + computeFlatTransposed as one device pipeline.  A long
+// clip is cut into units.  The PCM is copied in chunks; as soon as a chunk has landed the compute stream converts the
+// samples it completes (mixdown + polyphase / linear, see resample_kernels.cu) into the float buffer the mel kernel
+// reads, runs the frames those samples complete, and the D2H stream returns their rows — H2D of unit c+1, kernels of
+// unit c and D2H of unit c-1 overlap.  Identity input (mono float32 at the model rate) is copied straight into the float
+// buffer and needs no conversion kernel.
+int MelPlan::compute_host(const void *pcm, long long frames, const resample::AudioFormat &f, float last, int mode,
+                          long long expected, int layout, float *out, long long out_len, long long *mel_length,
+                          long long *num_frames, long long *resampled) {
     const long long n = resample::output_count(frames, f.in_rate, f.out_rate);
     if (resampled) *resampled = n;
     long long T, Tp;
-    if (!shape_of(*this, n, mode, -1, T, Tp)) {
-        if (mel_length) *mel_length = 0;
-        if (num_frames) *num_frames = mode == 2 ? 0 : 1;
-        if (mode != 2) {
-            if (out_len < cfg.n_mels) return FA_OUTPUT_TOO_SMALL;
-            for (int m = 0; m < cfg.n_mels; ++m) out[m] = 0.0f;
-        }
+    int st = clip_shape(*this, n, mode, expected, out_len, T, Tp, mel_length, num_frames);
+    if (st != FA_OK) return st;
+    if (T == 0) {
+        if (Tp) std::fill(out, out + cfg.n_mels, 0.0f);   // padValue
         return FA_OK;
     }
-    if (mel_length) *mel_length = T;
-    if (num_frames) *num_frames = Tp;
+    const bool identity = resample::is_identity(f);
     const long long need = Tp * cfg.n_mels;
-    if (out_len < need) {
-        fa::set_error("mel output needs %lld floats, buffer has %lld", need, out_len);
-        return FA_OUTPUT_TOO_SMALL;
-    }
-    int st = ensure_resampler(f.in_rate, f.out_rate);
+    st = ensure_resampler(f.in_rate, f.out_rate);
     if (st != FA_OK) return st;
     st = ensure_staging((size_t)n + 8, (size_t)need);
     if (st != FA_OK) return st;
     const size_t bps = f.format == resample::kPcmI16 ? 2 : 4;
     const size_t pcm_bytes = (size_t)frames * f.channels * bps;
-    if (pcm_bytes + 16 > d_pcm_cap) {
-        if (d_pcm) cudaFree(d_pcm);
-        d_pcm = nullptr;
-        d_pcm_cap = 0;
-        FA_CUDA_TRY(cudaMalloc(&d_pcm, pcm_bytes + 16));
-        d_pcm_cap = pcm_bytes + 16;
+    char *d_in = reinterpret_cast<char *>(d_audio);   // where the input lands
+    if (!identity) {
+        st = grow_buffer(d_pcm, d_pcm_bytes, pcm_bytes + 16);
+        if (st != FA_OK) return st;
+        d_in = static_cast<char *>(d_pcm);
     }
-    // pipeline depth: ~10 MB of PCM per chunk (the copy engines' fixed cost per transfer and the host's enqueue rate make
-    // finer chunks slower: int16 hour 3.08 ms at 8-12 chunks, 3.44 at 24, 3.61 at 96 — profiles/r02_mel.md)
-    const long long kMaxChunks = std::max<long long>(1, std::min<long long>(pipeline_chunks, (long long)(pcm_bytes / (10u << 20)) + 1));
-    const std::vector<long long> bounds = unit_bounds(T, kMaxChunks, 4096);
+    // Units: pipeline_chunks for identity input; converted input keeps ~10 MB of PCM per unit (the copy engines' fixed
+    // cost per transfer and the host's enqueue rate make finer units slower there: int16 hour 3.08 ms at 8-12 units,
+    // 3.44 at 24, 3.61 at 96).
+    const long long max_units =
+        identity ? pipeline_chunks : std::min<long long>(pipeline_chunks, (long long)(pcm_bytes / (10u << 20)) + 1);
+    const std::vector<long long> bounds = unit_bounds(T, max_units, 4096);
     const int chunks = (int)bounds.size() - 1;
-    float *out_alias = (zero_copy_out && layout == 0) ? device_alias_if_pinned(out) : nullptr;
+    // A single unit is the streaming callers' shape (a few thousand samples, SortformerDiarizer.swift:857-905): nothing
+    // to overlap, so one stream, no events, the unit descriptor passed in the kernel parameters, one synchronisation.
+    const bool single = chunks == 1;
+    float *out_alias = (zero_copy_out && layout == 0 && !single) ? device_alias_if_pinned(out) : nullptr;
     float *k_out = out_alias ? out_alias : d_out;   // where the kernel writes
     if (out_alias && Tp > T) std::memset(out + T * cfg.n_mels, 0, (size_t)(Tp - T) * cfg.n_mels * sizeof(float));
     st = ensure_units(chunks);
     if (st != FA_OK) return st;
     st = ensure_events(2 * (size_t)chunks);
     if (st != FA_OK) return st;
-    cudaStream_t s_in = streams[0], s_k = streams[1], s_out = streams[2];
+    cudaStream_t s_k = streams[1], s_in = single ? s_k : streams[0], s_out = single ? s_k : streams[2];
     for (int c = 0; c < chunks; ++c) h_units[c] = MelUnit{0, n, 0, Tp, bounds[c], bounds[c + 1] - bounds[c], last, 0};
-    FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, chunks * sizeof(MelUnit), cudaMemcpyHostToDevice, s_k));
-    if (Tp > T && !out_alias) FA_CUDA_TRY(cudaMemsetAsync(d_out, 0, need * sizeof(float), s_k));
+    if (!single) FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, chunks * sizeof(MelUnit), cudaMemcpyHostToDevice, s_k));
     const long long pad = mode == 0 ? cfg.n_fft / 2 : 0;
     const resample::Design &D = rs_design;
     const bool linear = f.in_rate != f.out_rate && resample::resolve_algorithm(f) == resample::kAlgoLinear;
@@ -1109,64 +988,69 @@ int MelPlan::compute_host_pcm(const void *pcm, long long frames, const resample:
     PipelineTrace trace;
     trace.start(s_in);
     for (int c = 0; c < chunks; ++c) {
-        const long long f_end = h_units[c].frame_begin + h_units[c].frame_count;
-        long long s_end = std::min(n, (f_end - 1) * cfg.hop_length + cfg.n_fft - pad);   // model-rate samples needed so far
-        if (c == chunks - 1) s_end = n;
-        // input frames those samples depend on
+        const bool tail = c == chunks - 1;
+        // model-rate samples needed so far, and the input frames those samples depend on
+        const long long s_end = tail ? n : std::min(n, (bounds[c + 1] - 1) * cfg.hop_length + cfg.n_fft - pad);
         long long in_need = frames;
-        if (c != chunks - 1) {
+        if (!tail) {
             if (f.in_rate == f.out_rate) in_need = s_end;
             else if (linear) in_need = (long long)((double)(s_end + 1) * (f.in_rate / f.out_rate)) + 4;
             else in_need = ((s_end + 2) * D.M) / D.L + D.half + 3;
             in_need = std::min(frames, std::max(in_need, in_copied));
         }
         if (in_need > in_copied) {
-            const char *src = reinterpret_cast<const char *>(pcm);
-            char *dst = reinterpret_cast<char *>(d_pcm);
+            const char *src = static_cast<const char *>(pcm);
             if (f.interleaved || f.channels == 1) {
                 const size_t a = (size_t)in_copied * f.channels * bps, b = (size_t)in_need * f.channels * bps;
-                FA_CUDA_TRY(cudaMemcpyAsync(dst + a, src + a, b - a, cudaMemcpyHostToDevice, s_in));
+                FA_CUDA_TRY(cudaMemcpyAsync(d_in + a, src + a, b - a, cudaMemcpyHostToDevice, s_in));
             } else {
                 for (int ch = 0; ch < f.channels; ++ch) {
                     const size_t a = ((size_t)ch * frames + in_copied) * bps, b = ((size_t)ch * frames + in_need) * bps;
-                    FA_CUDA_TRY(cudaMemcpyAsync(dst + a, src + a, b - a, cudaMemcpyHostToDevice, s_in));
+                    FA_CUDA_TRY(cudaMemcpyAsync(d_in + a, src + a, b - a, cudaMemcpyHostToDevice, s_in));
                 }
             }
             in_copied = in_need;
         }
-        FA_CUDA_TRY(cudaEventRecord(events[2 * c], s_in));
-        trace.mark(s_in, c, 0);
-        FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * c], 0));
-        long long ready = resample::outputs_ready(f, D, frames, in_copied, n);
-        if (ready < s_end) {
-            fa::set_error("internal: resampler window accounting (%lld < %lld)", ready, s_end);
-            return FA_RUNTIME_ERROR;
+        // zero the pad rows after the first input copy: a copy from pageable memory first waits for its stream's queue
+        if (c == 0 && Tp > T && !out_alias) FA_CUDA_TRY(cudaMemsetAsync(d_out, 0, need * sizeof(float), s_k));
+        if (!single) {
+            FA_CUDA_TRY(cudaEventRecord(events[2 * c], s_in));
+            FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * c], 0));
         }
-        ready = c == chunks - 1 ? n : s_end;
-        st = resample::launch_convert(d_pcm, frames, f, D, d_rs_tab, d_audio, converted, ready, s_k, &launches);
-        if (st != FA_OK) return st;
-        converted = std::max(converted, ready);
-        st = launch(d_audio, k_out, c, 1, tiles_of(h_units[c].frame_count), mode, layout, s_k, true);
+        trace.mark(s_in, c, 0);
+        if (!identity) {
+            const long long ready = resample::outputs_ready(f, D, frames, in_copied, n);
+            if (ready < s_end) {
+                fa::set_error("internal: resampler window accounting (%lld < %lld)", ready, s_end);
+                return FA_RUNTIME_ERROR;
+            }
+            st = resample::launch_convert(d_pcm, frames, f, D, d_rs_tab, d_audio, converted, s_end, s_k, &launches);
+            if (st != FA_OK) return st;
+            converted = std::max(converted, s_end);
+        }
+        inline_unit = single;
+        st = launch(d_audio, k_out, c, 1, tiles_of(bounds[c + 1] - bounds[c]), mode, layout, s_k, true);
+        inline_unit = false;
         if (st != FA_OK) return st;
         trace.mark(s_k, c, 1);
         if (out_alias) continue;   // the kernel stored its rows in the caller's pinned buffer: no D2H stage
-        FA_CUDA_TRY(cudaEventRecord(events[2 * c + 1], s_k));
-        FA_CUDA_TRY(cudaStreamWaitEvent(s_out, events[2 * c + 1], 0));
-        const long long fb = h_units[c].frame_begin, fc = h_units[c].frame_count;
-        if (layout == 0) {
-            const long long rows = (c == chunks - 1) ? (Tp - fb) : fc;
+        if (!single) {
+            FA_CUDA_TRY(cudaEventRecord(events[2 * c + 1], s_k));
+            FA_CUDA_TRY(cudaStreamWaitEvent(s_out, events[2 * c + 1], 0));
+        }
+        const long long fb = bounds[c], rows = (tail ? Tp : bounds[c + 1]) - fb;   // the last unit also returns the pad rows
+        if (layout == 0 || single) {   // a single unit returns the whole buffer in either layout
             FA_CUDA_TRY(cudaMemcpyAsync(out + fb * cfg.n_mels, d_out + fb * cfg.n_mels, rows * cfg.n_mels * sizeof(float),
                                         cudaMemcpyDeviceToHost, s_out));
         } else {
-            const long long cols = (c == chunks - 1) ? (Tp - fb) : fc;
             FA_CUDA_TRY(cudaMemcpy2DAsync(out + fb, Tp * sizeof(float), d_out + fb, Tp * sizeof(float),
-                                          cols * sizeof(float), cfg.n_mels, cudaMemcpyDeviceToHost, s_out));
+                                          rows * sizeof(float), cfg.n_mels, cudaMemcpyDeviceToHost, s_out));
         }
         trace.mark(s_out, c, 2);
     }
     FA_CUDA_TRY(cudaStreamSynchronize(s_out));
-    FA_CUDA_TRY(cudaStreamSynchronize(s_k));
-    trace.dump("pcm");
+    if (!single) FA_CUDA_TRY(cudaStreamSynchronize(s_k));
+    trace.dump(identity ? "f32" : "pcm");
     return FA_OK;
 }
 
@@ -1190,16 +1074,9 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
         doff[i] = same_layout ? offsets[i] - offsets[0] : a;
         a = same_layout ? ceil_to(offsets[i + 1] - offsets[0], 4) + 4 : a + ceil_to(n, 4) + 4;
         dout[i] = o;
-        long long T, Tp;
-        if (!shape_of(*this, n, mode, -1, T, Tp)) {
-            Ts[i] = 0;
-            Tps[i] = 0;
-            o += cfg.n_mels;
-        } else {
-            Ts[i] = T;
-            Tps[i] = Tp;
-            o += Tp * cfg.n_mels;
-        }
+        clip_shape(*this, n, mode, -1, kUnchecked, Ts[i], Tps[i], mel_lengths ? mel_lengths + i : nullptr,
+                   num_frames ? num_frames + i : nullptr);
+        o += std::max<long long>(Tps[i], 1) * cfg.n_mels;   // an empty clip returns one zero row, in every mode
     }
     doff[count] = a;
     dout[count] = o;
@@ -1219,8 +1096,6 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
         g_first[g] = used;
         int tiles = 0;
         for (int i = c0; i < c1; ++i) {
-            if (mel_lengths) mel_lengths[i] = Ts[i];
-            if (num_frames) num_frames[i] = Ts[i] ? Tps[i] : (mode == 2 ? 0 : 1);
             if (!Ts[i]) continue;
             h_units[used] = MelUnit{doff[i], offsets[i + 1] - offsets[i], dout[i], Tps[i], 0, Ts[i], last ? last[i] : 0.0f, tiles};
             tiles += tiles_of(Ts[i]);

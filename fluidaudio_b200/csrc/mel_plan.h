@@ -97,16 +97,18 @@ struct MelPlan {
     void *d_fb_slots = nullptr;
     int n_slots = 0;
 
+    // buffers grown on demand (grow_buffer); the *_bytes members are their capacities
     MelUnit *d_units = nullptr, *h_units = nullptr;
-    int units_cap = 0;
+    size_t d_units_bytes = 0, h_units_bytes = 0;
     float *d_audio = nullptr, *d_out = nullptr;   // staging for the host-buffer entry points
-    size_t d_audio_cap = 0, d_out_cap = 0;
+    size_t d_audio_bytes = 0, d_out_bytes = 0;
     // AudioConverter stage ahead of the kernel (fa_audio_to_mel): raw PCM staging + the polyphase table of the last ratio
     void *d_pcm = nullptr;
-    size_t d_pcm_cap = 0;
+    size_t d_pcm_bytes = 0;
     resample::Design rs_design;
     double rs_in = 0.0, rs_out = 0.0;
     float *d_rs_tab = nullptr;
+    size_t rs_tab_bytes = 0;
     cudaStream_t streams[3] = {nullptr, nullptr, nullptr};   // h2d, compute, d2h
     std::vector<cudaEvent_t> events;
     cudaEvent_t timer[2] = {nullptr, nullptr};   // fa_mel_timer_*: events on the compute stream
@@ -126,13 +128,12 @@ struct MelPlan {
     int compute_device(const float *d_in, long long n, float last, int mode, long long expected, int layout,
                        float *d_out_buf, long long out_len, long long *mel_length, long long *num_frames,
                        cudaStream_t stream);
-    int compute_host(const float *audio, long long n, float last, int mode, long long expected, int layout,
-                     float *out, long long out_len, long long *mel_length, long long *num_frames);
     // PCM in any AudioFormat (host) -> [device: mixdown + resample to cfg.sample_rate] -> log-mel (host).  Only the raw
-    // PCM crosses PCIe on the way in (int16 halves the bytes); *resampled = samples at the model rate.
-    int compute_host_pcm(const void *pcm, long long frames, const resample::AudioFormat &f, float last, int mode,
-                         int layout, float *out, long long out_len, long long *mel_length, long long *num_frames,
-                         long long *resampled);
+    // PCM crosses PCIe on the way in (int16 halves the bytes); *resampled = samples at the model rate.  Mono float32 at
+    // the model rate (resample::is_identity) is copied straight into the kernel's input, with no conversion kernel.
+    int compute_host(const void *pcm, long long frames, const resample::AudioFormat &f, float last, int mode,
+                     long long expected, int layout, float *out, long long out_len, long long *mel_length,
+                     long long *num_frames, long long *resampled);
     int ensure_resampler(double in_rate, double out_rate);
     int compute_batch_host(const float *audio, const long long *offsets, int count, const float *last, int mode,
                            int layout, float *out, const long long *out_offsets, long long *mel_lengths,

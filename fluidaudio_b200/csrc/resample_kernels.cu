@@ -10,15 +10,6 @@
 namespace fa {
 namespace resample {
 
-#define FA_CUDA_TRY(expr)                                                                   \
-    do {                                                                                    \
-        cudaError_t e__ = (expr);                                                           \
-        if (e__ != cudaSuccess) {                                                           \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            return FA_CUDA_ERROR;                                                           \
-        }                                                                                   \
-    } while (0)
-
 // ------------------------------------------------------------------------------------------------ design (host)
 bool rational_ratio(double in_rate, double out_rate, long long &L, long long &M) {
     double scale = 1.0;

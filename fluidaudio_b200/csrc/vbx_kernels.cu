@@ -21,15 +21,6 @@
 namespace fa {
 namespace vbx {
 
-#define FA_CUDA_TRY(expr)                                                                               \
-    do {                                                                                                \
-        cudaError_t e__ = (expr);                                                                       \
-        if (e__ != cudaSuccess) {                                                                       \
-            fa::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            return e__ == cudaErrorMemoryAllocation ? FA_ALLOCATION_FAILURE : FA_CUDA_ERROR;            \
-        }                                                                                               \
-    } while (0)
-
 constexpr int kChunks = 128;      // frame chunks for the two-level reductions (fewer when there are > 1024 speakers)
 constexpr int kEThreads = 128;    // threads per CTA in the E-step
 constexpr int kFChunks = 16;      // frame chunks of the two-kernel EM path
@@ -773,28 +764,7 @@ void Workspace::release() {
     pool_bytes = 0;
 }
 
-int Workspace::reserve(size_t bytes) {
-    if (bytes <= pool_bytes) return FA_OK;
-    if (pool) cudaFree(pool);
-    pool = nullptr;
-    pool_bytes = 0;
-    FA_CUDA_TRY(cudaMalloc(&pool, bytes));
-    pool_bytes = bytes;
-    return FA_OK;
-}
-
-namespace {
-struct Carver {
-    char *base;
-    size_t off = 0;
-    template <typename T> T *take(size_t count) {
-        off = (off + 255) & ~size_t(255);
-        T *p = reinterpret_cast<T *>(base + off);
-        off += count * sizeof(T);
-        return p;
-    }
-};
-} // namespace
+int Workspace::reserve(size_t bytes) { return grow_buffer(pool, pool_bytes, bytes); }
 
 size_t refine_bytes(int T, int D, int S, int max_it) {
     Carver c{nullptr};
