@@ -549,8 +549,10 @@ __device__ __forceinline__ float mel_dot_quads(const float4 *p4, const float4 *w
 // log of a mel value.  Device: one MUFU.LG2 and one multiply (|error| <= ~2 ulp of the result: 4e-6 at log(2^-24),
 // against the 1e-4 bar); host emulator: libm.  normal_floor: the floor is a normal float, so the argument never is a
 // denormal and the denormal pre-scaling of __log2f (three more instructions) can be skipped.
+// Clamped: max(v, floor) as Swift's max (AudioMelSpectrogram.swift:547) and std::max evaluate it, so a NaN mel value stays
+// NaN (`v > floor ? v : floor` would turn it into log(floor)); every other value gives the same bits either way.
 FA_HD float log_value(float v, float floor_, int clamped, int normal_floor = 0) {
-    const float x = clamped ? (v > floor_ ? v : floor_) : v + floor_;
+    const float x = clamped ? (floor_ >= v ? floor_ : v) : v + floor_;
 #if defined(__CUDA_ARCH__)
     float l;
     if (normal_floor) asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(l) : "f"(x));

@@ -225,17 +225,19 @@ __global__ void __launch_bounds__(kWarps * 32, 2) mel512_kernel(const MelLaunch 
     };
     // time-major tile is contiguous in HBM: nf rows of n_mels floats; flat, fully coalesced copy out of otile
     auto copy_out = [&](float *dst, int total) {
-        if ((P.n_mels & 3) == 0) {   // rows are whole float4s and dst is 64-byte aligned (f0 is a multiple of 16)
+        if (P.out_vec4) {   // rows are whole float4s and dst is 16-byte aligned (out, out_off checked by launch(); f0 % 16 == 0)
             float4 *d4 = reinterpret_cast<float4 *>(dst);
             for (int q = tid; q < (total >> 2); q += kWarps * 32) {
                 const int e = 4 * q;
                 const int row = (int)__umulhi((unsigned)e, P.inv_n_mels);                  // e / n_mels
                 d4[q] = *reinterpret_cast<const float4 *>(otile + e + 4 * row);             // row stride n_mels + 4: one LDS.128
             }
-        } else {
+        } else {   // any 4-byte aligned dst
+            const int row_pad = ot_stride - P.n_mels;   // 4 or 1
             for (int idx = tid; idx < total; idx += kWarps * 32) {
-                const int fi = (int)__umulhi((unsigned)idx, P.inv_n_mels);   // idx / n_mels (exact for idx < 2^16)
-                dst[idx] = otile[idx + fi];                                  // padded row stride n_mels + 1
+                // idx / n_mels (exact for idx < 2^16); one mel: 2^32 does not fit inv_n_mels
+                const int fi = P.n_mels == 1 ? idx : (int)__umulhi((unsigned)idx, P.inv_n_mels);
+                dst[idx] = otile[idx + fi * row_pad];
             }
         }
     };
@@ -519,8 +521,8 @@ int MelPlan::init(const MelConfig &c) {
 
     // banded filterbank: per mel the contiguous range of non-zero bins, widened with explicit zero weights to whole
     // bin quads.  Weights are stored times 1/4 because the kernel's power tile holds 4|X|^2 (mel_core.cuh).
-    std::vector<float> w;
     std::vector<int> lo(cfg.n_mels), hi(cfg.n_mels), off(cfg.n_mels);
+    fb_nnz = 0;
     for (int m = 0; m < cfg.n_mels; ++m) {
         int a = bins, b = 0;
         for (int k = 0; k < bins; ++k)
@@ -533,15 +535,9 @@ int MelPlan::init(const MelConfig &c) {
         b = (b + 3) & ~3;              // may reach 260 > 257: the tile's pad columns are zero, so are these weights
         lo[m] = a;
         hi[m] = b;
-        off[m] = (int)w.size();        // a multiple of four: 16-byte aligned weight quads
-        // packed in the order the kernel finds the bins in its power tile: mel512_kernel swizzles inside each bin quad
-        // (pow_pos, mel_core.cuh), the any-nFFT kernel keeps the natural order
-        for (int k = a; k < b; ++k) {
-            const int src = generic ? k : ((k & ~3) | ((k & 3) ^ ((k >> 4) & 3)));   // position k holds bin src: pow_pos is an involution
-            w.push_back(src < bins ? 0.25f * filterbank[(size_t)m * bins + src] : 0.0f);
-        }
+        off[m] = fb_nnz;               // a multiple of four: 16-byte aligned weight quads
+        fb_nnz += b - a;
     }
-    fb_nnz = (int)w.size();
     // filterbank-stage schedule of mel512_kernel: groups of four consecutive filters, dealt to the 8 warps longest first
     // (cost = widest band of the group, in quads); slot = (iteration * 8 + warp) * 4 + member
     std::vector<int4> slots;
@@ -586,6 +582,32 @@ int MelPlan::init(const MelConfig &c) {
     const int st = sm90_device_props(dev, prop);
     if (st != FA_OK) return st;
     num_sms = prop.multiProcessorCount;
+
+    if (!generic) {
+        pt_len = (kTileFrames - 1) * cfg.hop_length + kNfft;
+        pt_cap = (pt_len + 31) & ~31;
+        raw_cap = (pt_len + 1 + 3 + 3 + 31) & ~31;   // whole 128-byte lines: the pre-emphasised tile behind it stays line-aligned
+        fb_cap = (fb_nnz + 3) & ~3;
+        smem_bytes = sizeof(float) * ((size_t)2 * raw_cap + pt_cap + 0 +
+                                      (size_t)(kTileFrames / 2) * kPairStride + (size_t)kTileFrames * (cfg.n_mels + 4) + fb_cap) +
+                     sizeof(cpxd) * (size_t)kWarpsPerCta * kFftPad + sizeof(int) * 4 * (size_t)n_slots + 8 +
+                     2 * sizeof(uint64_t) + 3 * sizeof(TileInfo) + 16;
+        // three tiles of 15 hops + 512 samples: past the opt-in limit (on H100 even hops from about 900 at 80 mels) the
+        // any-nFFT kernel, whose budget does not depend on the hop, takes the configuration
+        if (smem_bytes > (size_t)prop.sharedMemPerBlockOptin) {
+            generic = true;
+            pt_len = pt_cap = raw_cap = fb_cap = 0;
+        }
+    }
+    // weights packed in the order the kernel finds the bins in its power tile: mel512_kernel swizzles inside each bin quad
+    // (pow_pos, mel_core.cuh), the any-nFFT kernel keeps the natural order
+    std::vector<float> w;
+    w.reserve(fb_nnz);
+    for (int m = 0; m < cfg.n_mels; ++m)
+        for (int k = lo[m]; k < hi[m]; ++k) {
+            const int src = generic ? k : ((k & ~3) | ((k & 3) ^ ((k >> 4) & 3)));   // position k holds bin src: pow_pos is an involution
+            w.push_back(src < bins ? 0.25f * filterbank[(size_t)m * bins + src] : 0.0f);
+        }
 
     std::vector<float> win_tab(n_fft, 0.0f);
     std::vector<uint8_t> in_tab(n_fft, 0);
@@ -648,19 +670,6 @@ int MelPlan::init(const MelConfig &c) {
         FA_CUDA_TRY(cudaFuncSetAttribute(mel_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
         return FA_OK;
     }
-    pt_len = (kTileFrames - 1) * cfg.hop_length + kNfft;
-    pt_cap = (pt_len + 31) & ~31;
-    raw_cap = (pt_len + 1 + 3 + 3 + 31) & ~31;   // whole 128-byte lines: the pre-emphasised tile behind it stays line-aligned
-    fb_cap = (fb_nnz + 3) & ~3;
-    smem_bytes = sizeof(float) * ((size_t)2 * raw_cap + pt_cap + 0 +
-                                  (size_t)(kTileFrames / 2) * kPairStride + (size_t)kTileFrames * (cfg.n_mels + 4) + fb_cap) +
-                 sizeof(cpxd) * (size_t)kWarpsPerCta * kFftPad + sizeof(int) * 4 * (size_t)n_slots + 8 +
-                 2 * sizeof(uint64_t) + 3 * sizeof(TileInfo) + 16;
-    if (smem_bytes > (size_t)prop.sharedMemPerBlockOptin) {
-        fa::set_error("mel config needs %zu bytes of shared memory per CTA, device allows %zu", smem_bytes,
-                      (size_t)prop.sharedMemPerBlockOptin);
-        return FA_UNSUPPORTED;
-    }
     FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, double, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
     FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, double, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
     FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, f32x2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
@@ -714,6 +723,10 @@ int MelPlan::launch(const float *d_audio_base, float *d_out_base, int first, int
     P.log_floor = cfg.log_floor;
     P.log_clamped = cfg.log_floor_mode;
     P.ot_stride = (cfg.n_mels & 3) == 0 ? cfg.n_mels + 4 : cfg.n_mels + 1;
+    // float4 copy-out only when every destination row is 16-byte aligned: the caller's d_out, a batch's out_offsets or a
+    // pinned output may sit at any 4-byte boundary (h_units mirrors the units of every launch)
+    P.out_vec4 = (cfg.n_mels & 3) == 0 && (reinterpret_cast<uintptr_t>(d_out_base) & 15) == 0;
+    for (int i = first; i < first + count && P.out_vec4; ++i) P.out_vec4 = (h_units[i].out_off & 3) == 0;
     P.log_normal = cfg.log_floor >= 1e-37f ? 1 : 0;   // mel energies are >= 0: log's argument is then never a denormal
     P.layout = layout;
     P.lane_tab = d_lane_tab[mode == 2 ? 1 : 0][precision == 1 ? 1 : 0];

@@ -119,7 +119,8 @@ int32_t fa_mel_get_precision(const fa_mel *mel);
 fa_status fa_mel_set_pipeline_chunks(fa_mel *mel, int32_t chunks);
 /* When the caller's time-major output buffer is pinned host memory (fa_host_alloc / cudaHostAlloc), the kernel stores its rows
  * straight into it over PCIe instead of staging them in HBM and copying.  Default OFF: the copy engine is the
- * measured default; pageable buffers always take the copy. */
+ * measured default; pageable buffers always take the copy.  Any 4-byte aligned `out` works (16-byte aligned rows are
+ * stored as 16-byte vectors, other rows one float at a time); results are identical either way. */
 fa_status fa_mel_set_zero_copy_output(fa_mel *mel, int32_t enabled);
 
 /* Host buffers in and out (the drop-in call).  On return *mel_length = valid frames, *num_frames = padded frames;
@@ -127,7 +128,11 @@ fa_status fa_mel_set_zero_copy_output(fa_mel *mel, int32_t enabled);
 fa_status fa_mel_compute(fa_mel *mel, const float *audio, size_t sample_count, float last_audio_sample,
                          int32_t padding_mode, int64_t expected_frames, int32_t layout, float *out, size_t out_len,
                          int64_t *mel_length, int64_t *num_frames);
-/* Same with buffers already resident in HBM (asynchronous on the library stream). */
+/* Same with buffers already resident in HBM (asynchronous on the library stream).  d_audio and d_out need only 4-byte
+ * (float) alignment; 16-byte aligned buffers take the faster bulk-copy input and vector stores, with identical results.
+ * As in every mel entry point: any hop is accepted (nFFT 512 with an even hop takes the specialised kernel while its shared
+ * memory fits, everything else the any-nFFT kernel), and a NaN sample makes every frame whose window holds it (after
+ * pre-emphasis) NaN in every mel with a non-empty filter band, in both log-floor modes. */
 fa_status fa_mel_compute_device(fa_mel *mel, const float *d_audio, size_t sample_count, float last_audio_sample,
                                 int32_t padding_mode, int64_t expected_frames, int32_t layout, float *d_out,
                                 size_t out_len, int64_t *mel_length, int64_t *num_frames);
@@ -136,6 +141,8 @@ fa_status fa_mel_compute_device(fa_mel *mel, const float *d_audio, size_t sample
 fa_status fa_mel_compute_batch(fa_mel *mel, const float *audio, const int64_t *offsets, int32_t clip_count,
                                const float *last_samples, int32_t padding_mode, int32_t layout, float *out,
                                const int64_t *out_offsets, int64_t *mel_lengths, int64_t *num_frames);
+/* The batch with buffers resident in HBM.  offsets and out_offsets may be any float offsets (d_audio and d_out 4-byte
+ * aligned); results are identical to fa_mel_compute_batch. */
 fa_status fa_mel_compute_batch_device(fa_mel *mel, const float *d_audio, const int64_t *offsets, int32_t clip_count,
                                       const float *last_samples, int32_t padding_mode, int32_t layout, float *d_out,
                                       const int64_t *out_offsets, int64_t *mel_lengths, int64_t *num_frames);

@@ -205,6 +205,101 @@ def test_kernel_lane_math_matches_oracle(tmp_path, oracle):
                       oracle.hann_window(), np.float32(2.0 ** -24), 0, T, out) == 0
     assert np.abs(out.T - ref).max() <= 1e-4
 
+    # The configuration space of the specialised kernel: even hops, window lengths on both sides of the mid_full boundary
+    # (buffer positions [64, 448)) centred and at offset 0, mel counts with empty filters, other sample rates, every log
+    # floor (subnormal and zero too) in both floor modes, with and without pre-emphasis.  FP64 transform: DESIGN's bar,
+    # |d| <= 1e-5 + 4e-7 |ref| (the second term: 2 ulp of the log at large magnitudes); float32 pairs: 1e-4 (f32_bar).
+    hops = (2, 64, 128, 158, 256, 320, 512, 514, 1000)
+    wins = (512, 449, 448, 400, 385, 384, 383, 256, 64)
+    mels = (1, 3, 23, 40, 81, 128, 200, 257)
+    rates = (8000, 22050, 48000, 16000)
+    floors = (2.0 ** -24, 1e-10, 1e-38, 0.0)
+    worst = {"f64": 0.0, "f32x2": 0.0}
+
+    def run(fn, x, cfg, mode, last, off, nm, sr):
+        """One emulator call against the oracle in the same mode: returns (emulated, oracle) as [T x nMels]."""
+        if mode == 2:
+            ref, T = oracle.mel_legacy(cfg, x)
+            ref = ref.T
+        else:
+            ref, T, _ = oracle.mel_flat_transposed(cfg, x, last=last, padding_mode=mode)
+            ref = ref[:T]
+        out = np.zeros((T, nm), np.float32)
+        pad, pre = (256 if mode == 0 else 0), (np.float32(0.0) if mode == 2 else np.float32(cfg.preemph))
+        assert fn(x, x.size, last, cfg.hop_length, cfg.win_length, off, pad, pre, nm, oracle.mel_filterbank(512, nm, sr),
+                  oracle.hann_window(cfg.win_length), np.float32(cfg.log_floor), cfg.log_floor_mode, T, out) == 0
+        return out, ref
+
+    def check(out, ref, fb, bar, what):
+        """NaN frames of the oracle (dense filterbank: every mel) must be NaN in every non-empty band; elsewhere the values
+        agree within the bar, non-finite values (log 0 = -inf) exactly."""
+        nan_rows = np.isnan(ref).all(axis=1)
+        assert not np.isnan(ref[~nan_rows]).any(), what
+        band = fb.any(axis=1)
+        assert np.isnan(out[nan_rows][:, band]).all(), what
+        o, r = out[~nan_rows], ref[~nan_rows]
+        fin = np.isfinite(r)
+        assert np.array_equal(o[~fin], r[~fin]) and np.isfinite(o[fin]).all(), what
+        top = np.broadcast_to(np.where(np.isfinite(r), r, -np.inf).max(axis=1, keepdims=True), r.shape)
+        d = np.abs(o[fin] - r[fin])
+        ok = d <= bar(r[fin], top[fin])
+        assert ok.all(), (what, float(d.max()), "largest so far", worst)
+        return float(d.max()) if d.size else 0.0, nan_rows
+
+    fp64_bar = lambda r, top: 1e-5 + 4e-7 * np.abs(r)
+    # float32 pairs: 1e-4, except for mel values more than 12 nats below the frame's strongest one.  There the float32
+    # transform's rounding noise (a fraction of an ulp of the strongest line in every bin, DESIGN §2) dominates the value:
+    # near-DC bands after pre-emphasis at 22.05 / 48 kHz reach 3e-4 at 18 nats down; the bar grows with exp(depth), capped
+    # at 2e-3 (the largest deviation measured here is 5.1e-4, on the GPU over tests/test_gpu_mel_sweep.py 9.8e-4).
+    f32_bar = lambda r, top: np.minimum(2e-3, 1e-4 * np.maximum(1.0, np.exp(top - r - 12.0)))
+    i = 0
+    for hop in hops:
+        for win in wins:
+            for mode in (0, 1, 2):   # centred with and without the centre padding; legacy: offset 0, no pre-emphasis
+                nm, sr, fl = mels[i % len(mels)], rates[i % len(rates)], floors[i % len(floors)]
+                clamped, pre = (i // len(floors)) % 2, (0.97 if (i // 2) % 2 == 0 else 0.0)
+                i += 1
+                cfg = oracle.mel_config(sample_rate=sr, n_mels=nm, hop_length=hop, win_length=win, preemph=pre,
+                                        log_floor=fl, log_floor_mode=clamped)
+                off = 0 if mode == 2 else (512 - win) // 2
+                frames = (17, 33, 2, 16, 1, 31, 15)[i % 7]
+                x = synth.tone_noise_audio(max(1, (frames - 1) * hop + 512 - (256 if mode == 0 else 0)), seed=i)
+                fb = oracle.mel_filterbank(512, nm, sr)
+                what = dict(hop=hop, win=win, mode=mode, n_mels=nm, sr=sr, floor=fl, clamped=clamped, pre=pre)
+                out, ref = run(L.mel_emul, x, cfg, mode, 0.3, off, nm, sr)
+                worst["f64"] = max(worst["f64"], check(out, ref, fb, fp64_bar, what)[0])
+                out, ref = run(L.mel_emul_f32x2, x, cfg, mode, 0.3, off, nm, sr)
+                worst["f32x2"] = max(worst["f32x2"], check(out, ref, fb, f32_bar, what)[0])
+    assert i == len(hops) * len(wins) * 3
+
+    # NaN samples: at the first and last in-window sample of a frame (the frame must be NaN), and one sample outside the
+    # window on either side (the kernel must select the in-window samples, not multiply the whole buffer by a window that is
+    # zero there: NaN * 0 = NaN).  Every window placement, both floor modes, both value types.
+    for win in wins:
+        for mode in (0, 2):
+            for clamped in (0, 1):
+                nm, hop = 40, 160
+                cfg = oracle.mel_config(n_mels=nm, hop_length=hop, win_length=win, preemph=0.97, log_floor=1e-10,
+                                        log_floor_mode=clamped)
+                off, pad = (0, 0) if mode == 2 else ((512 - win) // 2, 256)
+                f = 6
+                for j, inside in ((off, True), (off + win - 1, True), (off - 1, False), (off + win, False)):
+                    if j < 0 or j >= 512:
+                        continue
+                    x = synth.tone_noise_audio(16 * hop + 512, seed=win + j)
+                    x[f * hop + j - pad] = np.nan
+                    for fn, bar in ((L.mel_emul, fp64_bar), (L.mel_emul_f32x2, f32_bar)):
+                        what = dict(win=win, mode=mode, clamped=clamped, j=j, fn=fn.__name__)
+                        out, ref = run(fn, x, cfg, mode, 0.0, off, nm, 16000)
+                        _, nan_rows = check(out, ref, oracle.mel_filterbank(512, nm), bar, what)
+                        # not vacuous: a NaN inside the window poisons the frame, one outside it (after pre-emphasis
+                        # on the right; on the left only without it) leaves the frame finite
+                        if inside:
+                            assert nan_rows[f], what
+                        elif j > off or mode == 2:
+                            assert not nan_rows[f] and np.isfinite(out[f]).all(), what
+    print("largest |d log-mel| vs the oracle:", worst)
+
 
 def test_merge_control_plane_matches_reference_goldens(tmp_path, golden_dir, oracle):
     """ahc_core.cuh (slot-indexed heap + live bitmap, the code the device master warp runs) driven on the host in the
