@@ -71,6 +71,7 @@ EXPORTED_SYMBOLS = [
     "fa_mel_destroy", "fa_mel_get_window", "fa_mel_get_filterbank", "fa_mel_frame_count", "fa_mel_compute",
     "fa_mel_compute_device", "fa_mel_compute_batch", "fa_mel_compute_batch_device", "fa_mel_timer_start",
     "fa_mel_timer_stop_ms", "fa_mel_set_precision", "fa_mel_get_precision", "fa_mel_set_pipeline_chunks", "fa_mel_set_zero_copy_output", "fa_mel_normalize_per_feature", "fa_mel_unified_features", "fa_mel_lseend_features",
+    "fa_mel_stream_open", "fa_mel_stream_close", "fa_mel_stream_frames", "fa_mel_stream_push", "fa_mel_stream_push_device",
     "fa_resample_output_count", "fa_audio_resample", "fa_audio_to_mel",
     "fa_linear_resample", "fa_l2_normalize_rows", "fa_ahc_cluster", "fa_dendrogram_cut", "fa_vbx_default_config",
     "fa_vbx_refine", "fa_compute_centroids", "fa_assign_embeddings", "fa_cluster_default_config",
@@ -131,6 +132,12 @@ def load():
     L.fa_mel_normalize_per_feature.argtypes = [vp, i64, i32, i64]
     L.fa_mel_unified_features.argtypes = [vp, vp, sz, sz, vp, sz, C.POINTER(i64), C.POINTER(i32)]
     L.fa_mel_lseend_features.argtypes = [vp, vp, sz, vp, C.POINTER(i64), vp, sz, C.POINTER(i64)]
+    L.fa_mel_stream_open.argtypes = [vp, C.POINTER(i32)]
+    L.fa_mel_stream_close.argtypes = [vp, i32]
+    L.fa_mel_stream_frames.argtypes = [vp, i32, i64, i32]
+    L.fa_mel_stream_frames.restype = i64
+    L.fa_mel_stream_push.argtypes = [vp, i32, vp, vp, vp, vp, vp, sz, vp]
+    L.fa_mel_stream_push_device.argtypes = L.fa_mel_stream_push.argtypes
     L.fa_resample_output_count.argtypes = [C.POINTER(AudioFormat), i64]
     L.fa_resample_output_count.restype = i64
     L.fa_audio_resample.argtypes = [vp, i64, C.POINTER(AudioFormat), vp, i64, C.POINTER(i64)]

@@ -422,6 +422,7 @@ static thread_local cudaEvent_t t_ev0 = nullptr, t_ev1 = nullptr;
 
 struct MelHandle {
     mel::MelPlan plan;
+    mel::MelStreamSet sessions;   // fa_mel_stream_*: live streams on this plan
     int device = 0;
 };
 
@@ -732,6 +733,55 @@ FA_API fa_status fa_mel_timer_stop_ms(fa_mel *mel, float *elapsed_ms) {
     FA_CUDA_TRY(cudaEventSynchronize(h->plan.timer[1]));
     FA_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, h->plan.timer[0], h->plan.timer[1]));
     return FA_STATUS_OK;
+}
+
+// Live streams (SortformerDiarizer.swift:204-217, :417-424, :842-901): sessions on the handle, see mel_stream.cu.
+FA_API fa_status fa_mel_stream_open(fa_mel *mel, int32_t *session) {
+    if (!mel || !session) return FA_STATUS_INVALID_ARGUMENT;
+    FA_GUARD_BEGIN
+    auto *h = reinterpret_cast<MelHandle *>(mel);
+    int id = -1;
+    const int st = h->sessions.open(h->plan, &id);
+    if (st == FA_OK) *session = id;
+    return (fa_status)st;
+    FA_GUARD_END
+}
+
+FA_API fa_status fa_mel_stream_close(fa_mel *mel, int32_t session) {
+    if (!mel) return FA_STATUS_INVALID_ARGUMENT;
+    return (fa_status) reinterpret_cast<MelHandle *>(mel)->sessions.close(session);
+}
+
+FA_API int64_t fa_mel_stream_frames(const fa_mel *mel, int32_t session, int64_t new_samples, int32_t finish) {
+    if (!mel) return -1;
+    const auto *h = reinterpret_cast<const MelHandle *>(mel);
+    return h->sessions.frames(h->plan, session, new_samples, finish != 0);
+}
+
+static fa_status mel_stream_push(fa_mel *mel, int32_t count, const int32_t *sessions, const float *audio,
+                                 const int64_t *offsets, const int32_t *finish, bool device, float *out, size_t out_len,
+                                 int64_t *frames) {
+    if (!mel) return FA_STATUS_INVALID_ARGUMENT;
+    FA_GUARD_BEGIN
+    auto *h = reinterpret_cast<MelHandle *>(mel);
+    const long long before = h->plan.launches;
+    const int st = h->sessions.push(h->plan, count, sessions, audio, reinterpret_cast<const long long *>(offsets), finish,
+                                    device, out, (long long)out_len, reinterpret_cast<long long *>(frames));
+    g_launches += h->plan.launches - before;
+    return (fa_status)st;
+    FA_GUARD_END
+}
+
+FA_API fa_status fa_mel_stream_push(fa_mel *mel, int32_t count, const int32_t *sessions, const float *audio,
+                                    const int64_t *offsets, const int32_t *finish, float *out, size_t out_len,
+                                    int64_t *frames) {
+    return mel_stream_push(mel, count, sessions, audio, offsets, finish, false, out, out_len, frames);
+}
+
+FA_API fa_status fa_mel_stream_push_device(fa_mel *mel, int32_t count, const int32_t *sessions, const float *d_audio,
+                                           const int64_t *offsets, const int32_t *finish, float *d_out, size_t out_len,
+                                           int64_t *frames) {
+    return mel_stream_push(mel, count, sessions, d_audio, offsets, finish, true, d_out, out_len, frames);
 }
 
 // UnifiedMelExtractor.features(window:validCount:) (UnifiedMelExtractor.swift:52-86): log-mel + per-feature

@@ -490,6 +490,9 @@ void MelPlan::release() {
     d_units_bytes = h_units_bytes = d_audio_bytes = d_out_bytes = d_pcm_bytes = rs_tab_bytes = 0;
     if (h_units) cudaFreeHost(h_units);
     h_units = nullptr;
+    if (units_uploaded) cudaEventDestroy(units_uploaded);
+    units_uploaded = nullptr;
+    units_in_flight = false;
     for (auto &s : streams)
         if (s) cudaStreamDestroy(s), s = nullptr;
     for (auto &e : events)
@@ -686,9 +689,23 @@ long long MelPlan::frame_count(long long n, int mode, long long expected) const 
 }
 
 int MelPlan::ensure_units(int count) {
+    // the device entry points return with their descriptor upload still queued behind earlier work on the stream: the
+    // pinned h_units may be rewritten (or replaced) only once that copy has read it
+    if (units_in_flight) {
+        FA_CUDA_TRY(cudaEventSynchronize(units_uploaded));
+        units_in_flight = false;
+    }
     const size_t bytes = (size_t)std::max(count, 64) * sizeof(MelUnit);
     const int st = grow_buffer(d_units, d_units_bytes, bytes);
     return st != FA_OK ? st : grow_buffer(h_units, h_units_bytes, bytes, true);
+}
+
+int MelPlan::upload_units(int count, cudaStream_t stream) {
+    if (!units_uploaded) FA_CUDA_TRY(cudaEventCreateWithFlags(&units_uploaded, cudaEventDisableTiming));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, count * sizeof(MelUnit), cudaMemcpyHostToDevice, stream));
+    FA_CUDA_TRY(cudaEventRecord(units_uploaded, stream));
+    units_in_flight = true;
+    return FA_OK;
 }
 
 int MelPlan::ensure_staging(size_t audio_floats, size_t out_floats) {
@@ -707,14 +724,21 @@ int MelPlan::ensure_events(size_t count) {
 
 int MelPlan::launch(const float *d_audio_base, float *d_out_base, int first, int count, int total_tiles, int mode,
                     int layout, cudaStream_t stream, bool aligned16) {
+    return launch_units(d_units + first, h_units + first, count, d_audio_base, d_out_base, total_tiles, mode, layout,
+                        stream, aligned16);
+}
+
+int MelPlan::launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, const float *d_audio_base,
+                          float *d_out_base, int total_tiles, int mode, int layout, cudaStream_t stream,
+                          bool aligned16) {
     if (total_tiles <= 0) return FA_OK;
     MelLaunch P{};
     P.audio = d_audio_base;
     P.out = d_out_base;
-    P.units = d_units + first;
+    P.units = d_u;
     P.num_units = count;
     P.inline_unit = (inline_unit && count == 1) ? 1 : 0;
-    if (P.inline_unit) P.unit0 = h_units[first];
+    if (P.inline_unit) P.unit0 = h_u[0];
     P.total_tiles = total_tiles;
     P.hop = cfg.hop_length;
     P.pad = mode == 0 ? cfg.n_fft / 2 : 0;
@@ -726,7 +750,7 @@ int MelPlan::launch(const float *d_audio_base, float *d_out_base, int first, int
     // float4 copy-out only when every destination row is 16-byte aligned: the caller's d_out, a batch's out_offsets or a
     // pinned output may sit at any 4-byte boundary (h_units mirrors the units of every launch)
     P.out_vec4 = (cfg.n_mels & 3) == 0 && (reinterpret_cast<uintptr_t>(d_out_base) & 15) == 0;
-    for (int i = first; i < first + count && P.out_vec4; ++i) P.out_vec4 = (h_units[i].out_off & 3) == 0;
+    for (int i = 0; i < count && P.out_vec4; ++i) P.out_vec4 = (h_u[i].out_off & 3) == 0;
     P.log_normal = cfg.log_floor >= 1e-37f ? 1 : 0;   // mel energies are >= 0: log's argument is then never a denormal
     P.layout = layout;
     P.lane_tab = d_lane_tab[mode == 2 ? 1 : 0][precision == 1 ? 1 : 0];
@@ -816,7 +840,8 @@ int MelPlan::compute_device(const float *d_in, long long n, float last, int mode
     if (st != FA_OK) return st;
     if (Tp > T) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf, 0, Tp * cfg.n_mels * sizeof(float), stream));
     h_units[0] = MelUnit{0, n, 0, Tp, 0, T, last, 0};
-    FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, sizeof(MelUnit), cudaMemcpyHostToDevice, stream));
+    st = upload_units(1, stream);
+    if (st != FA_OK) return st;
     const bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
     return launch(d_in, d_out_buf, 0, 1, tiles_of(T), mode, layout, stream, aligned);
 }
@@ -844,7 +869,8 @@ int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, i
         ++used;
     }
     if (!used) return FA_OK;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, used * sizeof(MelUnit), cudaMemcpyHostToDevice, stream));
+    st = upload_units(used, stream);
+    if (st != FA_OK) return st;
     return launch(d_in, d_out_buf, 0, used, tiles, mode, layout, stream, aligned);
 }
 

@@ -101,6 +101,10 @@ struct MelPlan {
     // buffers grown on demand (grow_buffer); the *_bytes members are their capacities
     MelUnit *d_units = nullptr, *h_units = nullptr;
     size_t d_units_bytes = 0, h_units_bytes = 0;
+    // recorded after every asynchronous h_units -> d_units copy: ensure_units() waits on it before h_units is rewritten,
+    // so back-to-back device calls never overwrite descriptors whose upload is still queued
+    cudaEvent_t units_uploaded = nullptr;
+    bool units_in_flight = false;
     float *d_audio = nullptr, *d_out = nullptr;   // staging for the host-buffer entry points
     size_t d_audio_bytes = 0, d_out_bytes = 0;
     // AudioConverter stage ahead of the kernel (fa_audio_to_mel): raw PCM staging + the polyphase table of the last ratio
@@ -118,12 +122,18 @@ struct MelPlan {
     void release();
     int init(const MelConfig &c);
     long long frame_count(long long n, int mode, long long expected) const;
+    // h_units holds `count` units and may be written (waits for a queued upload of its previous contents)
     int ensure_units(int count);
+    // queues the copy of h_units[0, count) into d_units on `stream` and records units_uploaded behind it
+    int upload_units(int count, cudaStream_t stream);
     int ensure_staging(size_t audio_floats, size_t out_floats);
     int ensure_events(size_t count);
     // kernel launch over units [first, first+count) already resident in d_units
     int launch(const float *d_audio_base, float *d_out_base, int first, int count, int total_tiles, int mode,
                int layout, cudaStream_t stream, bool aligned16);
+    // the same over `count` units at d_u (device) whose host mirror is h_u (read for the output alignment); never inline
+    int launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, const float *d_audio_base, float *d_out_base,
+                     int total_tiles, int mode, int layout, cudaStream_t stream, bool aligned16);
 
     // mode: 0 .center, 1 .prePadded, 2 legacy compute(); layout: 0 time-major, 1 mel-major
     int compute_device(const float *d_in, long long n, float last, int mode, long long expected, int layout,
@@ -142,6 +152,42 @@ struct MelPlan {
     int compute_batch_device(const float *d_in, const long long *offsets, int count, const float *last, int mode,
                              int layout, float *d_out_buf, const long long *out_offsets, long long *mel_lengths,
                              long long *num_frames, cudaStream_t stream);
+};
+
+// mel_stream.cu: live streams on one plan, SortformerDiarizer's incremental mel stream (SortformerDiarizer.swift:204-217,
+// :417-424, :842-901) for many sessions at once.  Per session, the samples not yet consumed by a frame (the carry, fewer
+// than nFFT/2 + win/2 of them) and the pre-emphasis state `last` stay in HBM; the counters stay on the host.  One push
+// advances any number of sessions with one ingest launch and one mel launch.
+struct MelStreamJob;
+
+struct MelStreamSet {
+    int capacity = 0;                    // floats per session in d_carry: round_up4(nFFT/2 + win/2)
+    int slots = 0;                       // sessions d_carry / d_last hold
+    float *d_carry = nullptr;            // [slots x capacity]
+    float *d_last = nullptr;             // [slots] lastAudioSample
+    std::vector<long long> carry_len, received, emitted;
+    std::vector<uint8_t> live, finished;
+    // push staging: descriptors (units, then jobs) in one pinned buffer and its device copy, the pushed samples of a
+    // host push, and the arena the ingest kernel assembles every emitting session's contiguous input in
+    void *h_desc = nullptr, *d_desc = nullptr;
+    size_t h_desc_bytes = 0, d_desc_bytes = 0;
+    float *d_arena = nullptr;
+    size_t d_arena_bytes = 0;
+    cudaEvent_t desc_uploaded = nullptr;   // h_desc may be rewritten once this has completed
+    bool desc_in_flight = false;
+
+    ~MelStreamSet();
+    static int check_config(const MelConfig &c);   // pad_to <= 1 and hop <= win, or FA_INVALID_ARGUMENT
+    int open(MelPlan &p, int *session);
+    int close(int session);
+    bool valid(int session) const { return session >= 0 && session < slots && live[session]; }
+    // rows the next push of `n` samples (finish 0/1) to `session` emits
+    long long frames(const MelPlan &p, int session, long long n, bool finish) const;
+    // Session sessions[i] receives audio[offsets[i] .. offsets[i+1]); its frames[i] rows start at row sum_{j<i} frames[j]
+    // of out.  device: audio and out are HBM and the call is asynchronous on the compute stream; otherwise both are host
+    // buffers, the samples travel in one copy, the rows in one copy, and the call returns after one synchronisation.
+    int push(MelPlan &p, int count, const int *sessions, const float *audio, const long long *offsets, const int *finish,
+             bool device, float *out, long long out_len, long long *frames);
 };
 
 // mel_adapters.cu: device epilogues for the callers directly behind AudioMelSpectrogram (host buffers in and out)

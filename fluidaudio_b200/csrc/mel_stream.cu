@@ -1,0 +1,348 @@
+// Live log-mel streams: SortformerDiarizer's incremental mel stream (SortformerDiarizer.swift:204-217 reset, :417-424
+// addAudio, :842-870 emit every covered frame, :876-901 finish with a pre-emphasis-cancelling decay tail) for any number
+// of sessions on one MelPlan.
+//
+// The reference keeps, per session, an audio buffer seeded with nFFT/2 zeros, lastAudioSample, the real samples received
+// and the frames emitted.  Each emit runs computeFlatTransposed(.prePadded, expectedFrameCount: count) over the buffer,
+// then drops count*hop samples.  Here the buffer's unconsumed samples (the carry) and lastAudioSample live in HBM, one
+// fixed slot per session: between pushes a session carries fewer than nFFT/2 + win/2 samples (DESIGN §4.1c), so a slot
+// holds round_up4(nFFT/2 + win/2) floats.  The counters live on the host, which therefore knows every frame count before
+// anything runs.
+//
+// One push, whatever the number of sessions:
+//   H2D samples (host push) + H2D descriptors -> mel_stream_ingest_kernel (one CTA per session with work) -> one
+//   MelPlan launch over the emitting sessions' units (.prePadded, time-major) -> D2H rows + synchronise (host push).
+// The ingest CTA assembles [carry | new samples | tail] contiguously at a 16-byte aligned arena offset (the mel kernel's
+// bulk-copy path), copies the session's `last` into its MelUnit, then writes back the new carry and `last`.
+#include "fa_common.cuh"
+#include "mel_plan.h"
+
+#include <algorithm>
+#include <cstring>
+#include <cuda_runtime.h>
+#include <vector>
+
+namespace fa {
+namespace mel {
+
+struct MelStreamJob {
+    long long src;      // offset of the pushed samples in the source buffer
+    long long n_new;    // pushed samples
+    long long arena;    // offset of the session's input [carry | new (| tail)] in the arena, a multiple of 4; -1: no frame
+    long long arena2;   // finish after an emit in the same push: offset of [buffer[consumed ..) | tail]; -1 otherwise
+    int session;
+    int carry_len;      // samples carried in
+    int consumed;       // count * hop of the (first) emit
+    int tail;           // decay-tail samples appended to the last input (0 or nFFT/2)
+    int unit;           // MelUnit of the (first) emit; a split finish's second unit follows it
+    int finish;         // the session ends with this push: no carry write-back
+};
+
+static constexpr int kIngestThreads = 256;
+
+__global__ void __launch_bounds__(kIngestThreads) mel_stream_ingest_kernel(const MelStreamJob *__restrict__ jobs,
+                                                                           const float *__restrict__ src, float *carry_all,
+                                                                           float *last_all, float *arena, MelUnit *units,
+                                                                           int capacity, float preemph) {
+    const MelStreamJob J = jobs[blockIdx.x];
+    const int tid = threadIdx.x;
+    float *carry = carry_all + (size_t)J.session * capacity;
+    const float *x = src + J.src;
+    if (J.unit < 0) {   // no frame this push: the samples join the carry (its bound leaves room for them)
+        for (long long k = tid; k < J.n_new; k += kIngestThreads) carry[J.carry_len + k] = x[k];
+        return;
+    }
+    const long long L = J.carry_len + J.n_new;
+    float *buf = arena + J.arena;
+    for (int k = tid; k < J.carry_len; k += kIngestThreads) buf[k] = carry[k];
+    for (long long k = tid; k < J.n_new; k += kIngestThreads) buf[J.carry_len + k] = x[k];
+    if (tid == 0) units[J.unit].last = last_all[J.session];
+    __syncthreads();   // the whole buffer is in the arena: the carry may be overwritten, the split copy read
+    const bool split = J.arena2 >= 0;
+    const long long left = L - (split ? J.consumed : 0);   // the buffer the finishing emit sees, before its tail
+    if (split) {
+        float *buf2 = arena + J.arena2;
+        for (long long k = tid; k < left; k += kIngestThreads) buf2[k] = buf[J.consumed + k];
+        if (tid == 0) units[J.unit + 1].last = buf[J.consumed - 1];
+    }
+    if (J.tail && tid == 0) {
+        // padAndEmitRemainingMelLocked (:888-896): value = buffer.last, value *= preemph per sample, float32 rounded at
+        // every step; zeros when preemph is 0 or the buffer is empty
+        float *t = (split ? arena + J.arena2 : buf) + left;
+        const bool decay = preemph != 0.0f && left > 0;
+        float v = left > 0 ? buf[L - 1] : 0.0f;
+        for (int i = 0; i < J.tail; ++i) {
+            v = decay ? __fmul_rn(v, preemph) : 0.0f;
+            t[i] = v;
+        }
+    }
+    if (!J.finish) {   // emitMelFramesLocked (:862-865): lastAudioSample = buffer[consumed - 1], drop `consumed` samples
+        for (long long k = tid; k < L - J.consumed; k += kIngestThreads) carry[k] = buf[J.consumed + k];
+        if (tid == 0) last_all[J.session] = buf[J.consumed - 1];
+    }
+}
+
+static inline long long round_up4(long long v) { return (v + 3) & ~3LL; }
+
+// Frames of one push: `first` from addAudio's preprocessAudioToFeaturesLocked (:847-854), `second` from
+// padAndEmitRemainingMelLocked (:876-883) when the push finishes the session.  Integer division truncates like Swift's.
+static void push_frames(const MelConfig &c, long long received, long long emitted, bool finished, long long n, bool fin,
+                        long long &first, long long &second) {
+    first = second = 0;
+    if (finished) return;   // shouldDropAudioLocked
+    const long long r = received + n, half_win = c.win_length / 2;
+    if (r >= half_win) first = std::max(0LL, (r - half_win) / c.hop_length + 1 - emitted);
+    if (fin && r > 0) second = std::max(0LL, 1 + (r + c.n_fft - c.win_length) / c.hop_length - emitted - first);
+}
+
+MelStreamSet::~MelStreamSet() {
+    if (d_carry) cudaFree(d_carry);
+    if (d_last) cudaFree(d_last);
+    if (d_arena) cudaFree(d_arena);
+    if (d_desc) cudaFree(d_desc);
+    if (h_desc) cudaFreeHost(h_desc);
+    if (desc_uploaded) cudaEventDestroy(desc_uploaded);
+}
+
+int MelStreamSet::check_config(const MelConfig &c) {
+    if (c.pad_to > 1) {
+        fa::set_error("mel stream: pad_to must be 0 or 1 (an emit returns exactly its frames), got %d", c.pad_to);
+        return FA_INVALID_ARGUMENT;
+    }
+    if (c.hop_length > c.win_length) {
+        fa::set_error("mel stream: hop_length (%d) must not exceed win_length (%d)", c.hop_length, c.win_length);
+        return FA_INVALID_ARGUMENT;
+    }
+    return FA_OK;
+}
+
+int MelStreamSet::open(MelPlan &p, int *session) {
+    int st = check_config(p.cfg);
+    if (st != FA_OK) return st;
+    const int half = p.cfg.n_fft / 2;
+    capacity = (int)round_up4(half + p.cfg.win_length / 2);
+    cudaStream_t s = p.streams[1];
+    int id = 0;
+    while (id < slots && live[id]) ++id;   // ids are dense from 0: the lowest closed one is reused
+    if (id == slots) {
+        // grow, keeping the live sessions' carries and `last` (queued pushes finish first: same stream)
+        const int grown = std::max(64, 2 * slots);
+        float *c = nullptr, *l = nullptr;
+        cudaError_t e = cudaMalloc(&c, (size_t)grown * capacity * sizeof(float));
+        if (e == cudaSuccess) e = cudaMalloc(&l, (size_t)grown * sizeof(float));
+        if (e != cudaSuccess) {
+            if (c) cudaFree(c);
+            return fa::cuda_failure(e, "cudaMalloc(mel stream state)", __FILE__, __LINE__);
+        }
+        if (slots) {
+            FA_CUDA_TRY(cudaMemcpyAsync(c, d_carry, (size_t)slots * capacity * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            FA_CUDA_TRY(cudaMemcpyAsync(l, d_last, (size_t)slots * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            FA_CUDA_TRY(cudaStreamSynchronize(s));
+            cudaFree(d_carry);
+            cudaFree(d_last);
+        }
+        d_carry = c;
+        d_last = l;
+        slots = grown;
+        for (auto *v : {&carry_len, &received, &emitted}) v->resize(grown, 0);
+        live.resize(grown, 0);
+        finished.resize(grown, 0);
+    }
+    // resetMelStreamLocked (:204-217): the buffer is nFFT/2 zeros, lastAudioSample 0, counters cleared
+    FA_CUDA_TRY(cudaMemsetAsync(d_carry + (size_t)id * capacity, 0, (size_t)half * sizeof(float), s));
+    FA_CUDA_TRY(cudaMemsetAsync(d_last + id, 0, sizeof(float), s));
+    carry_len[id] = half;
+    received[id] = emitted[id] = 0;
+    finished[id] = 0;
+    live[id] = 1;
+    *session = id;
+    return FA_OK;
+}
+
+int MelStreamSet::close(int session) {
+    if (!valid(session)) {
+        fa::set_error("mel stream: session %d is not open", session);
+        return FA_INVALID_ARGUMENT;
+    }
+    live[session] = 0;
+    return FA_OK;
+}
+
+long long MelStreamSet::frames(const MelPlan &p, int session, long long n, bool finish) const {
+    if (!valid(session) || n < 0) return -1;
+    long long first, second;
+    push_frames(p.cfg, received[session], emitted[session], finished[session] != 0, n, finish, first, second);
+    return first + second;
+}
+
+int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *audio, const long long *offsets,
+                       const int *finish, bool device, float *out, long long out_len, long long *frames_out) {
+    const MelConfig &c = p.cfg;
+    const int M = c.n_mels, hop = c.hop_length, half = c.n_fft / 2;
+    if (count < 0 || (count > 0 && (!sessions || !offsets || !frames_out))) {
+        fa::set_error("mel stream push: count must be >= 0, sessions / offsets / frames non-null");
+        return FA_INVALID_ARGUMENT;
+    }
+    if (count == 0) return FA_OK;
+    // every argument is checked before any state changes: a failed push leaves every session as it was
+    if (offsets[0] < 0) {
+        fa::set_error("mel stream push: offsets[0] is negative (%lld)", offsets[0]);
+        return FA_INVALID_ARGUMENT;
+    }
+    std::vector<uint8_t> seen(slots, 0);
+    for (int i = 0; i < count; ++i) {
+        const int id = sessions[i];
+        if (!valid(id)) {
+            fa::set_error("mel stream push: session %d is not open", id);
+            return FA_INVALID_ARGUMENT;
+        }
+        if (seen[id]) {
+            fa::set_error("mel stream push: session %d appears twice", id);
+            return FA_INVALID_ARGUMENT;
+        }
+        seen[id] = 1;
+        if (offsets[i + 1] < offsets[i]) {
+            fa::set_error("mel stream push: offsets decrease at %d (%lld > %lld)", i, offsets[i], offsets[i + 1]);
+            return FA_INVALID_ARGUMENT;
+        }
+    }
+    const long long total_new = offsets[count] - offsets[0];
+    if (total_new > 0 && !audio) {
+        fa::set_error("mel stream push: audio is null");
+        return FA_INVALID_ARGUMENT;
+    }
+    struct Step {
+        long long first, second, L;
+        bool fin;
+    };
+    std::vector<Step> step(count);
+    long long rows = 0, arena = 0;
+    int units = 0, jobs = 0;
+    const long long bound = half + c.win_length / 2;   // carried samples stay below this (DESIGN §4.1c)
+    for (int i = 0; i < count; ++i) {
+        const int id = sessions[i];
+        Step &S = step[i];
+        const long long n = offsets[i + 1] - offsets[i];
+        S.fin = finish && finish[i];
+        push_frames(c, received[id], emitted[id], finished[id] != 0, n, S.fin, S.first, S.second);
+        S.L = carry_len[id] + n;
+        rows += S.first + S.second;
+        if (finished[id]) continue;
+        const long long consumed = S.first * hop, tail = S.second ? half : 0;
+        if (consumed > S.L || (!S.fin && S.L - consumed >= bound)) {
+            fa::set_error("internal: mel stream carry bound (session %d: %lld samples, %lld consumed)", id, S.L, consumed);
+            return FA_RUNTIME_ERROR;
+        }
+        if (S.first + S.second == 0) {
+            if (n > 0 && !S.fin) ++jobs;   // samples join the carry
+            continue;
+        }
+        ++jobs;
+        const bool split = S.first > 0 && S.second > 0;
+        units += split ? 2 : 1;
+        arena += round_up4(S.L + (split ? 0 : tail)) + (split ? round_up4(S.L - consumed + tail) : 0);
+    }
+    if (rows > 0 && (!out || out_len < rows * M)) {
+        fa::set_error("mel stream push: output needs %lld floats, buffer has %lld", rows * M, out ? out_len : 0);
+        return FA_OUTPUT_TOO_SMALL;
+    }
+
+    // ---- buffers: h_desc is rewritten only after its previous upload has read it
+    if (desc_in_flight) {
+        FA_CUDA_TRY(cudaEventSynchronize(desc_uploaded));
+        desc_in_flight = false;
+    }
+    if (!desc_uploaded) FA_CUDA_TRY(cudaEventCreateWithFlags(&desc_uploaded, cudaEventDisableTiming));
+    const size_t units_bytes = (((size_t)units * sizeof(MelUnit)) + 15) & ~size_t(15);
+    const size_t desc_bytes = units_bytes + (size_t)jobs * sizeof(MelStreamJob);
+    int st = grow_buffer(h_desc, h_desc_bytes, std::max<size_t>(desc_bytes, 4096), true);
+    if (st == FA_OK) st = grow_buffer(d_desc, d_desc_bytes, std::max<size_t>(desc_bytes, 4096));
+    if (st == FA_OK) st = grow_buffer(d_arena, d_arena_bytes, (size_t)std::max(arena, 1024LL) * sizeof(float));
+    if (st == FA_OK && !device) st = p.ensure_staging((size_t)std::max(total_new, 0LL) + 8, (size_t)rows * M);
+    if (st != FA_OK) return st;
+
+    // ---- descriptors
+    MelUnit *hu = static_cast<MelUnit *>(h_desc);
+    MelStreamJob *hj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(h_desc) + units_bytes);
+    MelUnit *du = static_cast<MelUnit *>(d_desc);
+    MelStreamJob *dj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(d_desc) + units_bytes);
+    const long long src0 = device ? 0 : offsets[0];   // a host push's samples land at d_audio[0]
+    long long row = 0, a = 0;
+    int u = 0, j = 0, tiles = 0;
+    for (int i = 0; i < count; ++i) {
+        const int id = sessions[i];
+        const Step &S = step[i];
+        const long long n = offsets[i + 1] - offsets[i], emit = S.first + S.second;
+        if (finished[id] || (emit == 0 && (n == 0 || S.fin))) continue;
+        MelStreamJob &J = hj[j++];
+        J = MelStreamJob{offsets[i] - src0, n, -1, -1, id, (int)carry_len[id], 0, 0, -1, S.fin ? 1 : 0};
+        if (emit == 0) continue;
+        const bool split = S.first > 0 && S.second > 0;
+        J.consumed = (int)(S.first * hop);
+        J.tail = S.second ? half : 0;
+        J.unit = u;
+        J.arena = a;
+        const long long c1 = split ? S.first : emit;   // frames of the first unit
+        const long long n1 = S.L + (split ? 0 : J.tail);
+        hu[u++] = MelUnit{a, n1, row * M, c1, 0, c1, 0.0f, tiles};   // .last: written by the ingest kernel
+        tiles += (int)((c1 + 15) / 16);
+        a += round_up4(n1);
+        if (split) {
+            J.arena2 = a;
+            const long long n2 = S.L - J.consumed + J.tail;
+            hu[u++] = MelUnit{a, n2, (row + c1) * M, S.second, 0, S.second, 0.0f, tiles};
+            tiles += (int)((S.second + 15) / 16);
+            a += round_up4(n2);
+        }
+        row += emit;
+    }
+
+    // ---- device work, all on the compute stream
+    cudaStream_t s = p.streams[1];
+    const float *src = audio;
+    if (!device) {
+        if (total_new > 0)
+            FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio, audio + offsets[0], (size_t)total_new * sizeof(float),
+                                        cudaMemcpyHostToDevice, s));
+        src = p.d_audio;
+    }
+    if (desc_bytes) {
+        FA_CUDA_TRY(cudaMemcpyAsync(d_desc, h_desc, desc_bytes, cudaMemcpyHostToDevice, s));
+        FA_CUDA_TRY(cudaEventRecord(desc_uploaded, s));
+        desc_in_flight = true;
+    }
+    if (jobs) {
+        mel_stream_ingest_kernel<<<jobs, kIngestThreads, 0, s>>>(dj, src, d_carry, d_last, d_arena, du, capacity, c.preemph);
+        FA_CUDA_TRY(cudaGetLastError());
+        ++p.launches;
+    }
+    float *k_out = device ? out : p.d_out;
+    if (units) {
+        // `last` lives in d_units (written by the ingest kernel): the launch must read its units from HBM, never inline
+        const bool saved = p.inline_unit;
+        p.inline_unit = false;
+        st = p.launch_units(du, hu, units, d_arena, k_out, tiles, 1, 0, s, true);
+        p.inline_unit = saved;
+        if (st != FA_OK) return st;
+    }
+    if (!device) {
+        if (rows) FA_CUDA_TRY(cudaMemcpyAsync(out, p.d_out, (size_t)rows * M * sizeof(float), cudaMemcpyDeviceToHost, s));
+        FA_CUDA_TRY(cudaStreamSynchronize(s));
+    }
+
+    // ---- commit the host-side state
+    for (int i = 0; i < count; ++i) {
+        const int id = sessions[i];
+        const Step &S = step[i];
+        frames_out[i] = S.first + S.second;
+        if (finished[id]) continue;
+        received[id] += offsets[i + 1] - offsets[i];
+        emitted[id] += S.first + S.second;
+        carry_len[id] = S.L - S.first * hop;
+        if (S.fin) finished[id] = 1;
+    }
+    return FA_OK;
+}
+
+} // namespace mel
+} // namespace fa

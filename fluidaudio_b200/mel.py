@@ -206,6 +206,75 @@ class AudioMelSpectrogram:
         return ml, nf
 
 
+class MelStreams:
+    """Live log-mel streams on one ``AudioMelSpectrogram``: SortformerDiarizer's incremental mel stream
+    (Diarizer/Sortformer/SortformerDiarizer.swift:204-217, :417-424, :842-901) for any number of sessions, each push
+    advancing every session it names with a fixed number of launches (``fa_mel_stream_*``).  The sessions share the
+    handle's configuration (``pad_to`` 0 or 1, ``hop_length <= win_length``) and precision."""
+
+    def __init__(self, mel: AudioMelSpectrogram):
+        self.mel = mel
+        self.n_mels = mel.n_mels
+        self._L = mel._L
+
+    def open(self) -> int:
+        """resetMelStreamLocked: a new session (the lowest free id) with nFFT/2 zeros buffered."""
+        sid = C.c_int32()
+        _lib.check(self._L.fa_mel_stream_open(self.mel._h, C.byref(sid)), "fa_mel_stream_open")
+        return int(sid.value)
+
+    def close(self, session: int):
+        _lib.check(self._L.fa_mel_stream_close(self.mel._h, int(session)), "fa_mel_stream_close")
+
+    def pending_frames(self, session: int, n: int, finish: bool = False) -> int:
+        """Rows the next push of ``n`` samples (and ``finish``) to ``session`` emits."""
+        v = int(self._L.fa_mel_stream_frames(self.mel._h, int(session), int(n), int(bool(finish))))
+        if v < 0:
+            raise ValueError(f"session {session} is not open (or n < 0)")
+        return v
+
+    def _pack(self, chunks, finish):
+        chunks = {int(s): a for s, a in chunks.items()}
+        done = {int(f) for f in finish}
+        ids = list(chunks) + sorted(done - set(chunks))
+        arrays = [np.ascontiguousarray(chunks.get(s, np.zeros(0, np.float32)), np.float32).reshape(-1) for s in ids]
+        offsets = np.zeros(len(ids) + 1, np.int64)
+        offsets[1:] = np.cumsum([a.size for a in arrays])
+        audio = np.concatenate(arrays) if arrays else np.zeros(0, np.float32)
+        fin = np.array([1 if s in done else 0 for s in ids], np.int32)
+        return np.array(ids, np.int32), audio, offsets, fin
+
+    def push(self, chunks: dict, finish=()) -> dict:
+        """``chunks``: {session: samples} (addAudio); sessions in ``finish`` are finalised after their samples
+        (padAndEmitRemainingMelLocked).  Returns {session: [frames x nMels] float32} for every session named."""
+        ids, audio, offsets, fin = self._pack(chunks, finish)
+        counts = [self.pending_frames(s, int(offsets[i + 1] - offsets[i]), bool(fin[i])) for i, s in enumerate(ids)]
+        out = np.empty(max(1, sum(counts)) * self.n_mels, np.float32)
+        frames = np.zeros(ids.size, np.int64)
+        _lib.check(self._L.fa_mel_stream_push(self.mel._h, ids.size, _lib.ptr(ids), _lib.ptr(audio) if audio.size else None,
+                                              _lib.ptr(offsets), _lib.ptr(fin), out.ctypes.data, out.size,
+                                              frames.ctypes.data), "fa_mel_stream_push")
+        res, row = {}, 0
+        for s, f in zip(ids.tolist(), frames.tolist()):
+            res[s] = out[row * self.n_mels:(row + f) * self.n_mels].reshape(f, self.n_mels)
+            row += f
+        return res
+
+    def push_device(self, sessions, d_audio: "_lib.DeviceBuffer", offsets, d_out: "_lib.DeviceBuffer", finish=None,
+                    out_offset: int = 0) -> np.ndarray:
+        """The push with samples and rows in HBM: session ``sessions[i]`` reads ``d_audio[offsets[i]:offsets[i+1]]``; the
+        rows land at float ``out_offset`` of ``d_out`` in call order.  Asynchronous; returns the frame counts."""
+        ids = np.ascontiguousarray(sessions, np.int32)
+        offsets = np.ascontiguousarray(offsets, np.int64)
+        fin = None if finish is None else np.ascontiguousarray(finish, np.int32)
+        frames = np.zeros(ids.size, np.int64)
+        out_ptr = d_out.ptr.value + 4 * int(out_offset)
+        _lib.check(self._L.fa_mel_stream_push_device(self.mel._h, ids.size, _lib.ptr(ids), d_audio.ptr, _lib.ptr(offsets),
+                                                     _lib.ptr(fin), out_ptr, d_out.nbytes // 4 - int(out_offset),
+                                                     frames.ctypes.data), "fa_mel_stream_push_device")
+        return frames
+
+
 def normalize_per_feature(mel_time_major: np.ndarray, valid_frames: int) -> np.ndarray:
     """UnifiedMelExtractor.normalizePerFeature (UnifiedMelExtractor.swift:88-113) on a [frames x nMels] array."""
     x = np.ascontiguousarray(mel_time_major, np.float32).copy()

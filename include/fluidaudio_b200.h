@@ -147,6 +147,38 @@ fa_status fa_mel_compute_batch_device(fa_mel *mel, const float *d_audio, const i
                                       const float *last_samples, int32_t padding_mode, int32_t layout, float *d_out,
                                       const int64_t *out_offsets, int64_t *mel_lengths, int64_t *num_frames);
 
+/* Live streams: SortformerDiarizer's incremental mel stream (Diarizer/Sortformer/SortformerDiarizer.swift:204-217
+ * resetMelStreamLocked, :417-424 addAudio, :842-870 preprocessAudioToFeaturesLocked / emitMelFramesLocked, :876-901
+ * padAndEmitRemainingMelLocked) for many sessions on one handle, which they share config, precision and streams with.
+ * A session starts with nFFT/2 zero samples buffered.  A push appends its samples and emits every frame whose window they
+ * cover: count = (received - win/2) / hop + 1 - emitted, the .prePadded log-mel of the buffer with expected_frames = count
+ * and the session's last_audio_sample, after which count*hop samples are dropped.  finish (after the push's samples)
+ * appends nFFT/2 samples of the decay value *= preemph (zeros for preemph 0) and emits the frames left up to the .center
+ * count 1 + (received + nFFT - win) / hop; later pushes to a finished session are ignored.  Only configurations with
+ * pad_to <= 1 and hop_length <= win_length open a session (else FA_STATUS_INVALID_ARGUMENT).
+ *   fa_mel_stream_open     resets and returns the lowest free id (ids are dense from 0 and reused after close).
+ *   fa_mel_stream_frames   rows the next push of new_samples (finish 0/1) to `session` emits; -1 for a bad handle / session.
+ *   fa_mel_stream_push     session sessions[i] receives audio[offsets[i] .. offsets[i+1]) (packed as in
+ *                          fa_mel_compute_batch; count + 1 offsets), finished after them when finish[i] != 0 (finish may
+ *                          be NULL).  The sessions of one push are distinct.  frames[i] receives session i's rows; out
+ *                          receives them time-major in call order (session i at row sum_{j<i} frames[j]), out_len floats
+ *                          must hold all of them.  Every argument is checked before any state changes: a failed push
+ *                          leaves every session as it was.  One push costs one copy of the samples, one of the
+ *                          descriptors, two kernel launches, one copy of the rows and one synchronisation, whatever the
+ *                          number of sessions.
+ *   fa_mel_stream_push_device  the same with d_audio / d_out in HBM, asynchronous on the handle's compute stream
+ *                          (frames[] is still returned on return).
+ * Rows equal fa_mel_compute(buffer, last, FA_MEL_PAD_PREPADDED, count) of the reference's buffer bit for bit.  Sessions are
+ * not thread-safe, like the handle. */
+fa_status fa_mel_stream_open(fa_mel *mel, int32_t *session);
+fa_status fa_mel_stream_close(fa_mel *mel, int32_t session);
+int64_t fa_mel_stream_frames(const fa_mel *mel, int32_t session, int64_t new_samples, int32_t finish);
+fa_status fa_mel_stream_push(fa_mel *mel, int32_t count, const int32_t *sessions, const float *audio,
+                             const int64_t *offsets, const int32_t *finish, float *out, size_t out_len, int64_t *frames);
+fa_status fa_mel_stream_push_device(fa_mel *mel, int32_t count, const int32_t *sessions, const float *d_audio,
+                                    const int64_t *offsets, const int32_t *finish, float *d_out, size_t out_len,
+                                    int64_t *frames);
+
 /* CUDA-event timer on the stream the mel kernels run on: bracket any number of fa_mel_compute*_device calls. */
 fa_status fa_mel_timer_start(fa_mel *mel);
 fa_status fa_mel_timer_stop_ms(fa_mel *mel, float *elapsed_ms);
