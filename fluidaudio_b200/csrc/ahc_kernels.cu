@@ -25,7 +25,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <limits>
@@ -221,8 +220,10 @@ __global__ void ahc_filter_prep_kernel(const double *__restrict__ cols, int N, i
     }
 }
 
-template <bool kCollect>
-__global__ void __launch_bounds__(256) ahc_filter_tile_kernel(int N, int D, int Ns, FilterBufs F) {
+// Pass 2, dense form (when pass 1 did not keep its per (row, column tile) bounds, or a row of x does not fit the sparse
+// form's shared memory): the 64 x 64 tiles of the lower triangle recomputed as a SIMT GEMM, appending every pair inside
+// the band.  With the bounds kept, tiles in which no row can have a candidate exit early.
+__global__ void __launch_bounds__(256) ahc_filter_dense_kernel(int N, int D, int Ns, FilterBufs F) {
     __shared__ __align__(16) float As[kFK][kFT], Bs[kFK][kFT];
     // lower-triangular tile pair (ti >= tj) from the linear block index
     const int b = blockIdx.x;
@@ -232,7 +233,7 @@ __global__ void __launch_bounds__(256) ahc_filter_tile_kernel(int N, int D, int 
     const int tj = b - (int)((long long)ti * (ti + 1) / 2);
     const int i0 = ti * kFT, j0 = tj * kFT;
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    if (kCollect && F.tmin) {   // skip tiles in which no row can have a candidate (almost all of them)
+    if (F.tmin) {   // skip tiles in which no row can have a candidate (almost all of them)
         int any = 0;
         if (threadIdx.x < kFT) {
             const int i = i0 + threadIdx.x;
@@ -267,10 +268,9 @@ __global__ void __launch_bounds__(256) ahc_filter_tile_kernel(int N, int D, int 
 #pragma unroll
     for (int a = 0; a < 4; ++a) {
         const int i = i0 + ty * 4 + a;
-        double rowmin = 1.7976931348623157e308, rowlo = 1.7976931348623157e308;
         const double ni = i < N ? F.nrm2[i] : 0.0;
         const double ri = i < N ? (double)F.rn[i] : 0.0;
-        const double Ui = (kCollect && i < N) ? __longlong_as_double((long long)F.U[i]) : 0.0;
+        const double Ui = i < N ? __longlong_as_double((long long)F.U[i]) : 0.0;
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
             const int j = j0 + tx * 4 + c;
@@ -278,26 +278,11 @@ __global__ void __launch_bounds__(256) ahc_filter_tile_kernel(int N, int D, int 
                 const double nj = F.nrm2[j];
                 const double approx = (ni + nj) - 2.0 * (double)acc[a][c];
                 const double E = F.c1 * ri * (double)F.rn[j] + F.c2 * (ni + nj);
-                if (!kCollect) {
-                    rowmin = fmin(rowmin, fmax(approx + E, 0.0));
-                    rowlo = fmin(rowlo, approx - E);
-                } else if (approx - E <= Ui) {
+                if (approx - E <= Ui) {
                     const int slot = atomicAdd(&F.counters[0], 1);
                     if (slot < F.cap) F.cand[slot] = make_int2(i, j);
                     else F.counters[2] = 1;
                 }
-            }
-        }
-        if (!kCollect) {   // the 16 threads of a row group are one half-warp: fold, one atomic per (row, tile)
-#pragma unroll
-            for (int o = 8; o >= 1; o >>= 1) {
-                rowmin = fmin(rowmin, __shfl_xor_sync(0xffffffffu, rowmin, o));
-                rowlo = fmin(rowlo, __shfl_xor_sync(0xffffffffu, rowlo, o));
-            }
-            if (tx == 0 && i < N) {
-                if (rowmin < 1.7976931348623157e308) atomicMin(&F.U[i], (unsigned long long)__double_as_longlong(rowmin));
-                // what pass 2 needs to know about this (row, tile): can any pair in it be a candidate?
-                if (F.tmin) F.tmin[(size_t)i * F.nt + tj] = rowlo < 1.7976931348623157e308 ? __double2float_rd(rowlo) : 3.0e38f;
             }
         }
     }
@@ -545,15 +530,6 @@ __device__ __forceinline__ void st_relaxed_u64(u64 *p, u64 v) {
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 __device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
-__device__ __forceinline__ u64 global_ns() {
-    u64 t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define FA_TRACE(slot)                                                                         \
-    do {                                                                                       \
-        if ((P.flags & 4) && trace_step >= 0 && trace_step < kTraceSteps) P.trace[trace_step * 16 + (slot)] = global_ns(); \
-    } while (0)
 
 __device__ __forceinline__ u64 pack_cmd(int type, unsigned counter, int a, int b) {
     return ((u64)type << 62) | ((u64)(counter & 0x3fffu) << 48) | ((u64)(unsigned)a << 24) | (u64)(unsigned)b;
@@ -582,14 +558,13 @@ __device__ __forceinline__ void warp_cand_min(double &d, int &id) {
 // One polling snapshot: both words of up to Q slots per lane plus (optionally) the threshold words.
 template <int Q> struct PollSnap {
     u64 a0[Q], a1[Q], t0, t1;
-    __device__ __forceinline__ void issue(const ResultSlot *results, int shift, int W, int lane, unsigned tag,
-                                          const u64 *thr) {
+    __device__ __forceinline__ void issue(const ResultSlot *results, int W, int lane, unsigned tag, const u64 *thr) {
 #pragma unroll
         for (int q = 0; q < Q; ++q) {
             const int w = lane + 32 * q;
             a0[q] = (u64)(tag & 0xffu);
             a1[q] = (u64)tag;
-            if (w < W) ld_relaxed_v2(&results[(size_t)w << shift].w0, a0[q], a1[q]);   // one 16-byte request per slot
+            if (w < W) ld_relaxed_v2(&results[(size_t)w << kSlotShift].w0, a0[q], a1[q]);   // one 16-byte request per slot
         }
         t0 = t1 = (u64)tag;
         if (thr) ld_relaxed_v2(thr, t0, t1);
@@ -623,24 +598,23 @@ template <int Q> struct PollSnap {
 // service warp of every worker CTA: the exchange is all-to-all) and, optionally, the round's threshold words in the
 // same polling loop.  Each lane owns slots lane, lane+32, ...; all words are self-validating, all loads relaxed.
 // ~90 CTAs poll the same few lines, so the polling traffic itself sets the latency of the exchange: one 16-byte
-// request per candidate, one snapshot in flight, and every candidate in its own 128-byte line (slot_shift = 3)
+// request per candidate, one snapshot in flight, and every candidate in its own 128-byte line (kSlotShift = 3)
 // measured 1.1 us from the last candidate's store to the decision, against 1.9 us with two 8-byte loads per
 // packed slot, and three staggered snapshots in flight were slower than one (profiles/r01c_ahc_trace.md).
 // Returns the lexicographic (distance, id) minimum in every lane; `bad` = a NaN seen by any CTA.
-__device__ __forceinline__ void gather_candidates(const ResultSlot *results, int shift, int W, int lane, unsigned tag,
-                                                  double &d, int &id, bool &bad, const u64 *thr = nullptr,
-                                                  double *T = nullptr) {
+__device__ __forceinline__ void gather_candidates(const ResultSlot *results, int W, int lane, unsigned tag, double &d,
+                                                  int &id, bool &bad, const u64 *thr = nullptr, double *T = nullptr) {
     const unsigned full = 0xffffffffu;
     if (W <= 96) {
         PollSnap<3> s0;
         do {
-            s0.issue(results, shift, W, lane, tag, thr);
+            s0.issue(results, W, lane, tag, thr);
         } while (!s0.complete(tag));
         s0.reduce(W, lane, d, id, bad, T);
     } else {
         PollSnap<8> s0;   // W <= 255 worker CTAs
         do {
-            s0.issue(results, shift, W, lane, tag, thr);
+            s0.issue(results, W, lane, tag, thr);
         } while (!s0.complete(tag));
         s0.reduce(W, lane, d, id, bad, T);
     }
@@ -721,7 +695,6 @@ __device__ void ahc_master(const Problem &P, int W, unsigned char *sm) {
     bool failed = false;
     __shared__ int path_pos[40], path_slot[40], path_depth;
     __shared__ double path_key[40];
-    const bool allow_self = (P.flags & 8) == 0;
 
     auto publish = [&](int type, int a, int b) {   // lane 0
         st_release_u64(P.cmd, pack_cmd(type, ++cmd_counter, a, b));
@@ -731,7 +704,6 @@ __device__ void ahc_master(const Problem &P, int W, unsigned char *sm) {
     bool self_issued = false; // the workers already know the pair of this step
     for (int step = 0; step < N - 1 && !failed; ++step) {
         const int fresh = N + step;
-        const int trace_step = step - N / 2;   // trace a window in the middle of the run
         if (!self_issued) {
             for (;;) {    // lazy repair of a stale nearest neighbour (:1706-1734)
                 int stale = 0;
@@ -746,7 +718,7 @@ __device__ void ahc_master(const Problem &P, int W, unsigned char *sm) {
                 double d;
                 int id;
                 bool bad;
-                gather_candidates(P.results + (round & 1u) * P.result_stride, P.slot_shift, W, lane, round, d, id, bad);
+                gather_candidates(P.results + (round & 1u) * P.result_stride, W, lane, round, d, id, bad);
                 if (bad) {
                     failed = true;
                     break;
@@ -765,7 +737,6 @@ __device__ void ahc_master(const Problem &P, int W, unsigned char *sm) {
             a = node_of[sa];
             b = nn[sa];
             if (step < N - 2 && !self_issued) publish(CMD_MERGE, a, b);
-            FA_TRACE(0);
             live.drop(a);
             live.drop(b);
             P.merge_a[step] = a;
@@ -798,18 +769,15 @@ __device__ void ahc_master(const Problem &P, int W, unsigned char *sm) {
                 }
                 path_depth = depth;
                 T = depth >= 1 ? path_key[1] : INFINITY;
-                if (!allow_self) T = -1.0;   // tuning hook: never self-issue
                 publish_threshold(P.threshold + 2 * ((round + 1) & 1u), T, round + 1);
             }
-            FA_TRACE(1);
         }
         if (step < N - 2) {
             ++round;
             double d;
             int id;
             bool bad;
-            gather_candidates(P.results + (round & 1u) * P.result_stride, P.slot_shift, W, lane, round, d, id, bad);
-            if (lane == 0) FA_TRACE(2);
+            gather_candidates(P.results + (round & 1u) * P.result_stride, W, lane, round, d, id, bad);
             if (bad) {
                 failed = true;
                 break;
@@ -834,7 +802,6 @@ __device__ void ahc_master(const Problem &P, int W, unsigned char *sm) {
                 where[sa] = (Idx)to;
                 key[sa] = d;
                 nn[sa] = id;
-                FA_TRACE(3);
             }
             __syncwarp();
             self_issued = d <= T;   // same doubles, same comparison as in every worker CTA
@@ -936,10 +903,6 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
             if (type == CMD_EXIT) break;
         }
         ++round;
-        const int trace_step = (wb == 0 && lane == 0 && type == CMD_MERGE) ? merges - N / 2 : -1;
-        if (t == 0) FA_TRACE(4);
-        const int all_step = (lane == 0 && type == CMD_MERGE) ? merges - N / 2 : -1;   // any CTA (trace of the slowest)
-        if ((P.flags & 4) && t == 0 && all_step >= 0 && all_step < kTraceSteps) atomicMax(&P.trace[all_step * 16 + 12], global_ns());
         int limit;
         const double *v;
         if (type == CMD_MERGE) {
@@ -1009,7 +972,6 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
             __syncthreads();
             limit = a;
         }
-        if (t == 0) FA_TRACE(5);
         __syncwarp();   // lane 0's single-thread work above must not leave the warp split across the scan chain
         // ---- scan: one sequential chain per owned live node with id < limit ------------------------------
         if (!svc) {
@@ -1058,7 +1020,6 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
                     }
                 }
             }
-            if (t == 0) FA_TRACE(6);
             if (bad) best = INFINITY, best_id = INT_MAX;   // keep NaN bit patterns out of the integer-ordered reduction
             warp_cand_min(best, best_id);
             const bool warp_bad = __any_sync(0xffffffffu, bad);
@@ -1066,15 +1027,11 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
                 red_d[warp] = best;
                 red_id[warp] = warp_bad ? -2 : best_id;
             }
-            if (t == 0) FA_TRACE(11);
         }
-        if (t == kMergeThreads) FA_TRACE(13);
         __syncthreads();
-        if (t == 0) FA_TRACE(15);
         const bool last_scan = type == CMD_MERGE && merges >= N - 2;   // the master finishes the dendrogram alone
         if (svc) {
             if (lane == 0) {
-                FA_TRACE(8);
                 double best = INFINITY;
                 int best_id = INT_MAX;
                 bool any_bad = false;
@@ -1083,12 +1040,10 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
                 }
                 const u64 bits = (u64)__double_as_longlong(best);
                 const unsigned oid = any_bad ? 0xfffffeu : (best_id == INT_MAX ? 0xffffffu : (unsigned)best_id);
-                ResultSlot *slot = P.results + (round & 1u) * P.result_stride + ((size_t)wb << P.slot_shift);   // double-buffered by round parity:
+                ResultSlot *slot = P.results + (round & 1u) * P.result_stride + ((size_t)wb << kSlotShift);   // double-buffered by round parity:
                 // a CTA reuses a slot two rounds later, which it can only reach after every reader finished this round
                 st_relaxed_u64(&slot->w0, (bits & 0xffffffff00000000ull) | ((u64)oid << 8) | (u64)(round & 0xffu));
                 st_relaxed_u64(&slot->w1, (bits << 32) | (u64)round);
-                FA_TRACE(7);
-                if ((P.flags & 4) && all_step >= 0 && all_step < kTraceSteps) atomicMax(&P.trace[all_step * 16 + 14], global_ns());
                 s_owner = -1;
             }
             __syncwarp();   // lane 0 publishes before anybody starts polling
@@ -1098,10 +1053,9 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
                 int id;
                 bool any_bad;
                 double T;
-                gather_candidates(P.results + (round & 1u) * P.result_stride, P.slot_shift, W, lane, round, d, id, any_bad,
+                gather_candidates(P.results + (round & 1u) * P.result_stride, W, lane, round, d, id, any_bad,
                                   P.threshold + 2 * (round & 1u), &T);
                 if (lane == 0) {
-                    FA_TRACE(9);
                     s_have_pair = (!any_bad && d <= T) ? 1 : 0;
                     s_next_b = id;
                 }
@@ -1117,10 +1071,7 @@ __global__ void __launch_bounds__(kWorkerThreads, 1) ahc_merge_kernel(const Prob
         have_pair = s_have_pair != 0;
         a = prev_fresh;
         b = s_next_b;
-        if (svc) {
-            fence_acq_rel_gpu();   // the CTA's one fence per round, off the critical path (see above)
-            if (lane == 0) FA_TRACE(10);
-        }
+        if (svc) fence_acq_rel_gpu();   // the CTA's one fence per round, off the critical path (see above)
     }
 }
 
@@ -1204,7 +1155,7 @@ int Solver::init(cudaStream_t s, int worker_limit) {
 namespace {
 struct Layout {
     size_t rows, cols, node_weight, key, nn, heap_at, heap_where, node_of, slot_of, live_bits, merge_a, merge_b, merge_d,
-        cmd, threshold, results, error, trace, init_partial, problem, total;
+        cmd, threshold, results, error, init_partial, problem, total;
     size_t f_cf, f_nrm2, f_rn, f_U, f_best_d, f_best_j, f_cand, f_cand_d, f_counters, f_tmin;
     bool f_keep_tmin;
     int ranges, filter_cap;
@@ -1227,9 +1178,8 @@ Layout make_layout(int N, int D, int Ns, int workers) {
     L.merge_d = c.at<double>((size_t)N);
     L.cmd = c.at<unsigned long long>(32);         // own 256-byte line
     L.threshold = c.at<unsigned long long>(32);   // own 256-byte line
-    L.results = c.at<ResultSlot>(2 * 8 * ((size_t)workers + 1));
+    L.results = c.at<ResultSlot>(2 * (((size_t)workers + 1) << kSlotShift));
     L.error = c.at<int>(64);
-    L.trace = c.at<unsigned long long>((size_t)kTraceSteps * 16);
     L.ranges = (N + kJR - 1) / kJR;
     L.init_partial = c.at<Cand>((size_t)L.ranges * N);
     L.problem = c.at<Problem>(1);
@@ -1283,24 +1233,18 @@ int Solver::ensure_pool(int N, int D) {
     return grow_buffer(h_pool, h_pool_bytes, hneed, true);
 }
 
-// FA_AHC_* environment hooks (test / tuning only: fall-back placements at small N, trace, candidate spacing), read once.
+// FA_AHC_* environment hooks (tests only: fall-back placements and the float32 filter at small N), read once.
 struct Hooks {
     bool force_global = false, force_stream = false;
-    int slot_shift = 3, flags = 0;
     int filter_min_n = 2048;   // FA_AHC_FILTER_MIN_N: problems at least this large take the float32 filter (0 = never)
-    int filter_impl = 0;       // FA_AHC_FILTER_IMPL: bit 0 = 64 x 64 tiles in pass 1, bit 1 = dense pass 2 (A/B measurements)
 };
 static const Hooks &hooks() {
     static const Hooks h = [] {
         Hooks x;
         const char *g = std::getenv("FA_AHC_FORCE_GLOBAL_MASTER"), *s = std::getenv("FA_AHC_FORCE_STREAMED");
-        const char *sh = std::getenv("FA_AHC_SLOT_SHIFT"), *f = std::getenv("FA_AHC_FLAGS");
         x.force_global = g && g[0] == '1';
         x.force_stream = s && s[0] == '1';
-        if (sh) x.slot_shift = std::min(3, std::max(0, std::atoi(sh)));
-        if (f) x.flags = std::atoi(f);
         if (const char *m = std::getenv("FA_AHC_FILTER_MIN_N")) x.filter_min_n = std::atoi(m);
-        if (const char *m = std::getenv("FA_AHC_FILTER_IMPL")) x.filter_impl = std::atoi(m);
         return x;
     }();
     return h;
@@ -1371,15 +1315,12 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     P.cmd = reinterpret_cast<unsigned long long *>(base + L.cmd);
     P.threshold = reinterpret_cast<unsigned long long *>(base + L.threshold);
     P.results = reinterpret_cast<ResultSlot *>(base + L.results);
-    P.slot_shift = hk.slot_shift;   // tuning hook: 0 = packed, 1 = 32 B, 3 = 128 B per candidate (default)
-    P.result_stride = (max_workers + 1) << P.slot_shift;
+    P.result_stride = (max_workers + 1) << kSlotShift;
     P.error = reinterpret_cast<int *>(base + L.error);
-    P.trace = reinterpret_cast<unsigned long long *>(base + L.trace);
     P.resident = resident ? 1 : 0;
     P.slots_per_cta = slots_per_cta;
     P.idx16 = idx16 ? 1 : 0;
     P.smem_level = level;
-    P.flags = hk.flags;             // tuning hooks: 4 = globaltimer trace, 8 = never self-issue
     Cand *init_partial = reinterpret_cast<Cand *>(base + L.init_partial);
     Problem *d_prob = reinterpret_cast<Problem *>(base + L.problem);
 
@@ -1403,13 +1344,11 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
         cudaEvent_t &operator[](int i) { return e[i]; }
     } ev;
     for (int i = 0; i < 4; ++i) FA_CUDA_TRY(cudaEventCreate(&ev.e[i]));
-    auto drop_events = [&]() {};
 
     FA_CUDA_TRY(cudaMemsetAsync(base + L.cmd, 0, 256, stream));
     FA_CUDA_TRY(cudaMemsetAsync(base + L.threshold, 0, 256, stream));
-    FA_CUDA_TRY(cudaMemsetAsync(base + L.results, 0, 2 * 8 * sizeof(ResultSlot) * (size_t)(max_workers + 1), stream));
+    FA_CUDA_TRY(cudaMemsetAsync(base + L.results, 0, 2 * sizeof(ResultSlot) * ((size_t)(max_workers + 1) << kSlotShift), stream));
     FA_CUDA_TRY(cudaMemsetAsync(base + L.error, 0, 256, stream));
-    FA_CUDA_TRY(cudaMemsetAsync(base + L.trace, 0, sizeof(unsigned long long) * kTraceSteps * 16, stream));
     FA_CUDA_TRY(cudaEventRecord(ev[0], stream));
     {
         dim3 grid((Ns + 31) / 32, (D + 31) / 32), block(32, 8);
@@ -1447,18 +1386,14 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
         F.c2 = 2e-12;
         FA_CUDA_TRY(cudaMemsetAsync(F.counters, 0, 64 * sizeof(int), stream));
         ahc_filter_prep_kernel<<<(Ns + 127) / 128, 128, 0, stream>>>(P.cols, N, D, Ns, F);
-        const int nt = (N + kFT - 1) / kFT;
-        const unsigned tiles = (unsigned)((long long)nt * (nt + 1) / 2);
-        if (hk.filter_impl & 1) {
-            ahc_filter_tile_kernel<false><<<tiles, 256, 0, stream>>>(N, D, Ns, F);
-        } else {
-            const int nt2 = (N + kGT - 1) / kGT;
-            ahc_filter_tile128_kernel<<<(unsigned)((long long)nt2 * (nt2 + 1) / 2), 256, 0, stream>>>(N, D, Ns, F);
-        }
-        if (!(hk.filter_impl & 2) && F.tmin && (size_t)8 * D * sizeof(float) <= 48 * 1024)
+        const int nt2 = (N + kGT - 1) / kGT;
+        ahc_filter_tile128_kernel<<<(unsigned)((long long)nt2 * (nt2 + 1) / 2), 256, 0, stream>>>(N, D, Ns, F);
+        if (F.tmin && (size_t)8 * D * sizeof(float) <= 48 * 1024) {
             ahc_filter_rows_kernel<<<(N + 7) / 8, 256, (size_t)8 * D * sizeof(float), stream>>>(N, D, Ns, F);
-        else
-            ahc_filter_tile_kernel<true><<<tiles, 256, 0, stream>>>(N, D, Ns, F);
+        } else {
+            const unsigned tiles = (unsigned)((long long)F.nt * (F.nt + 1) / 2);
+            ahc_filter_dense_kernel<<<tiles, 256, 0, stream>>>(N, D, Ns, F);
+        }
         const unsigned cgrid = (unsigned)((F.cap + 255) / 256);
         ahc_filter_exact_kernel<<<cgrid, 256, 0, stream>>>(P.cols, D, Ns, F);
         ahc_filter_argmin_kernel<<<cgrid, 256, 0, stream>>>(F);
@@ -1480,7 +1415,6 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     FA_CUDA_TRY(cudaMemcpyAsync(h_err, P.error, sizeof(int), cudaMemcpyDeviceToHost, stream));
     FA_CUDA_TRY(cudaStreamSynchronize(stream));
     if (*h_err != 0) {
-        drop_events();
         fa::set_error("NaN distance between input vectors");
         return FA_RUNTIME_ERROR;   // reference: nan_error -> FASTCLUSTER_WRAPPER_RUNTIME_ERROR
     }
@@ -1521,36 +1455,10 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     FA_CUDA_TRY(cudaMemcpyAsync(h_md, P.merge_d, sizeof(double) * (N - 1), cudaMemcpyDeviceToHost, stream));
     FA_CUDA_TRY(cudaMemcpyAsync(h_err, P.error, sizeof(int), cudaMemcpyDeviceToHost, stream));
     FA_CUDA_TRY(cudaStreamSynchronize(stream));
-    cudaEventElapsedTime(&last_ms[0], ev[0], ev[1]);
-    cudaEventElapsedTime(&last_ms[1], ev[1], ev[2]);
-    cudaEventElapsedTime(&last_ms[2], ev[2], ev[3]);
-    cudaEventElapsedTime(&last_ms[3], ev[0], ev[3]);
-    for (int q = 0; q < 4; ++q) g_last_ms[q] = last_ms[q];
-    if ((P.flags & 4) && N > 2 * kTraceSteps + 8) {
-        std::vector<unsigned long long> tr((size_t)kTraceSteps * 16);
-        cudaMemcpy(tr.data(), P.trace, tr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-        double acc[16] = {0};
-        int used = 0;
-        for (int i = 1; i + 1 < kTraceSteps; ++i) {
-            const unsigned long long t0 = tr[(size_t)i * 16];
-            if (!t0) continue;
-            for (int q = 0; q < 16; ++q)
-                if (tr[(size_t)i * 16 + q]) acc[q] += (double)((long long)(tr[(size_t)i * 16 + q] - t0));
-            acc[0] += (double)((long long)(tr[(size_t)(i + 1) * 16] - t0));   // slot 0: step period
-            ++used;
-        }
-        for (int q = 0; q < 8; ++q) trace_avg_ns[q] = used ? acc[q] / used : 0.0;
-        const auto avg = [&](int q) { return used ? acc[q] / used : 0.0; };
-        std::fprintf(stderr,
-                     "[ahc trace] ns from the master's step start, mean of %d steps | period %.0f | master: bookkeeping+erase+"
-                     "path %.0f, candidates gathered %.0f, heap rotated %.0f | worker 0: round start %.0f, centroid built %.0f, "
-                     "scan done %.0f, warp reduce done %.0f, service warp at barrier %.0f / released %.0f, candidate published "
-                     "%.0f, all gathered %.0f, fence retired %.0f | slowest CTA: round start %.0f, candidate published %.0f",
-                     used, avg(0), avg(1), avg(2), avg(3), avg(4), avg(5), avg(6), avg(11), avg(13), avg(8), avg(7), avg(9),
-                     avg(10), avg(12), avg(14));
-        std::fprintf(stderr, "\n");
-    }
-    drop_events();
+    cudaEventElapsedTime(&g_last_ms[0], ev[0], ev[1]);
+    cudaEventElapsedTime(&g_last_ms[1], ev[1], ev[2]);
+    cudaEventElapsedTime(&g_last_ms[2], ev[2], ev[3]);
+    cudaEventElapsedTime(&g_last_ms[3], ev[0], ev[3]);
     if (*h_err != 0) {
         fa::set_error("NaN distance during merging");
         return FA_RUNTIME_ERROR;

@@ -23,6 +23,8 @@ struct ResultSlot {
     unsigned long long w0;
     unsigned long long w1;
 };
+// log2 of the distance (in slots) between two CTAs' candidates: every candidate in its own 128-byte line
+constexpr int kSlotShift = 3;
 
 // Everything the persistent kernel needs, resident in HBM.
 struct Problem {
@@ -45,18 +47,13 @@ struct Problem {
     unsigned long long *threshold;  // [2 parities][2 words] per-round self-issue threshold (master -> workers)
     ResultSlot *results;     // [2][result_stride]: per-CTA candidates, double-buffered by scan-round parity
     int result_stride;       // slots between the two parities
-    int slot_shift;          // log2 of the distance (in slots) between two CTAs' candidates
     int *error;              // 0 ok, 1 NaN distance (host-visible copy)
     int heap_size;           // after host heapify
     int idx16;               // heap index arrays are uint16_t and the master state lives in shared memory
     int smem_level;          // how much master state fits in smem: 1 = heap, 2 = + nn, 3 = + node_of
-    unsigned long long *trace;   // [kTraceSteps x 8] globaltimer stamps (flags bit 2), diagnostics only
-    int flags;               // bit 2: globaltimer trace; bit 3: never self-issue (every merge waits for the master)
     int resident;            // 1: every worker keeps its nodes' vectors in shared memory; 0: streamed from `cols`
     int slots_per_cta;       // resident mode: slots [w*slots_per_cta, (w+1)*slots_per_cta) belong to worker w
 };
-
-constexpr int kTraceSteps = 256;
 
 struct Solver {
     int num_sms = 0;
@@ -72,8 +69,6 @@ struct Solver {
     // pinned host mirrors
     void *h_pool = nullptr;
     size_t h_pool_bytes = 0;
-    float last_ms[4] = {0, 0, 0, 0};
-    double trace_avg_ns[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // mean offsets from "command published" (flags bit 2)   // init-nn, host heapify + copies, merge loop, total
 
     ~Solver();
     void release();

@@ -559,7 +559,6 @@ int MelPlan::init(const MelConfig &c) {
         // 0.2982 ms per audio-hour, identical output; profiles/r02_mel.md), so warp 0 only takes a group when the others
         // are this far ahead
         load[0] = 24;
-        if (const char *h = std::getenv("FA_MEL_ISSUE_HANDICAP")) load[0] = std::atoi(h);   // tuning hook (schedule only)
         for (int g : order) {
             int best = 0;
             for (int wv = 1; wv < kWarpsPerCta; ++wv)

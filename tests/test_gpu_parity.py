@@ -515,7 +515,7 @@ def test_linkage_float32_filter_is_bit_exact(gpu_lib, golden_dir, oracle):
     """The float32 GEMM-form filter of the initial nearest-neighbour pass (ahc_filter_*_kernel: rigorous error bound,
     exact chains only for candidates) forced on at every size (FA_AHC_FILTER_MIN_N=2): the reference's goldens — exact
     ties on a lattice, duplicates, a line — and fresh inputs incl. zero vectors, huge and non-finite values (which must
-    fall back to the exact pass and keep the reference's status codes) stay bit-identical."""
+    fall back to the exact pass and keep the reference's status codes) and rows wider than 1 536 stay bit-identical."""
     code = (
         "import sys, os, numpy as np; sys.path.insert(0, %r);"
         "from fluidaudio_b200 import clustering as cl; from oracle import oracle as O;"
@@ -527,6 +527,9 @@ def test_linkage_float32_filter_is_bit_exact(gpu_lib, golden_dir, oracle):
         " np.concatenate([np.zeros((5, 16)), rng.standard_normal((300, 16))]), rng.standard_normal((200, 16)) * 1e30]\n"
         "from fluidaudio_b200 import synth\n"
         "e, _ = synth.speaker_embeddings(3000, 256, 4, seed=2); cases.append(O.l2_normalize_rows(e.astype(np.float64)))\n"
+        # D > 1 536: a row no longer fits the row kernel's shared memory, so pass 2 is ahc_filter_dense_kernel
+        "w = np.random.default_rng(10)\n"
+        "cases += [w.standard_normal((300, 1600)), np.repeat(w.standard_normal((30, 1600)), 10, axis=0)[w.permutation(300)]]\n"
         "for x in cases:\n"
         "    st, z = cl.centroid_linkage(x); st2, z2 = O.centroid_linkage(x, use_ref=O.ref_available()); ok = ok and st == st2 and np.array_equal(z, z2)\n"
         "bad = rng.standard_normal((100, 8)); bad[50, 3] = np.nan\n"
