@@ -2,6 +2,7 @@
 // mono float32 at the model rate, written straight into the buffer the log-mel kernel reads (no host round trip).
 // See resample_plan.h for the reference lines and the filter design.
 #include "resample_plan.h"
+#include "resample_core.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -14,6 +15,7 @@ namespace resample {
 bool rational_ratio(double in_rate, double out_rate, long long &L, long long &M) {
     double scale = 1.0;
     if (std::fabs(in_rate - std::round(in_rate)) > 1e-9 || std::fabs(out_rate - std::round(out_rate)) > 1e-9) scale = 1000.0;
+    if (!(out_rate * scale < 0x1p53) || !(in_rate * scale < 0x1p53)) return false;   // past 2^53 the grid is not exact
     const long long a = (long long)std::llround(out_rate * scale), b = (long long)std::llround(in_rate * scale);
     if (a <= 0 || b <= 0) return false;
     const long long g = std::gcd(a, b);
@@ -37,6 +39,11 @@ int make_design(double in_rate, double out_rate, Design &d) {
     if (!(in_rate > 0) || !(out_rate > 0)) return FA_INVALID_ARGUMENT;
     if (!rational_ratio(in_rate, out_rate, d.L, d.M)) {
         fa::set_error("sample rates %.6f -> %.6f are not on a 1/1000 Hz grid", in_rate, out_rate);
+        return FA_UNSUPPORTED;
+    }
+    if (d.L >= (1LL << 32) || d.M >= (1LL << 32)) {   // sinc_kernel's phase arithmetic (resample_core.cuh)
+        fa::set_error("sample rates %.6f -> %.6f reduce to %lld/%lld: terms of 2^32 or more are not supported", in_rate,
+                      out_rate, d.L, d.M);
         return FA_UNSUPPORTED;
     }
     const double lower = std::min(1.0, (double)d.L / (double)d.M);
@@ -153,35 +160,41 @@ __global__ void __launch_bounds__(256) linear_kernel(Source s, double ratio, flo
 // Kaiser-windowed-sinc polyphase.  One CTA = 256 consecutive outputs; their input span (mixed down, widened) is staged
 // in shared memory once, every thread then runs its 2H-tap dot product out of shared memory: coefficients as 16-byte
 // loads through the read-only path (a single row when L == 1, i.e. integer decimation: every lane reads the same
-// address), four independent accumulators, 32-bit index arithmetic relative to one 64-bit division per CTA.
-__global__ void __launch_bounds__(256)
+// address), four independent accumulators, index arithmetic relative to one 64-bit division per CTA (resample_core.cuh).
+// Idx = unsigned when base_ph + 255 * M fits 32 bits (sinc_narrow_index: every whole-Hz pair of audio rates), else
+// unsigned long long.  Rows are padded to whole float4s, so when H is odd the last float4 holds two zero taps: they are
+// skipped, not multiplied, so that an output depends on its 2H-tap window only (0 * NaN would be NaN).
+template <typename Idx>
+__global__ void __launch_bounds__(kSincBlock)
 sinc_kernel(Source s, long long L, long long M, int half, int phases, int exact, int row_stride,
             const float *__restrict__ tab, float *out, long long o_begin, long long o_end) {
     extern __shared__ float xs[];
     __shared__ long long base_n0;
-    __shared__ unsigned base_ph;
-    const long long i0 = o_begin + (long long)blockIdx.x * 256;
+    __shared__ Idx base_ph;
+    const long long i0 = o_begin + (long long)blockIdx.x * kSincBlock;
     if (threadIdx.x == 0) {
-        const long long num = i0 * M;
-        base_n0 = num / L;
-        base_ph = (unsigned)(num - base_n0 * L);
+        long long n0;
+        unsigned long long ph;
+        sinc_cta_base(i0, L, M, n0, ph);
+        base_n0 = n0;
+        base_ph = (Idx)ph;
     }
     __syncthreads();
-    const unsigned uL = (unsigned)L, uM = (unsigned)M;   // L, M < 2^22 (rates on a 1/1000 Hz grid): 255 * M + L < 2^31
-    const int last = (int)(min(i0 + 255, o_end - 1) - i0);
+    const Idx uL = (Idx)L, uM = (Idx)M;
+    const int last = (int)(min(i0 + kSincBlock - 1, o_end - 1) - i0);
     const long long n_lo = base_n0 - half + 1;
-    const int span = (int)((base_ph + (unsigned)last * uM) / uL) + 2 * half;
-    for (int j = threadIdx.x; j < span + 4; j += 256) {
+    const int span = sinc_span<Idx>(base_ph, (unsigned)last, uL, uM, half);
+    for (int j = threadIdx.x; j < span; j += kSincBlock) {
         const long long n = n_lo + j;
-        xs[j] = (j < span && n >= 0 && n < s.frames) ? mono_at(s, n) : 0.0f;
+        xs[j] = (n >= 0 && n < s.frames) ? mono_at(s, n) : 0.0f;
     }
     __syncthreads();
     const long long i = i0 + threadIdx.x;
     if (i >= o_end) return;
-    const unsigned t = base_ph + threadIdx.x * uM;
-    const unsigned dn = t / uL, ph = t - dn * uL;
+    Idx dn, ph;
+    sinc_offset<Idx>(base_ph, threadIdx.x, uL, uM, dn, ph);
     const float *x = xs + dn;          // input n0 - H + 1 + k sits at xs[dn + k]
-    const int nq = row_stride >> 2;
+    const int nq = half >> 1;          // whole float4s of taps; with H odd two more taps follow in a padded float4
     float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f, a3 = 0.0f;
     if (exact) {
         const float4 *row = reinterpret_cast<const float4 *>(tab + (size_t)ph * row_stride);
@@ -193,11 +206,16 @@ sinc_kernel(Source s, long long L, long long M, int half, int phases, int exact,
             a2 = fmaf(c.z, x[4 * q + 2], a2);
             a3 = fmaf(c.w, x[4 * q + 3], a3);
         }
+        if (half & 1) {
+            const float4 c = __ldg(row + nq);
+            a0 = fmaf(c.x, x[4 * nq], a0);
+            a1 = fmaf(c.y, x[4 * nq + 1], a1);
+        }
     } else {
         const double pos = (double)ph / (double)L * (double)phases;
         const int p = (int)pos;
         const float a = (float)(pos - (double)p);
-        const float4 *r0 = reinterpret_cast<const float4 *>(tab + (size_t)p * row_stride), *r1 = r0 + nq;
+        const float4 *r0 = reinterpret_cast<const float4 *>(tab + (size_t)p * row_stride), *r1 = r0 + (row_stride >> 2);
 #pragma unroll 2
         for (int q = 0; q < nq; ++q) {
             const float4 c0 = __ldg(r0 + q), c1 = __ldg(r1 + q);
@@ -206,8 +224,24 @@ sinc_kernel(Source s, long long L, long long M, int half, int phases, int exact,
             a2 = fmaf(fmaf(a, c1.z - c0.z, c0.z), x[4 * q + 2], a2);
             a3 = fmaf(fmaf(a, c1.w - c0.w, c0.w), x[4 * q + 3], a3);
         }
+        if (half & 1) {
+            const float4 c0 = __ldg(r0 + nq), c1 = __ldg(r1 + nq);
+            a0 = fmaf(fmaf(a, c1.x - c0.x, c0.x), x[4 * nq], a0);
+            a1 = fmaf(fmaf(a, c1.y - c0.y, c0.y), x[4 * nq + 1], a1);
+        }
     }
     out[i] = (a0 + a1) + (a2 + a3);
+}
+
+template <typename Idx>
+static int launch_sinc(const Source &s, const Design &d, const float *d_tab, float *d_out, long long o_begin,
+                       long long o_end, unsigned grid, cudaStream_t stream) {
+    const size_t smem = sizeof(float) * (size_t)sinc_smem_floats(d.L, d.M, d.taps);
+    if (smem > 48 * 1024)
+        FA_CUDA_TRY(cudaFuncSetAttribute(sinc_kernel<Idx>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sinc_kernel<Idx><<<grid, kSincBlock, smem, stream>>>(s, d.L, d.M, d.half, d.phases, d.exact ? 1 : 0, d.row_stride,
+                                                          d_tab, d_out, o_begin, o_end);
+    return FA_OK;
 }
 
 int launch_convert(const void *d_pcm, long long frames, const AudioFormat &f, const Design &d, const float *d_tab,
@@ -220,11 +254,10 @@ int launch_convert(const void *d_pcm, long long frames, const AudioFormat &f, co
     } else if (resolve_algorithm(f) == kAlgoLinear) {
         linear_kernel<<<grid, 256, 0, stream>>>(s, f.in_rate / f.out_rate, d_out, o_begin, o_end);
     } else {
-        const size_t smem = sizeof(float) * (size_t)((255 * d.M) / d.L + d.taps + 12);
-        if (smem > 48 * 1024)
-            FA_CUDA_TRY(cudaFuncSetAttribute(sinc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        sinc_kernel<<<grid, 256, smem, stream>>>(s, d.L, d.M, d.half, d.phases, d.exact ? 1 : 0, d.row_stride, d_tab, d_out,
-                                                 o_begin, o_end);
+        const int st = sinc_narrow_index(d.L, d.M)
+                           ? launch_sinc<unsigned>(s, d, d_tab, d_out, o_begin, o_end, grid, stream)
+                           : launch_sinc<unsigned long long>(s, d, d_tab, d_out, o_begin, o_end, grid, stream);
+        if (st != FA_OK) return st;
     }
     FA_CUDA_TRY(cudaGetLastError());
     if (launches) ++*launches;

@@ -13,16 +13,25 @@
 // path IS in-repo arithmetic and is reproduced bit for bit (float32 operations individually rounded, the source
 // position in double).
 //
-// Filter design (oracle/oracle.py::sinc_design restates it in float64):
-//   ratio out/in = L/M in lowest terms (integer rates), fc = min(1, L/M) * kRolloff (1 = input Nyquist),
-//   H = ceil(kZeros / min(1, L/M)) input samples either side, taps = 2H,
+// Filter design (oracle/oracle.py::sinc_design / sinc_resample restate it in float64):
+//   ratio out/in = L/M in lowest terms: on the 1 Hz grid when both rates are whole, else on the 1/1000 Hz grid,
+//   fc = min(1, L/M) * kRolloff (1 = input Nyquist), H = ceil(kZeros / min(1, L/M)) input samples either side, taps = 2H,
 //   g(t) = fc * sinc(fc * t) * I0(beta * sqrt(1 - (t/H)^2)) / I0(beta),  |t| < H,
 //   row p (phase p/P of an input sample) holds g(k - p/P), k = -H+1 .. H, normalised to unit DC gain;
-//   P = L when L <= kMaxExactPhases (every output lands exactly on a row), otherwise P = kInterpPhases rows and the two
-//   neighbouring rows are blended linearly.
-//   y[i] = sum_k row[p(i)][k] * x[n0(i) - H + 1 + k],   n0 = floor(i * M / L),  phase = frac(i * M / L).
+//   P = L when L <= kMaxExactPhases (every output lands exactly on a row), otherwise P = kInterpPhases rows (+ 1 stored)
+//   blended linearly: pos = ph / L * P in double, p = (int)pos, a = (float)(pos - p), taps c_p + a (c_{p+1} - c_p).
+//   y[i] = sum_k row[p(i)][k] * x[n0(i) - H + 1 + k],   n0 = floor(i * M / L),  phase ph = (i * M) mod L.
 //   Samples outside [0, n) are zero (the converter's start-up / drain behaviour, without added latency: output i is
 //   centred on input time i * M / L).
+// Guarantees of make_design / sinc_kernel:
+//   * FA_UNSUPPORTED (with a message) for a rate off the 1/1000 Hz grid, a reduced term L or M >= 2^32, and a window
+//     that does not fit shared memory: (255 M / L + 2H + 8) floats > 200 KB, i.e. decimation by more than 168.
+//   * phases exact for every accepted (L, M) and any output index (resample_core.cuh; 32-bit offsets when
+//     255 M + L < 2^32, 64-bit otherwise).
+//   * output i depends on its 2H-tap window only: a NaN / Inf input makes exactly the outputs whose window holds it
+//     non-finite (rows are padded to whole float4s; the padding is never multiplied).
+//   * error bar against the float64 evaluation, per output: (taps/4 + 6) * 2^-24 * sum_k A_k |x_k|, A_k = |g_k|, or
+//     |g_{p,k}| + |g_{p+1,k}| where two rows are blended (four FMA chains, two adds, float32 taps, the blend).
 #pragma once
 
 #include "fa_common.cuh"
@@ -61,7 +70,7 @@ struct Design {
     std::vector<float> table; // [(exact ? P : P + 1) x row_stride]
 };
 
-// out/in reduced to L/M when both rates are integers (in Hz) — otherwise a 1/1000 Hz grid
+// out/in reduced to L/M on the 1 Hz grid when both rates are whole, otherwise on the 1/1000 Hz grid (false: off grid)
 bool rational_ratio(double in_rate, double out_rate, long long &L, long long &M);
 int make_design(double in_rate, double out_rate, Design &d);
 long long output_count(long long frames, double in_rate, double out_rate);   // Int(Double(n) / (in / out))

@@ -16,6 +16,7 @@ import ctypes as C
 import os
 import subprocess
 from dataclasses import dataclass
+from typing import NamedTuple
 
 import numpy as np
 
@@ -264,20 +265,88 @@ def resample_output_count(frames: int, in_rate: float, out_rate: float) -> int:
     return int(frames) if in_rate == out_rate else int(float(frames) / (in_rate / out_rate))
 
 
-def sinc_design(in_rate: float, out_rate: float):
-    """Returns (L, M, half, fc): out/in = L/M, half = taps / 2, fc relative to the input Nyquist."""
+SINC_MAX_EXACT_PHASES, SINC_INTERP_PHASES = 2048, 1024
+SINC_SMEM_BYTES = 200 * 1024          # make_design's bound on one CTA's staged window (255 M / L + 2H + 8 floats)
+
+
+class SincDesign(NamedTuple):
+    """unpacks as (L, M, half, fc)"""
+    L: int            # out / in = L / M in lowest terms
+    M: int
+    half: int         # H: taps = 2H
+    fc: float         # cut-off relative to the input Nyquist
+
+    @property
+    def exact(self) -> bool:      # L <= 2048: every output lands on one of the L rows
+        return self.L <= SINC_MAX_EXACT_PHASES
+
+    @property
+    def phases(self) -> int:      # P: L rows when exact, else 1024 (+ 1 stored row) blended linearly
+        return self.L if self.exact else SINC_INTERP_PHASES
+
+
+def _llround(x: float) -> int:
+    """std::llround of a finite double: nearest integer, halves away from zero."""
+    i = int(x)
+    f = x - i
+    return i + (1 if f >= 0.5 else -1 if f <= -0.5 else 0)
+
+
+def rational_ratio(in_rate: float, out_rate: float):
+    """resample_kernels.cu rational_ratio: (L, M) with out/in = L/M in lowest terms, on the whole-Hz grid when both rates
+    are whole, else on the 1/1000 Hz grid; None when a rate is not on that grid."""
     from math import gcd
-    a, b = int(round(out_rate)), int(round(in_rate))
+    scale = 1.0
+    if abs(in_rate - _llround(in_rate)) > 1e-9 or abs(out_rate - _llround(out_rate)) > 1e-9:
+        scale = 1000.0
+    if not (out_rate * scale < 2.0 ** 53 and in_rate * scale < 2.0 ** 53):
+        return None
+    a, b = _llround(out_rate * scale), _llround(in_rate * scale)
+    if a <= 0 or b <= 0:
+        return None
+    if not (abs(a / scale - out_rate) < 1e-6 and abs(b / scale - in_rate) < 1e-6):
+        return None
     g = gcd(a, b)
-    L, M = a // g, b // g
+    return a // g, b // g
+
+
+def sinc_design(in_rate: float, out_rate: float) -> SincDesign:
+    """resample_kernels.cu make_design without the table; raises ValueError where make_design returns FA_UNSUPPORTED
+    (off the rate grid, L or M of 2^32 or more, a window larger than the shared-memory bound)."""
+    if not (in_rate > 0 and out_rate > 0):
+        raise ValueError("sample rates must be positive")
+    r = rational_ratio(in_rate, out_rate)
+    if r is None:
+        raise ValueError(f"sample rates {in_rate} -> {out_rate} are not on a 1/1000 Hz grid")
+    L, M = r
+    if L >= 2 ** 32 or M >= 2 ** 32:
+        raise ValueError(f"{in_rate} -> {out_rate} reduces to {L}/{M}: terms of 2^32 or more")
     lower = min(1.0, L / M)
-    return L, M, int(np.ceil(SINC_ZEROS / lower)), lower * SINC_ROLLOFF
+    half = int(np.ceil(SINC_ZEROS / lower))
+    if (255.0 * M / L + 2 * half + 8) * 4 > SINC_SMEM_BYTES:
+        raise ValueError(f"ratio {L}/{M} needs a filter window larger than shared memory")
+    return SincDesign(L, M, half, lower * SINC_ROLLOFF)
+
+
+def sinc_positions(count: int, L: int, M: int):
+    """n0 = floor(i M / L) and the phase (i M) mod L of outputs 0 .. count-1, exact for every L, M < 2^32."""
+    i = np.arange(count, dtype=np.uint64)
+    L, M = np.uint64(L), np.uint64(M)
+    q, rm = i // L, (i % L) * M
+    return (q * M + rm // L).astype(np.int64), rm % L
 
 
 def _sinc_kernel(t: np.ndarray, half: int, fc: float) -> np.ndarray:
     u = np.clip(1.0 - (t / half) ** 2, 0.0, None)
     g = fc * np.sinc(fc * t) * np.i0(SINC_BETA * np.sqrt(u)) / np.i0(SINC_BETA)
     return np.where(np.abs(t) < half, g, 0.0)
+
+
+def _sinc_rows(d: SincDesign, frac: np.ndarray) -> np.ndarray:
+    """rows g(k - frac), k = -H+1 .. H, in float64, each normalised to unit DC gain"""
+    k = np.arange(-d.half + 1, d.half + 1)
+    rows = _sinc_kernel(k[None, :] - np.asarray(frac, np.float64)[:, None], d.half, d.fc)
+    return rows / rows.sum(axis=1, keepdims=True)
 
 
 def mixdown(pcm: np.ndarray) -> np.ndarray:
@@ -295,28 +364,54 @@ def mixdown(pcm: np.ndarray) -> np.ndarray:
     return s if x.shape[0] == 1 else (s * np.float32(1.0 / np.float32(x.shape[0]))).astype(np.float32)
 
 
-def sinc_resample(mono: np.ndarray, in_rate: float, out_rate: float) -> np.ndarray:
-    """float64 evaluation of the documented polyphase filter on a mono float32 signal (rows normalised to unit DC gain
-    exactly as the library's float32 table is, so the only difference left is float32 rounding of taps and sums)."""
+def sinc_resample(mono: np.ndarray, in_rate: float, out_rate: float, with_magnitude: bool = False,
+                  exact_phase: bool = False):
+    """float64 evaluation of the documented polyphase filter on a mono float32 signal, rows normalised to unit DC gain
+    exactly as the library's float32 table is.  Exact path (L <= 2048): output i applies row (i M) mod L.  Interpolated
+    path: pos = ph / L * 1024 in double, p = int(pos), a = float32(pos - p), and the taps are r_p + a (r_{p+1} - r_p)
+    of the float64 rows p and p + 1, the blend the kernel performs, so the interpolation is part of the specification.
+
+    with_magnitude: also returns S_i = sum_k A_k |x_k| (float64), A_k = |g_k| on the exact path and |g_{p,k}| + |g_{p+1,k}|
+    on the interpolated one: the scale of output i's float32 rounding error.  exact_phase: evaluate every output at its
+    exact phase instead (a float64 yardstick for the interpolation itself)."""
     x = np.asarray(mono, np.float32).astype(np.float64)
     n = x.size
     count = resample_output_count(n, in_rate, out_rate)
     if in_rate == out_rate:
-        return x.astype(np.float32)
-    L, M, half, fc = sinc_design(in_rate, out_rate)
-    xp = np.concatenate([np.zeros(half), x, np.zeros(half + 2)])
-    out = np.zeros(count)
-    k = np.arange(-half + 1, half + 1)
-    i = np.arange(count, dtype=np.int64)
-    n0 = (i * M) // L
-    ph = (i * M) % L
-    for p in np.unique(ph):
-        sel = np.nonzero(ph == p)[0]
-        row = _sinc_kernel(k - p / L, half, fc)
-        row = row / row.sum()
-        idx = n0[sel][:, None] + k[None, :] + half
-        out[sel] = (xp[idx] * row[None, :]).sum(axis=1)
-    return out.astype(np.float32)
+        return (x.astype(np.float32), np.abs(x)) if with_magnitude else x.astype(np.float32)
+    d = sinc_design(in_rate, out_rate)
+    taps = 2 * d.half
+    n0, ph = sinc_positions(count, d.L, d.M)
+    xp = np.concatenate([np.zeros(d.half), x, np.zeros(d.half + 2)])   # x[n] at xp[n + H]
+    out, mag = np.zeros(count), np.zeros(count)
+    if exact_phase:
+        table = None
+    elif d.exact:
+        table = _sinc_rows(d, np.arange(d.L) / d.L)
+    else:
+        table = _sinc_rows(d, np.arange(d.phases + 1) / d.phases)
+    step = max(1, (1 << 21) // taps)   # outputs per block: bounds the [outputs x taps] temporaries
+    for b in range(0, count, step):
+        sl = slice(b, min(count, b + step))
+        win = xp[n0[sl, None] + np.arange(1, taps + 1)[None, :]]      # inputs n0 - H + 1 .. n0 + H
+        if exact_phase:
+            g = _sinc_rows(d, ph[sl].astype(np.float64) / d.L)
+            a_k = np.abs(g)
+        elif d.exact:
+            g = table[ph[sl].astype(np.int64)]
+            a_k = np.abs(g)
+        else:
+            pos = ph[sl].astype(np.float64) / float(d.L) * float(d.phases)
+            p = pos.astype(np.int64)
+            a = (pos - p).astype(np.float32).astype(np.float64)
+            r0, r1 = table[p], table[p + 1]
+            g = r0 + a[:, None] * (r1 - r0)
+            a_k = np.abs(r0) + np.abs(r1)
+        out[sl] = (win * g).sum(axis=1)
+        if with_magnitude:
+            mag[sl] = (np.abs(win) * a_k).sum(axis=1)
+    y = out.astype(np.float32)
+    return (y, mag) if with_magnitude else y
 
 
 # ------------------------------------------------------------------------------------------------ clustering

@@ -31,6 +31,14 @@ conv.resample(st[0][:22050], 22050)
 conv.resample_buffer(np.round(st * 32767).astype(np.int16), 44100)
 conv.resample_buffer(np.stack([st[0], st[1], st[0], st[1]])[:, :8000], 8000)
 conv.resample_buffer(st[:, :16000], 16000)
+# sinc: 32-bit phases on the interpolated path, 64-bit phases (44100.001 Hz), the largest accepted ratio (opt-in shared
+# memory), an odd H (padded rows) with a non-finite sample
+conv.resample(st[0][:16001], 16001)
+conv.resample(st[0][:44100], 44100.001)
+conv.resample(np.tile(st[0], 4)[:16000 * 168 // 4], 16000 * 168)
+nan_in = st[0][:8820].copy()
+nan_in[4000] = np.nan
+conv.resample(nan_in, 44100)
 m.compute_from_pcm(np.ascontiguousarray(np.round(st.T * 32767).astype(np.int16)), 48000, interleaved=True)
 m.compute_from_pcm(np.round(st[0] * 32767).astype(np.int16)[:16000], 16000)
 UnifiedMelExtractor(24000).features(np.concatenate([a[:20000], np.zeros(4000, np.float32)]), 20000)

@@ -301,6 +301,64 @@ def test_kernel_lane_math_matches_oracle(tmp_path, oracle):
     print("largest |d log-mel| vs the oracle:", worst)
 
 
+def test_sinc_kernel_index_math_is_exact(tmp_path, oracle):
+    """resample_core.cuh (the per-CTA and per-thread index arithmetic of sinc_kernel) on the host: for the extreme ratios
+    make_design accepts, every thread of CTAs at the start, the middle (aligned and not: the fused pipeline launches at any
+    output) and the end of an hour-long output gets n0 = floor(i M / L) and phase (i M) mod L exactly, in the index width
+    the kernel selects; the staged span covers every tap any thread reads and fits the shared memory the launch asks for.
+    32-bit offsets are shown to be wrong where the kernel must not select them (44100.001 Hz: L = 16e6, M = 44 100 001)."""
+    L_ = _compile("resample_emul.cpp", str(tmp_path / "libresample_emul.so"))
+    i64p = np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS")
+    L_.resample_index.argtypes = [C.c_longlong, C.c_longlong, C.c_int, C.c_longlong, C.c_int, C.c_int, i64p, i64p, i64p,
+                                  i64p]
+    L_.resample_narrow.argtypes = [C.c_longlong, C.c_longlong]
+    L_.resample_smem_floats.argtypes = [C.c_longlong, C.c_longlong, C.c_int]
+    L_.resample_smem_floats.restype = C.c_longlong
+
+    def run(d, i0, count, wide):
+        n0, ph, dn, span = (np.zeros(count, np.int64), np.zeros(count, np.int64), np.zeros(count, np.int64),
+                            np.zeros(1, np.int64))
+        assert L_.resample_index(d.L, d.M, d.half, i0, count, int(wide), n0, ph, dn, span) == 0
+        return n0, ph, dn, int(span[0])
+
+    def exact(d, i0, count):
+        return ([(i0 + j) * d.M // d.L for j in range(count)], [(i0 + j) * d.M % d.L for j in range(count)])
+
+    down = 1                    # the largest decimation ratio make_design accepts (window bound); upsampling keeps H = 24
+    while True:
+        try:
+            oracle.sinc_design(16000 * (down + 1), 16000)
+        except ValueError:
+            break
+        down += 1
+    assert down == 168
+    pairs = [(16000 * down, 16000), (16000 * down - 0.001, 16000), (1000, 4000000.001), (44100, 16000), (44100.5, 16000),
+             (44100.001, 16000), (48000.001, 16000), (47999.998, 16000), (16001, 16000), (8000.1, 16000),
+             (16000, 192000.001), (4000000.003, 4000000.001)]
+    selected = {}
+    for rin, rout in pairs:
+        d = oracle.sinc_design(rin, rout)
+        wide = not L_.resample_narrow(d.L, d.M)
+        selected[(rin, rout)] = "64" if wide else "32"
+        assert wide == (255 * d.M + d.L >= 2 ** 32)
+        taps, smem = 2 * d.half, L_.resample_smem_floats(d.L, d.M, 2 * d.half)
+        count = oracle.resample_output_count(int(round(rin * 3600)), rin, rout)
+        mid = count // 2 // 256 * 256
+        for i0, n in ((0, 256), (mid, 256), (mid + 77, 256), ((count - 1) // 256 * 256, count - (count - 1) // 256 * 256)):
+            n0, ph, dn, span = run(d, i0, n, wide)
+            e_n0, e_ph = exact(d, i0, n)
+            assert n0.tolist() == e_n0 and ph.tolist() == e_ph, (rin, rout, i0)
+            assert dn[0] == 0 and (dn + taps).max() <= span <= smem, (rin, rout, i0, span, smem)
+    # the parent's 32-bit arithmetic at 44100.001 Hz: most threads of a CTA read the wrong window at the wrong phase
+    d = oracle.sinc_design(44100.001, 16000)
+    n0, ph, _, _ = run(d, 256 * 1000, 256, False)
+    e_n0, e_ph = exact(d, 256 * 1000, 256)
+    assert (n0 != np.array(e_n0)).sum() > 100 and selected[(44100.001, 16000)] == "64"
+    assert selected[(44100, 16000)] == selected[(16000 * down, 16000)] == selected[(16000, 192000.001)] == "32"
+    # i0 * M passes 2^63 within the hour at 4 MHz: the split form keeps n0 exact (checked above)
+    assert (count - 1) * 4000000003 >= 2 ** 63
+
+
 def test_merge_control_plane_matches_reference_goldens(tmp_path, golden_dir, oracle):
     """ahc_core.cuh (slot-indexed heap + live bitmap, the code the device master warp runs) driven on the host in the
     merge kernel's order: dendrograms must equal the reference's bit for bit."""

@@ -576,6 +576,45 @@ def test_resampler_spec_and_reference_length_contract(oracle):
     assert lin.size == 333 and np.abs(lin - m[::3][:333]).max() < 1e-6
 
 
+def test_resampler_design_restates_the_rate_grid(oracle):
+    """sinc_design restates make_design's rational_ratio: whole-Hz rates reduce on the 1 Hz grid, any other rate on the
+    1/1000 Hz grid (44100.001 Hz -> 16 kHz is 16 000 000 / 44 100 001, whose phases overflow 32 bits), off-grid rates are
+    rejected, and so are ratios whose window passes the shared-memory bound."""
+    cases = {(44100, 16000): (160, 441, 67, True, 160), (44100.5, 16000): (32000, 88201, 67, False, 1024),
+             (44100.001, 16000): (16000000, 44100001, 67, False, 1024), (48000, 16000): (1, 3, 72, True, 1),
+             (16001, 16000): (16000, 16001, 25, False, 1024), (8000, 44100): (441, 80, 24, True, 441),
+             (47999.998, 16000): (8000000, 23999999, 72, False, 1024)}
+    for (rin, rout), want in cases.items():
+        d = oracle.sinc_design(rin, rout)
+        assert (d.L, d.M, d.half, d.exact, d.phases) == want, (rin, rout, d)
+    for rin in (44100.0004, 16000.0005, 0.0, -8000.0):
+        with pytest.raises(ValueError):
+            oracle.sinc_design(rin, 16000)
+    oracle.sinc_design(16000 * 168, 16000)
+    with pytest.raises(ValueError):
+        oracle.sinc_design(16000 * 169, 16000)
+    # positions exact where i * M passes 2^63: i = 3e11 outputs at M = 4e9 + 3
+    L, M = 4000000001, 4000000003
+    n0, ph = oracle.sinc_positions(10, L, M)
+    assert n0.tolist() == [i * M // L for i in range(10)] and ph.tolist() == [i * M % L for i in range(10)]
+
+
+def test_interpolated_phases_stay_close_to_the_exact_phase_filter(oracle):
+    """16001 Hz -> 16 kHz takes the interpolated path (L = 16000 > 2048): rows at 1024 phases blended linearly.  That blend
+    is specified, so the oracle evaluates it; here it is held against the same filter evaluated at every output's exact
+    phase.  Measured: 8.3e-7 of full scale on unit-amplitude noise (a bar of 2e-6): the interpolation error the design
+    accepts, which an oracle without the blend would have to absorb into the GPU tolerance."""
+    x = np.random.default_rng(3).uniform(-1, 1, 6000).astype(np.float32)
+    y, mag = oracle.sinc_resample(x, 16001, 16000, with_magnitude=True)
+    ref = oracle.sinc_resample(x, 16001, 16000, exact_phase=True)
+    gap = np.abs(y.astype(np.float64) - ref).max()
+    assert 0 < gap <= 2e-6, gap
+    # on the exact path the blend is not used: both evaluations are the same
+    x = x[:4410]
+    assert np.array_equal(oracle.sinc_resample(x, 44100, 16000), oracle.sinc_resample(x, 44100, 16000, exact_phase=True))
+    assert np.all(mag > 0)
+
+
 def test_timed_cpu_arm_matches_the_oracle(oracle):
     """oracle_mel_fast.cpp — the float32-FFT, SIMD-across-frames CPU implementation bench.py times as the reference arm —
     agrees with the parity oracle within the spread of two float32 FFTs (2e-4), frame counts exact."""
