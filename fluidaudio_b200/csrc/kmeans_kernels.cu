@@ -321,8 +321,12 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
         FA_CUDA_TRY(cudaGetLastError());
         FA_CUDA_TRY(cudaMemcpyAsync(&h, d_state, sizeof(RunState), cudaMemcpyDeviceToHost, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));
-        if (runs == 1 || h.inertia < best) {                  // :122-125: strictly lower inertia wins
-            best = h.inertia;
+        // :122-125: strictly lower inertia wins.  Run 0 (the base seed) is always taken first, so a NaN inertia in every
+        // run (a NaN row makes every distance NaN) returns the base-seed run; a later run beats it only by comparing
+        // below `best`, which a NaN inertia never lowers.
+        const bool better = h.inertia < best;
+        if (run == 0 || better) {
+            if (better) best = h.inertia;
             FA_CUDA_TRY(cudaMemcpyAsync(d_labels, final_labels, sizeof(int) * N, cudaMemcpyDeviceToDevice, s));
             FA_CUDA_TRY(cudaMemcpyAsync(d_centroids, d_cent, sizeof(double) * (size_t)k * D, cudaMemcpyDeviceToDevice, s));
             if (best_init) *best_init = run;

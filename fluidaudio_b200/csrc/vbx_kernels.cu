@@ -339,8 +339,12 @@ __global__ void __launch_bounds__(kEThreads) vbx_partials0_kernel(Dev d) {
 }
 
 // closing == 1: only the pi / ELBO bookkeeping of the last E-step (after max_iterations launches)
+// Convergence: the launch that finds it stores its own `it` (>= 2) in state[0], which turns every later kernel into a
+// no-op.  This kernel's S CTAs test it at entry, so they skip only when an EARLIER launch converged: a CTA of the
+// converging launch that starts after CTA 0's store must still write its pi.
 __global__ void __launch_bounds__(kEThreads) vbx_update_kernel2(Dev d, int it, int closing) {
-    if (d.state[0]) return;   // converged in an earlier launch
+    const int conv = d.state[0];
+    if (conv && conv < it) return;   // converged in an earlier launch
     __shared__ double pi_sh[kFusedMaxS];
     __shared__ double red[kEThreads];
     __shared__ double scal[4];
@@ -396,7 +400,7 @@ __global__ void __launch_bounds__(kEThreads) vbx_update_kernel2(Dev d, int it, i
         if (s == 0) {
             d.elbos[it - 1] = scal[1];
             d.state[1] = it;
-            if (done_sh && !closing) d.state[0] = 1;
+            if (done_sh && !closing) d.state[0] = it;
         }
     }
     if (done_sh || closing) return;

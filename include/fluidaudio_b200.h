@@ -355,6 +355,7 @@ fa_status fa_build_speaker_database(const int32_t *seg_cluster, int32_t segment_
 /* KMeansClustering.clusterWithCentroidsNInit (Diarizer/Offline/Clustering/KMeansClustering.swift:39-130) on raw
  * embeddings [N x D]: labels [N], centroids (normalised space) [min(num_clusters, N) x D] -> *centroid_rows rows;
  * *best_init = index of the winning seed.  n_init <= 1 runs the single seeded clustering (:39-92).
+ * A NaN or Inf in a row makes the inertia of every run NaN: the base-seed run is then returned (*best_init = 0).
  * fa_speaker_constraints_resolve = SpeakerCountConstraints.resolve (SpeakerCountConstraints.swift:27-71);
  * FA_NO_VALUE = nil. */
 fa_status fa_kmeans_cluster(const double *embeddings, size_t N, size_t D, int32_t num_clusters, int32_t max_iterations,

@@ -8,6 +8,7 @@ The product package ``fluidaudio_b200`` must never import this module (tests enf
 Pipeline glue restated here (pure Python, O(N)):
   * ``ahc_cluster``      AHCClustering.cluster            AHCClustering.swift:20-67
   * ``vbx_refine``       VBxClustering.refine             VBxClustering.swift:41-165
+                         (``vbx_step``: one EM iteration of it, from a given gamma and pi)
   * ``diarize_cluster``  OfflineDiarizerManager.cluster   OfflineDiarizerManager.swift:270-384 (+591-611)
 """
 from __future__ import annotations
@@ -87,6 +88,9 @@ def lib():
         L.oracle_vbx_refine.argtypes = [_f64p, C.c_int64, C.c_int64, _f64p, C.c_int64, C.c_void_p,
                                         C.POINTER(VbxConfig), C.c_int32, _f64p, _f64p, _f64p, _i32p]
         L.oracle_vbx_refine.restype = C.c_int32
+        L.oracle_vbx_step.argtypes = [_f64p, C.c_int64, C.c_int64, _f64p, _f64p, _f64p, C.c_int32, C.c_double,
+                                      C.c_double, _f64p, _f64p]
+        L.oracle_vbx_step.restype = C.c_double
         L.oracle_compute_centroids.argtypes = [_f64p, C.c_int64, C.c_int64, _f64p, _f64p, C.c_int32, _f64p, _i32p]
         L.oracle_compute_centroids.restype = C.c_int32
         L.oracle_centroids_from_clusters.argtypes = [_f64p, C.c_int64, C.c_int64, _i32p, _f64p, C.c_int32]
@@ -471,7 +475,8 @@ class VBxOutput:
 
 
 def vbx_refine(rho: np.ndarray, psi: np.ndarray, initial: np.ndarray, Fa=0.07, Fb=0.8, max_iterations=20,
-               epsilon=1e-4, init_smoothing=7.0) -> VBxOutput:
+               epsilon=1e-4, init_smoothing=7.0, speakers: int | None = None) -> VBxOutput:
+    """``speakers`` overrides the speaker count S (the number of distinct initial labels), as the C ABI allows."""
     rho = np.ascontiguousarray(rho, np.float64)
     T = rho.shape[0]
     if T == 0 or rho.ndim < 2 or rho.shape[1] == 0:
@@ -479,7 +484,7 @@ def vbx_refine(rho: np.ndarray, psi: np.ndarray, initial: np.ndarray, Fa=0.07, F
     D = rho.shape[1]
     psi = np.ascontiguousarray(psi, np.float64)
     initial = np.ascontiguousarray(initial, np.int32)
-    S = max(1, len(set(initial.tolist())))
+    S = max(1, len(set(initial.tolist()))) if speakers is None else int(speakers)
     gamma = np.zeros((T, S), np.float64)
     pi = np.zeros(S, np.float64)
     elbos = np.zeros(max(max_iterations, 1), np.float64)
@@ -489,6 +494,23 @@ def vbx_refine(rho: np.ndarray, psi: np.ndarray, initial: np.ndarray, Fa=0.07, F
     iters = lib().oracle_vbx_refine(rho, T, D, psi if psi.size else np.zeros(1), psi.size, init_ptr, C.byref(cfg), S,
                                     gamma, pi, elbos, hard)
     return VBxOutput(gamma, pi, hard, S, elbos[:iters].copy())
+
+
+def vbx_step(rho: np.ndarray, psi: np.ndarray, gamma: np.ndarray, pi: np.ndarray, Fa=0.07, Fb=0.8):
+    """One EM iteration of ``vbx_refine`` from (gamma, pi): (gamma', pi', ELBO of the iteration).  ``psi`` of the
+    wrong length is the identity, as in ``vbx_refine``."""
+    rho = np.ascontiguousarray(rho, np.float64)
+    T, D = rho.shape
+    psi = np.ascontiguousarray(psi, np.float64)
+    phi = psi if psi.size == D else np.ones(D)
+    gamma = np.ascontiguousarray(gamma, np.float64)
+    pi = np.ascontiguousarray(pi, np.float64)
+    S = pi.size
+    assert gamma.shape == (T, S)
+    g_out = np.zeros((T, S), np.float64)
+    p_out = np.zeros(S, np.float64)
+    elbo = lib().oracle_vbx_step(rho, T, D, phi, gamma, pi, S, Fa, Fb, g_out, p_out)
+    return g_out, p_out, float(elbo)
 
 
 def compute_centroids(train: np.ndarray, vbx: VBxOutput, initial: np.ndarray) -> np.ndarray:

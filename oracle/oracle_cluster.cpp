@@ -317,6 +317,96 @@ struct oracle_vbx_config {
     double init_smoothing;  // 7.0
 };
 
+// One EM iteration of refine (:239-282 for rho and G, :304-661 for the step): from (gamma_in, pi_in) to (gamma_out,
+// pi_out), returning the iteration's ELBO.  features: T x D row-major, phi: D (unclamped psi).  The outputs may alias
+// the inputs; every read of gamma_in and pi_in happens before the first write.
+double oracle_vbx_step(const double *features, int64_t T, int64_t D, const double *phi, const double *gamma_in,
+                       const double *pi_in, int32_t S, double Fa, double Fb, double *gamma_out, double *pi_out) {
+    std::vector<double> phic(D), sq(D);
+    for (int64_t d = 0; d < D; ++d) {
+        phic[d] = std::max(phi[d], 1e-12);
+        sq[d] = std::sqrt(phic[d]);
+    }
+    std::vector<double> rho((size_t)T * D), G(T);
+    const double log_const = (double)D * std::log(2.0 * M_PI);
+    for (int64_t t = 0; t < T; ++t) {
+        double ss = 0;
+        for (int64_t d = 0; d < D; ++d) {
+            rho[t * D + d] = features[t * D + d] * sq[d];
+            ss += features[t * D + d] * features[t * D + d];
+        }
+        G[t] = -0.5 * (ss + log_const);
+    }
+    const double ratio = Fa / Fb;
+    std::vector<double> invL((size_t)S * D), alpha((size_t)S * D), gsum(S), phiTerm(S), logP((size_t)T * S), logPi(S),
+        row(S);
+    for (int s = 0; s < S; ++s) gsum[s] = 0;
+    for (int64_t t = 0; t < T; ++t)
+        for (int s = 0; s < S; ++s) gsum[s] += gamma_in[t * S + s];
+    for (int s = 0; s < S; ++s) {
+        const double w = ratio * gsum[s];
+        for (int64_t d = 0; d < D; ++d) invL[s * D + d] = 1.0 / std::max(1.0 + w * phic[d], 1e-12);
+    }
+    // temp = gamma^T rho  (S x D), then alpha = ratio * invL .* temp
+    std::fill(alpha.begin(), alpha.end(), 0.0);
+    for (int64_t t = 0; t < T; ++t)
+        for (int s = 0; s < S; ++s) {
+            const double g = gamma_in[t * S + s];
+            for (int64_t d = 0; d < D; ++d) alpha[s * D + d] += g * rho[t * D + d];
+        }
+    for (size_t i = 0; i < alpha.size(); ++i) alpha[i] = (alpha[i] * invL[i]) * ratio;
+    for (int s = 0; s < S; ++s) {
+        double sum = 0;
+        for (int64_t d = 0; d < D; ++d) sum += (alpha[s * D + d] * alpha[s * D + d] + invL[s * D + d]) * phic[d];
+        phiTerm[s] = sum;
+    }
+    for (int64_t t = 0; t < T; ++t)
+        for (int s = 0; s < S; ++s) {
+            double acc = 0;
+            for (int64_t d = 0; d < D; ++d) acc += rho[t * D + d] * alpha[s * D + d];
+            logP[t * S + s] = ((acc + (-0.5 * phiTerm[s])) + G[t]) * Fa;
+        }
+    for (int s = 0; s < S; ++s) logPi[s] = std::log(std::max(pi_in[s], 1e-8));
+    double ll = 0;
+    for (int64_t t = 0; t < T; ++t) {
+        double mx = -std::numeric_limits<double>::max();
+        for (int s = 0; s < S; ++s) {
+            row[s] = logP[t * S + s] + logPi[s];
+            mx = std::max(mx, row[s]);
+        }
+        double sum = 0;
+        for (int s = 0; s < S; ++s) {
+            row[s] = std::exp(row[s] - mx);
+            sum += row[s];
+        }
+        double *g = gamma_out + t * S;
+        if (sum <= 0.0 || !std::isfinite(sum)) {
+            for (int s = 0; s < S; ++s) g[s] = 1.0 / (double)S;
+            ll += mx;
+        } else {
+            const double inv = 1.0 / sum;
+            for (int s = 0; s < S; ++s) g[s] = row[s] * inv;
+            ll += mx + std::log(sum);
+        }
+    }
+    for (int s = 0; s < S; ++s) pi_out[s] = 0;
+    for (int64_t t = 0; t < T; ++t)
+        for (int s = 0; s < S; ++s) pi_out[s] += gamma_out[t * S + s];
+    double ps = 0;
+    for (int s = 0; s < S; ++s) ps += pi_out[s];
+    if (ps > 0.0 && std::isfinite(ps)) {
+        const double inv = 1.0 / ps;
+        for (int s = 0; s < S; ++s) pi_out[s] *= inv;
+    } else for (int s = 0; s < S; ++s) pi_out[s] = 1.0 / (double)S;
+    double sLog = 0, sInv = 0, sA2 = 0;
+    for (size_t i = 0; i < invL.size(); ++i) {
+        sLog += std::log(invL[i]);
+        sInv += invL[i];
+        sA2 += alpha[i] * alpha[i];
+    }
+    return ll + Fb * 0.5 * (sLog - sInv - sA2 + (double)invL.size());
+}
+
 // V1+V2.  features: T x D row-major (rho), phi: D (psi), init: T labels (may be null -> uniform gamma).
 // gamma out: T x S, pi out: S, elbos out: max(max_iterations,1) capacity, hard: T.
 // Returns the number of iterations run; *speakers = S.
@@ -368,94 +458,13 @@ int32_t oracle_vbx_refine(const double *features, int64_t T, int64_t D, const do
         }
     }
     for (int s = 0; s < S; ++s) pi[s] = 1.0 / (double)S;
-    std::vector<double> phic(D), sq(D);
-    for (int64_t d = 0; d < D; ++d) {
-        phic[d] = std::max(phi[d], 1e-12);
-        sq[d] = std::sqrt(phic[d]);
-    }
-    std::vector<double> rho((size_t)T * D), G(T);
-    const double log_const = (double)D * std::log(2.0 * M_PI);
-    for (int64_t t = 0; t < T; ++t) {
-        double ss = 0;
-        for (int64_t d = 0; d < D; ++d) {
-            rho[t * D + d] = features[t * D + d] * sq[d];
-            ss += features[t * D + d] * features[t * D + d];
-        }
-        G[t] = -0.5 * (ss + log_const);
-    }
-    const double ratio = cfg->Fa / cfg->Fb;
-    std::vector<double> invL((size_t)S * D), alpha((size_t)S * D), gsum(S), phiTerm(S), logP((size_t)T * S), logPi(S);
     double prev = -std::numeric_limits<double>::max();
     int32_t iterations = 0;
     const int32_t cap = std::max(cfg->max_iterations, 1);
     for (int i = 0; i < cap; ++i) elbos[i] = 0.0;
     for (int32_t it = 0; it < cfg->max_iterations; ++it) {
         iterations = it + 1;
-        for (int s = 0; s < S; ++s) gsum[s] = 0;
-        for (int64_t t = 0; t < T; ++t)
-            for (int s = 0; s < S; ++s) gsum[s] += gamma[t * S + s];
-        for (int s = 0; s < S; ++s) {
-            const double w = ratio * gsum[s];
-            for (int64_t d = 0; d < D; ++d) invL[s * D + d] = 1.0 / std::max(1.0 + w * phic[d], 1e-12);
-        }
-        // temp = gamma^T rho  (S x D), then alpha = ratio * invL .* temp
-        std::fill(alpha.begin(), alpha.end(), 0.0);
-        for (int64_t t = 0; t < T; ++t)
-            for (int s = 0; s < S; ++s) {
-                const double g = gamma[t * S + s];
-                for (int64_t d = 0; d < D; ++d) alpha[s * D + d] += g * rho[t * D + d];
-            }
-        for (size_t i = 0; i < alpha.size(); ++i) alpha[i] = (alpha[i] * invL[i]) * ratio;
-        for (int s = 0; s < S; ++s) {
-            double sum = 0;
-            for (int64_t d = 0; d < D; ++d) sum += (alpha[s * D + d] * alpha[s * D + d] + invL[s * D + d]) * phic[d];
-            phiTerm[s] = sum;
-        }
-        for (int64_t t = 0; t < T; ++t)
-            for (int s = 0; s < S; ++s) {
-                double acc = 0;
-                for (int64_t d = 0; d < D; ++d) acc += rho[t * D + d] * alpha[s * D + d];
-                logP[t * S + s] = ((acc + (-0.5 * phiTerm[s])) + G[t]) * cfg->Fa;
-            }
-        for (int s = 0; s < S; ++s) logPi[s] = std::log(std::max(pi[s], 1e-8));
-        double ll = 0;
-        for (int64_t t = 0; t < T; ++t) {
-            double mx = -std::numeric_limits<double>::max();
-            for (int s = 0; s < S; ++s) {
-                row[s] = logP[t * S + s] + logPi[s];
-                mx = std::max(mx, row[s]);
-            }
-            double sum = 0;
-            for (int s = 0; s < S; ++s) {
-                row[s] = std::exp(row[s] - mx);
-                sum += row[s];
-            }
-            double *g = gamma + t * S;
-            if (sum <= 0.0 || !std::isfinite(sum)) {
-                for (int s = 0; s < S; ++s) g[s] = 1.0 / (double)S;
-                ll += mx;
-            } else {
-                const double inv = 1.0 / sum;
-                for (int s = 0; s < S; ++s) g[s] = row[s] * inv;
-                ll += mx + std::log(sum);
-            }
-        }
-        for (int s = 0; s < S; ++s) pi[s] = 0;
-        for (int64_t t = 0; t < T; ++t)
-            for (int s = 0; s < S; ++s) pi[s] += gamma[t * S + s];
-        double ps = 0;
-        for (int s = 0; s < S; ++s) ps += pi[s];
-        if (ps > 0.0 && std::isfinite(ps)) {
-            const double inv = 1.0 / ps;
-            for (int s = 0; s < S; ++s) pi[s] *= inv;
-        } else for (int s = 0; s < S; ++s) pi[s] = 1.0 / (double)S;
-        double sLog = 0, sInv = 0, sA2 = 0;
-        for (size_t i = 0; i < invL.size(); ++i) {
-            sLog += std::log(invL[i]);
-            sInv += invL[i];
-            sA2 += alpha[i] * alpha[i];
-        }
-        const double elbo = ll + cfg->Fb * 0.5 * (sLog - sInv - sA2 + (double)invL.size());
+        const double elbo = oracle_vbx_step(features, T, D, phi.data(), gamma, pi, S, cfg->Fa, cfg->Fb, gamma, pi);
         if (it < cap) elbos[it] = elbo;
         if (it > 0 && std::fabs(elbo - prev) < cfg->epsilon) {
             prev = elbo;

@@ -623,7 +623,10 @@ def test_vbx_centroids_assignment_against_oracle(gpu_lib, oracle):
         assert cents.shape == ocents.shape and np.abs(cents - ocents).max() <= 1e-12
         labels, scores = cl.assign_embeddings(emb.astype(np.float64), cents, want_scores=True)
         olabels, oscores = oracle.assign_embeddings(emb.astype(np.float64), ocents, want_scores=True)
-        assert np.array_equal(labels, olabels) and np.abs(scores - oscores).max() <= 1e-4
+        assert np.array_equal(labels, olabels)
+        oscores_of_gpu = oracle.assign_embeddings(emb.astype(np.float64), cents, want_scores=True)[1]
+        assert scores.tobytes() == oscores_of_gpu.tobytes()          # the same arithmetic per (n, c): bit-exact
+        assert np.abs(scores - oscores).max() <= 1e-4
     # psi of the wrong length -> identity (VBxClustering.swift:71-76); no initial labels -> uniform gamma
     v = cl.VBxClustering(psi=np.ones(7)).refine(rho[:200], init[:200])
     o = oracle.vbx_refine(rho[:200], np.ones(7), init[:200])

@@ -199,6 +199,77 @@ def test_vbx_matches_independent_numpy_restatement(oracle):
     assert np.array_equal(out.hard, g.argmax(1))
 
 
+def _vbx_refine_cases(oracle):
+    """(name, (rho, psi, initial), config) on the fixture above: the default run and every edge of the config."""
+    emb, _ = synth.speaker_embeddings(600, 256, 5, seed=5)
+    rho, psi = synth.synthetic_plda(emb)
+    init = oracle.ahc_cluster(emb.astype(np.float64), 0.6)
+    bad = rho.copy()
+    bad[3, 5], bad[40, 0] = np.nan, np.inf
+    wild = np.where(np.arange(300) % 7 == 0, 99, init[:300] % 3).astype(np.int32)
+    return [
+        ("default", (rho, psi, init), {}),
+        ("never_converges", (rho, psi, init), dict(max_iterations=6, epsilon=-1.0)),
+        ("zero_iterations", (rho, psi, init), dict(max_iterations=0)),
+        ("one_iteration", (rho, psi, init), dict(max_iterations=1)),
+        ("converges_at_once", (rho, psi, init), dict(epsilon=1e300)),
+        ("no_initial_labels", (rho[:200], psi, np.zeros(0, np.int32)), {}),
+        ("no_smoothing", (rho, psi, init), dict(init_smoothing=-1.0)),
+        ("out_of_range_labels", (rho[:300], psi, wild), {}),
+        ("psi_wrong_length", (rho[:200], np.ones(7), init[:200]), {}),
+        ("psi_tiny", (rho[:200], np.where(np.arange(psi.size) % 3 == 0, 0.0, psi), init[:200]), {}),
+        ("non_finite_rho", (bad, psi, init), dict(max_iterations=3)),
+    ]
+
+
+# sha256 (first 32 hex digits) of gamma, pi, elbos and hard of oracle.vbx_refine on _vbx_refine_cases, computed before
+# the EM iteration moved into oracle_vbx_step: the refactor must not change one bit
+_VBX_REFINE_DIGESTS = {
+    "default": "6023b1d7739a82b2ed09bfd1527bd463",
+    "never_converges": "ab1efa83d4bebe9be0fe141104776289",
+    "zero_iterations": "f89cffc0f56dcf094e7efe73fabc6305",
+    "one_iteration": "3b9e7882ce80c4a0dbecc090e2c24303",
+    "converges_at_once": "6cedc784cfc4a22732b80cf3162c3a17",
+    "no_initial_labels": "4465dbea568e48187e1166f7fbcf0e1f",
+    "no_smoothing": "a42cabbb2f1fae93f43271eba7580ad7",
+    "out_of_range_labels": "0b927164e1d79ab4df13dcf678dfc570",
+    "psi_wrong_length": "39363faf6cc82aeb7fc8c628c361d8e5",
+    "psi_tiny": "4bf1a606b57a36a5a6ea8ef8402b1bb2",
+    "non_finite_rho": "bc806287c708ca20b7ec5d0ce2deb103",
+}
+
+
+def test_vbx_refine_is_bit_identical_after_the_step_refactor(oracle):
+    for name, args, kw in _vbx_refine_cases(oracle):
+        o = oracle.vbx_refine(*args, **kw)
+        h = hashlib.sha256()
+        for a in (o.gamma, o.pi, o.elbos, o.hard):
+            h.update(np.ascontiguousarray(a).tobytes())
+        assert h.hexdigest()[:32] == _VBX_REFINE_DIGESTS[name], name
+
+
+def test_chained_vbx_steps_reproduce_refine(oracle):
+    """vbx_refine = its initial state (max_iterations 0) followed by vbx_step until |dELBO| < epsilon, bit for bit."""
+    for name, (rho, psi, init), kw in _vbx_refine_cases(oracle):
+        if kw.get("max_iterations") == 0:
+            continue
+        Fa, Fb = kw.get("Fa", 0.07), kw.get("Fb", 0.8)
+        its, eps = kw.get("max_iterations", 20), kw.get("epsilon", 1e-4)
+        smoothing = kw.get("init_smoothing", 7.0)
+        start = oracle.vbx_refine(rho, psi, init, max_iterations=0, init_smoothing=smoothing)
+        want = oracle.vbx_refine(rho, psi, init, **kw)
+        g, p, elbos = start.gamma, start.pi, []
+        assert np.array_equal(p, np.full(p.size, 1.0 / p.size))
+        for it in range(its):
+            g, p, e = oracle.vbx_step(rho, psi, g, p, Fa, Fb)
+            elbos.append(e)
+            if it > 0 and abs(e - elbos[-2]) < eps:
+                break
+        assert len(elbos) == want.elbos.size, name
+        assert np.array(elbos).tobytes() == want.elbos.tobytes(), name
+        assert g.tobytes() == want.gamma.tobytes() and p.tobytes() == want.pi.tobytes(), name
+
+
 def test_pipeline_recovers_speakers_and_filters_nan(oracle):
     emb, who = synth.speaker_embeddings(400, 256, 4, weights=(0.4, 0.3, 0.2, 0.1), seed=9)
     emb[7, 100] = np.inf
