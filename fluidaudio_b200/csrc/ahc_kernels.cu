@@ -1099,22 +1099,19 @@ __global__ void ahc_widen_kernel(const float *__restrict__ in, double *__restric
 
 int launch_normalize_rows(const double *d_in, double *d_out, int rows, int dim, cudaStream_t s) {
     if (rows <= 0) return FA_OK;
-    ahc_normalize_rows_kernel<<<(rows + 127) / 128, 128, 0, s>>>(d_in, d_out, rows, dim, 0.0);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(ahc_normalize_rows_kernel, (rows + 127) / 128, 128, 0, s, d_in, d_out, rows, dim, 0.0));
     return FA_OK;
 }
 
 int launch_normalize_rows_keep(const double *d_in, double *d_out, int rows, int dim, cudaStream_t s) {
     if (rows <= 0) return FA_OK;
-    ahc_normalize_rows_kernel<<<(rows + 127) / 128, 128, 0, s>>>(d_in, d_out, rows, dim, 1.0);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(ahc_normalize_rows_kernel, (rows + 127) / 128, 128, 0, s, d_in, d_out, rows, dim, 1.0));
     return FA_OK;
 }
 
 int launch_widen_rows(const float *d_in, double *d_out, long long count, cudaStream_t s) {
     if (count <= 0) return FA_OK;
-    ahc_widen_kernel<<<(unsigned)((count + 255) / 256), 256, 0, s>>>(d_in, d_out, count);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(ahc_widen_kernel, (unsigned)((count + 255) / 256), 256, 0, s, d_in, d_out, count));
     return FA_OK;
 }
 
@@ -1153,55 +1150,6 @@ int Solver::init(cudaStream_t s, int worker_limit) {
 }
 
 namespace {
-struct Layout {
-    size_t rows, cols, node_weight, key, nn, heap_at, heap_where, node_of, slot_of, live_bits, merge_a, merge_b, merge_d,
-        cmd, threshold, results, error, init_partial, problem, total;
-    size_t f_cf, f_nrm2, f_rn, f_U, f_best_d, f_best_j, f_cand, f_cand_d, f_counters, f_tmin;
-    bool f_keep_tmin;
-    int ranges, filter_cap;
-};
-Layout make_layout(int N, int D, int Ns, int workers) {
-    Layout L{};
-    Carver c;
-    L.rows = c.at<double>((size_t)(2 * N - 1) * D);
-    L.cols = c.at<double>((size_t)D * Ns);
-    L.node_weight = c.at<int>((size_t)2 * N);
-    L.key = c.at<double>((size_t)N + 2);
-    L.nn = c.at<int>((size_t)N + 2);
-    L.heap_at = c.at<int>((size_t)N + 2);
-    L.heap_where = c.at<int>((size_t)N + 2);
-    L.node_of = c.at<int>((size_t)N + 2);
-    L.slot_of = c.at<int>((size_t)2 * N);
-    L.live_bits = c.at<unsigned>((size_t)(2 * N + 31) / 32 + 2);
-    L.merge_a = c.at<int>((size_t)N);
-    L.merge_b = c.at<int>((size_t)N);
-    L.merge_d = c.at<double>((size_t)N);
-    L.cmd = c.at<unsigned long long>(32);         // own 256-byte line
-    L.threshold = c.at<unsigned long long>(32);   // own 256-byte line
-    L.results = c.at<ResultSlot>(2 * (((size_t)workers + 1) << kSlotShift));
-    L.error = c.at<int>(64);
-    L.ranges = (N + kJR - 1) / kJR;
-    L.init_partial = c.at<Cand>((size_t)L.ranges * N);
-    L.problem = c.at<Problem>(1);
-    // float32 filter of the initial nearest-neighbour pass (N >= kFilterMinN only, but sized unconditionally: small)
-    L.filter_cap = (int)std::min<long long>(64LL * N, 1 << 24);
-    L.f_cf = c.at<float>((size_t)((D + 7) & ~7) * Ns);   // rows rounded up to the GEMM's k-chunk (zero rows)
-    L.f_nrm2 = c.at<double>((size_t)N);
-    L.f_rn = c.at<float>((size_t)N);
-    L.f_U = c.at<unsigned long long>((size_t)N);
-    L.f_best_d = c.at<unsigned long long>((size_t)N);
-    L.f_best_j = c.at<int>((size_t)N);
-    L.f_cand = c.at<int2>((size_t)L.filter_cap);
-    L.f_cand_d = c.at<double>((size_t)L.filter_cap);
-    L.f_counters = c.at<int>(64);
-    {
-        const long long nt = (N + 63) / 64;
-        L.f_keep_tmin = (long long)N * nt <= (16LL << 20);   // <= 64 MB
-        L.f_tmin = c.at<float>(L.f_keep_tmin ? (size_t)((long long)N * nt) : 1);
-    }
-    L.total = (c.off + 255) & ~size_t(255);
-    return L;
-}
 // bytes of master state staged in shared memory at each level (must mirror ahc_master's carving)
 size_t master_smem_bytes(int N, int level) {
     auto up = [](size_t b) { return (b + 15) & ~size_t(15); };
@@ -1211,26 +1159,28 @@ size_t master_smem_bytes(int N, int level) {
     if (level >= 3) b += up(sizeof(int) * N);
     return b;
 }
+
+// Dynamic shared memory the merge kernel may use: leaves room for its static shared memory.
+constexpr size_t kMergeSmemCap = 227 * 1024 - 2048;
+
+// Shared memory of one worker CTA before any resident node vector: the target vector and the reduction scratch.
+size_t worker_fixed_smem(int D) {
+    return 3 * sizeof(double) * (size_t)((D + 1) & ~1) + 2 * sizeof(double) * (kMergeThreads / 32) + 64;
+}
+
+// Node vectors one worker CTA can keep in shared memory (at most one per thread), 0 if not even one fits.
+int resident_slot_capacity(int D) {
+    const size_t fixed = worker_fixed_smem(D);
+    if (fixed + sizeof(double) * D > kMergeSmemCap) return 0;
+    return (int)std::min<size_t>(kMergeThreads, (kMergeSmemCap - fixed) / (sizeof(double) * (size_t)D));
+}
 } // namespace
 
 // Worker CTAs a problem needs to keep every node vector in shared memory (the fast placement), or 0 if a single CTA
-// cannot hold even one vector.  Mirrors the sizing in linkage_device.
+// cannot hold even one vector.
 int resident_workers_needed(int N, int D) {
-    const size_t smem_cap = 227 * 1024 - 2048;
-    const size_t worker_fixed = 3 * sizeof(double) * (size_t)((D + 1) & ~1) + 2 * sizeof(double) * (kMergeThreads / 32) + 64;
-    if (worker_fixed + sizeof(double) * D > smem_cap) return 0;
-    const int cap_slots = (int)std::min<size_t>(kMergeThreads, (smem_cap - worker_fixed) / (sizeof(double) * (size_t)D));
-    if (cap_slots < 1) return 0;
-    return (N + cap_slots - 1) / cap_slots;
-}
-
-int Solver::ensure_pool(int N, int D) {
-    const int Ns = (N + 31) & ~31;
-    const Layout L = make_layout(N, D, Ns, max_workers);
-    const int st = grow_buffer(d_pool, pool_bytes, L.total);
-    if (st != FA_OK) return st;
-    const size_t hneed = sizeof(double) * (size_t)(2 * N + 16) + sizeof(int) * (size_t)(4 * N + 64);
-    return grow_buffer(h_pool, h_pool_bytes, hneed, true);
+    const int cap_slots = resident_slot_capacity(D);
+    return cap_slots ? (N + cap_slots - 1) / cap_slots : 0;
 }
 
 // FA_AHC_* environment hooks (tests only: fall-back placements and the float32 filter at small N), read once.
@@ -1254,11 +1204,10 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     if (N < 2) return FA_OK;
     const int Ns = (N + 31) & ~31;
     // master placement: slot-indexed heap (+ nn, + node_of) in shared memory when it fits
-    const size_t smem_cap = 227 * 1024 - 2048;   // leaves room for the kernel's static shared memory
     int level = 0;
     if (N <= 65535)
         for (int l = 1; l <= 3; ++l)
-            if (master_smem_bytes(N, l) <= smem_cap) level = l;
+            if (master_smem_bytes(N, l) <= kMergeSmemCap) level = l;
     // test hooks: exercise the fall-back placements at small N (tests/test_gpu_parity.py)
     // (all FA_AHC_* hooks are read ONCE per process, see hooks(): stray variables cannot change behaviour mid-run)
     const Hooks &hk = hooks();
@@ -1267,16 +1216,15 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     const bool idx16 = level >= 1;
     // worker placement: resident (each CTA keeps <= 128 node vectors in shared memory) when the whole problem fits
     // into max_workers CTAs, else streamed from the k-major global copy
-    const size_t worker_fixed = 3 * sizeof(double) * (size_t)((D + 1) & ~1) + 2 * sizeof(double) * (kMergeThreads / 32) + 64;
-    if (worker_fixed + sizeof(double) * D > smem_cap) {
+    const int cap_slots = resident_slot_capacity(D);
+    if (cap_slots == 0) {
         fa::set_error("dimension %d too large for the merge kernel's shared-memory target vector", D);
         return FA_RUNTIME_ERROR;
     }
-    const int cap_slots = (int)std::min<size_t>(kMergeThreads, (smem_cap - worker_fixed) / (sizeof(double) * (size_t)D));
-    bool resident = cap_slots >= 1 && (long long)cap_slots * max_workers >= N;
+    bool resident = (long long)cap_slots * max_workers >= N;
     if (force_stream) resident = false;
     int workers, slots_per_cta = 0;
-    size_t worker_smem = worker_fixed;
+    size_t worker_smem = worker_fixed_smem(D);
     if (resident) {
         // enough CTAs to hold every node, but no more than needed: the per-step barrier cost grows with CTA count
         workers = std::min(max_workers, std::max(1, (N + cap_slots - 1) / cap_slots));
@@ -1291,48 +1239,71 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
         }
     }
     const size_t smem = std::max(worker_smem, level ? master_smem_bytes(N, level) : (size_t)0);
-    int st = ensure_pool(N, D);
-    if (st != FA_OK) return st;
-    const Layout L = make_layout(N, D, Ns, max_workers);
-    char *base = static_cast<char *>(d_pool);
+
+    // device arena: problem state, then the float32 filter of the initial nearest-neighbour pass (N >= filter_min_n
+    // only, but sized unconditionally: small)
+    const int ranges = (N + kJR - 1) / kJR;
+    const int filter_cap = (int)std::min<long long>(64LL * N, 1 << 24);
+    const long long nt = (N + 63) / 64;
+    const bool keep_tmin = (long long)N * nt <= (16LL << 20);   // <= 64 MB
     Problem P{};
+    FilterBufs F{};
+    Cand *init_partial = nullptr;
+    Problem *d_prob = nullptr;
+    int st = carve_arena(d_pool, pool_bytes, [&](Carver &c) {
+        P.rows = c.take<double>((size_t)(2 * N - 1) * D);
+        P.cols = c.take<double>((size_t)D * Ns);
+        P.node_weight = c.take<int>((size_t)2 * N);
+        P.key = c.take<double>((size_t)N + 2);
+        P.nn = c.take<int>((size_t)N + 2);
+        P.heap_at = c.take<int>((size_t)N + 2);
+        P.heap_where = c.take<int>((size_t)N + 2);
+        P.node_of = c.take<int>((size_t)N + 2);
+        P.slot_of = c.take<int>((size_t)2 * N);
+        P.live_bits = c.take<unsigned>((size_t)(2 * N + 31) / 32 + 2);
+        P.merge_a = c.take<int>((size_t)N);
+        P.merge_b = c.take<int>((size_t)N);
+        P.merge_d = c.take<double>((size_t)N);
+        P.cmd = c.take<unsigned long long>(32);         // own 256-byte line
+        P.threshold = c.take<unsigned long long>(32);   // own 256-byte line
+        P.results = c.take<ResultSlot>(2 * (((size_t)max_workers + 1) << kSlotShift));
+        P.error = c.take<int>(64);
+        init_partial = c.take<Cand>((size_t)ranges * N);
+        d_prob = c.take<Problem>(1);
+        F.cf = c.take<float>((size_t)((D + 7) & ~7) * Ns);   // rows rounded up to the GEMM's k-chunk (zero rows)
+        F.nrm2 = c.take<double>((size_t)N);
+        F.rn = c.take<float>((size_t)N);
+        F.U = c.take<unsigned long long>((size_t)N);
+        F.best_d = c.take<unsigned long long>((size_t)N);
+        F.best_j = c.take<int>((size_t)N);
+        F.cand = c.take<int2>((size_t)filter_cap);
+        F.cand_d = c.take<double>((size_t)filter_cap);
+        F.counters = c.take<int>(64);
+        float *tmin = c.take<float>(keep_tmin ? (size_t)(N * nt) : 1);
+        F.tmin = keep_tmin ? tmin : nullptr;
+    }, 255);
+    if (st != FA_OK) return st;
+    // pinned host mirrors
+    double *h_key = nullptr, *h_md = nullptr;
+    int *h_at = nullptr, *h_where = nullptr, *h_ma = nullptr, *h_mb = nullptr, *h_err = nullptr;
+    st = carve_arena(h_pool, h_pool_bytes, [&](Carver &c) {
+        h_key = c.take<double>((size_t)N + 4);
+        h_md = c.take<double>((size_t)N + 4);
+        h_at = c.take<int>((size_t)N + 2);   // reused as uint16 when idx16
+        h_where = c.take<int>((size_t)N + 2);
+        h_ma = c.take<int>((size_t)N);
+        h_mb = c.take<int>((size_t)N);
+        h_err = c.take<int>(4);          // error flag, then the filter's three counters
+    }, 0, true);
+    if (st != FA_OK) return st;
     P.N = N;
     P.D = D;
     P.Ns = Ns;
-    P.rows = reinterpret_cast<double *>(base + L.rows);
-    P.cols = reinterpret_cast<double *>(base + L.cols);
-    P.node_weight = reinterpret_cast<int *>(base + L.node_weight);
-    P.key = reinterpret_cast<double *>(base + L.key);
-    P.nn = reinterpret_cast<int *>(base + L.nn);
-    P.heap_at = base + L.heap_at;
-    P.heap_where = base + L.heap_where;
-    P.node_of = reinterpret_cast<int *>(base + L.node_of);
-    P.slot_of = reinterpret_cast<int *>(base + L.slot_of);
-    P.live_bits = reinterpret_cast<unsigned *>(base + L.live_bits);
-    P.merge_a = reinterpret_cast<int *>(base + L.merge_a);
-    P.merge_b = reinterpret_cast<int *>(base + L.merge_b);
-    P.merge_d = reinterpret_cast<double *>(base + L.merge_d);
-    P.cmd = reinterpret_cast<unsigned long long *>(base + L.cmd);
-    P.threshold = reinterpret_cast<unsigned long long *>(base + L.threshold);
-    P.results = reinterpret_cast<ResultSlot *>(base + L.results);
     P.result_stride = (max_workers + 1) << kSlotShift;
-    P.error = reinterpret_cast<int *>(base + L.error);
     P.resident = resident ? 1 : 0;
     P.slots_per_cta = slots_per_cta;
     P.idx16 = idx16 ? 1 : 0;
     P.smem_level = level;
-    Cand *init_partial = reinterpret_cast<Cand *>(base + L.init_partial);
-    Problem *d_prob = reinterpret_cast<Problem *>(base + L.problem);
-
-    // pinned host mirrors
-    char *hb = static_cast<char *>(h_pool);
-    double *h_key = reinterpret_cast<double *>(hb);
-    double *h_md = h_key + N + 4;
-    int *h_at = reinterpret_cast<int *>(h_md + N + 4);   // N ints (reused as uint16 when idx16)
-    int *h_where = h_at + N + 2;
-    int *h_ma = h_where + N + 2;
-    int *h_mb = h_ma + N;
-    int *h_err = h_mb + N;
 
     // timing events live in a guard: every early return below (FA_CUDA_TRY) releases them
     struct Events {
@@ -1345,61 +1316,41 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     } ev;
     for (int i = 0; i < 4; ++i) FA_CUDA_TRY(cudaEventCreate(&ev.e[i]));
 
-    FA_CUDA_TRY(cudaMemsetAsync(base + L.cmd, 0, 256, stream));
-    FA_CUDA_TRY(cudaMemsetAsync(base + L.threshold, 0, 256, stream));
-    FA_CUDA_TRY(cudaMemsetAsync(base + L.results, 0, 2 * sizeof(ResultSlot) * ((size_t)(max_workers + 1) << kSlotShift), stream));
-    FA_CUDA_TRY(cudaMemsetAsync(base + L.error, 0, 256, stream));
+    FA_CUDA_TRY(cudaMemsetAsync(P.cmd, 0, 256, stream));
+    FA_CUDA_TRY(cudaMemsetAsync(P.threshold, 0, 256, stream));
+    FA_CUDA_TRY(cudaMemsetAsync(P.results, 0, 2 * sizeof(ResultSlot) * ((size_t)(max_workers + 1) << kSlotShift), stream));
+    FA_CUDA_TRY(cudaMemsetAsync(P.error, 0, 256, stream));
     FA_CUDA_TRY(cudaEventRecord(ev[0], stream));
-    {
-        dim3 grid((Ns + 31) / 32, (D + 31) / 32), block(32, 8);
-        ahc_stage_kernel<<<grid, block, 0, stream>>>(d_rows, P.rows, P.cols, N, D, Ns);
-        FA_CUDA_TRY(cudaGetLastError());
-        launches += 1;
-    }
+    FA_CUDA_TRY(fa::launch(ahc_stage_kernel, dim3((Ns + 31) / 32, (D + 31) / 32), dim3(32, 8), 0, stream, d_rows, P.rows, P.cols,
+                           N, D, Ns));
     auto exact_init = [&]() -> int {
-        dim3 g2((N + kTI - 1) / kTI, L.ranges);
-        ahc_init_nn_kernel<<<g2, kTI, 0, stream>>>(P.cols, N, D, Ns, init_partial, P.error);
-        FA_CUDA_TRY(cudaGetLastError());
-        ahc_init_reduce_kernel<<<(N + 127) / 128, 128, 0, stream>>>(init_partial, N, L.ranges, P.key, P.nn,
-                                                                     P.node_weight);
-        FA_CUDA_TRY(cudaGetLastError());
-        launches += 2;
+        FA_CUDA_TRY(fa::launch(ahc_init_nn_kernel, dim3((N + kTI - 1) / kTI, ranges), kTI, 0, stream, P.cols, N, D, Ns,
+                               init_partial, P.error));
+        FA_CUDA_TRY(fa::launch(ahc_init_reduce_kernel, (N + 127) / 128, 128, 0, stream, init_partial, N, ranges, P.key, P.nn,
+                               P.node_weight));
         return FA_OK;
     };
     const bool use_filter = hk.filter_min_n > 0 && N >= hk.filter_min_n;
     int *h_fc = h_err + 1;   // [3] filter counters (pinned)
     if (use_filter) {
-        FilterBufs F{};
-        F.cf = reinterpret_cast<float *>(base + L.f_cf);
-        F.nrm2 = reinterpret_cast<double *>(base + L.f_nrm2);
-        F.rn = reinterpret_cast<float *>(base + L.f_rn);
-        F.U = reinterpret_cast<unsigned long long *>(base + L.f_U);
-        F.best_d = reinterpret_cast<unsigned long long *>(base + L.f_best_d);
-        F.best_j = reinterpret_cast<int *>(base + L.f_best_j);
-        F.cand = reinterpret_cast<int2 *>(base + L.f_cand);
-        F.cand_d = reinterpret_cast<double *>(base + L.f_cand_d);
-        F.counters = reinterpret_cast<int *>(base + L.f_counters);
-        F.cap = L.filter_cap;
+        F.cap = filter_cap;
         F.nt = (N + kFT - 1) / kFT;
-        F.tmin = L.f_keep_tmin ? reinterpret_cast<float *>(base + L.f_tmin) : nullptr;
         F.c1 = 2.02 * (double)(D + 3) * 5.9604644775390625e-08;   // 2^-24
         F.c2 = 2e-12;
         FA_CUDA_TRY(cudaMemsetAsync(F.counters, 0, 64 * sizeof(int), stream));
-        ahc_filter_prep_kernel<<<(Ns + 127) / 128, 128, 0, stream>>>(P.cols, N, D, Ns, F);
+        FA_CUDA_TRY(fa::launch(ahc_filter_prep_kernel, (Ns + 127) / 128, 128, 0, stream, P.cols, N, D, Ns, F));
         const int nt2 = (N + kGT - 1) / kGT;
-        ahc_filter_tile128_kernel<<<(unsigned)((long long)nt2 * (nt2 + 1) / 2), 256, 0, stream>>>(N, D, Ns, F);
+        FA_CUDA_TRY(fa::launch(ahc_filter_tile128_kernel, (unsigned)((long long)nt2 * (nt2 + 1) / 2), 256, 0, stream, N, D, Ns, F));
         if (F.tmin && (size_t)8 * D * sizeof(float) <= 48 * 1024) {
-            ahc_filter_rows_kernel<<<(N + 7) / 8, 256, (size_t)8 * D * sizeof(float), stream>>>(N, D, Ns, F);
+            FA_CUDA_TRY(fa::launch(ahc_filter_rows_kernel, (N + 7) / 8, 256, (size_t)8 * D * sizeof(float), stream, N, D, Ns, F));
         } else {
             const unsigned tiles = (unsigned)((long long)F.nt * (F.nt + 1) / 2);
-            ahc_filter_dense_kernel<<<tiles, 256, 0, stream>>>(N, D, Ns, F);
+            FA_CUDA_TRY(fa::launch(ahc_filter_dense_kernel, tiles, 256, 0, stream, N, D, Ns, F));
         }
         const unsigned cgrid = (unsigned)((F.cap + 255) / 256);
-        ahc_filter_exact_kernel<<<cgrid, 256, 0, stream>>>(P.cols, D, Ns, F);
-        ahc_filter_argmin_kernel<<<cgrid, 256, 0, stream>>>(F);
-        ahc_filter_finish_kernel<<<(N + 127) / 128, 128, 0, stream>>>(N, F, P.key, P.nn, P.node_weight);
-        FA_CUDA_TRY(cudaGetLastError());
-        launches += 6;
+        FA_CUDA_TRY(fa::launch(ahc_filter_exact_kernel, cgrid, 256, 0, stream, P.cols, D, Ns, F));
+        FA_CUDA_TRY(fa::launch(ahc_filter_argmin_kernel, cgrid, 256, 0, stream, F));
+        FA_CUDA_TRY(fa::launch(ahc_filter_finish_kernel, (N + 127) / 128, 128, 0, stream, N, F, P.key, P.nn, P.node_weight));
         FA_CUDA_TRY(cudaMemcpyAsync(h_fc, F.counters, 3 * sizeof(int), cudaMemcpyDeviceToHost, stream));
         FA_CUDA_TRY(cudaStreamSynchronize(stream));
         if (h_fc[1] || h_fc[2]) {   // non-finite / huge input, or more candidates than the list holds: the exact pass decides
@@ -1441,13 +1392,10 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
         static std::once_flag once;   // a per-function attribute: set it once to the maximum, solvers run concurrently
         static cudaError_t attr_err = cudaSuccess;
         std::call_once(once, [&]() {
-            attr_err = cudaFuncSetAttribute(ahc_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
+            attr_err = cudaFuncSetAttribute(ahc_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmemCap);
         });
         FA_CUDA_TRY(attr_err);
-        void *args[] = {&d_prob};
-        FA_CUDA_TRY(cudaLaunchCooperativeKernel((void *)ahc_merge_kernel, dim3(workers + 1), dim3(kWorkerThreads), args,
-                                                smem, stream));
-        ++launches;
+        FA_CUDA_TRY(fa::launch_cooperative(ahc_merge_kernel, workers + 1, kWorkerThreads, smem, stream, d_prob));
     }
     FA_CUDA_TRY(cudaEventRecord(ev[3], stream));
     FA_CUDA_TRY(cudaMemcpyAsync(h_ma, P.merge_a, sizeof(int) * (N - 1), cudaMemcpyDeviceToHost, stream));

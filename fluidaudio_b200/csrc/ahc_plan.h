@@ -58,12 +58,10 @@ struct Problem {
 struct Solver {
     int num_sms = 0;
     int max_workers = 0;      // worker CTAs available for one problem (grid = workers + 1)
-    long long launches = 0;
     cudaStream_t stream = nullptr;
     // device storage (grown on demand, reused across calls)
     void *d_pool = nullptr;
     size_t pool_bytes = 0;
-    Problem *d_problem = nullptr;
     double *d_input = nullptr;   // staging of the caller's [N x D] rows when they come from the host
     size_t input_bytes = 0;
     // pinned host mirrors
@@ -77,7 +75,6 @@ struct Solver {
     // Z: host buffer of (N-1) x 4 doubles.  Status codes follow FastClusterWrapper.h.
     int linkage_device(const double *d_rows, int N, int D, double *Z_host);
     int linkage_host(const double *rows_host, size_t N, size_t D, double *Z_host, size_t z_len);
-    int ensure_pool(int N, int D);
 };
 
 // [0] initial nearest-neighbour kernels, [1] heapify + copies, [2] merge kernel, [3] total (ms) of the calling

@@ -37,7 +37,7 @@ void set_error(const char *fmt, ...) {
 }
 const char *last_error() { return g_error; }
 
-static std::atomic<long long> g_launches{0};
+std::atomic<long long> g_launches{0};
 
 static int usable_device_count() {
     int n = 0;
@@ -100,10 +100,6 @@ struct ClusterContext {
             if (e) cudaEventDestroy(e);
         if (stream) cudaStreamDestroy(stream);
     }
-    int reserve(size_t dbytes, size_t hbytes) {
-        const int st = grow_buffer(d_buf, d_bytes, dbytes);
-        return st != FA_OK ? st : grow_buffer(h_buf, h_bytes, hbytes, true);
-    }
 };
 
 static std::mutex g_pool_mutex;
@@ -141,6 +137,37 @@ struct Lease {
     }
 };
 
+// Leases a context for `worker_limit`, runs body(ClusterContext &) on it and returns the body's status.  The status is
+// recorded on the lease, so a context whose call ended in FA_CUDA_ERROR is freed rather than pooled.
+template <typename Body> static int with_context(int worker_limit, Body &&body) {
+    Lease lease(worker_limit);
+    if (lease.status != FA_OK) return lease.status;
+    lease.status = body(*lease.ctx);
+    return lease.status;
+}
+
+static vbx::Config to_vbx(const fa_vbx_config &c) {
+    vbx::Config vc;
+    vc.Fa = c.Fa;
+    vc.Fb = c.Fb;
+    vc.max_iterations = c.max_iterations;
+    vc.epsilon = c.epsilon;
+    vc.init_smoothing = c.init_smoothing;
+    return vc;
+}
+
+// VBxOutput.assignedClusterCount: the distinct row-argmax winners among S speakers
+static int distinct_winners(const std::vector<int> &hard, int S) {
+    std::vector<char> seen(S, 0);
+    int count = 0;
+    for (const int h : hard)
+        if (h >= 0 && h < S && !seen[h]) {
+            seen[h] = 1;
+            ++count;
+        }
+    return count;
+}
+
 static float ms_between(cudaEvent_t a, cudaEvent_t b) {
     float ms = 0;
     cudaEventElapsedTime(&ms, a, b);
@@ -155,45 +182,38 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     const auto wall0 = std::chrono::steady_clock::now();
     cudaStream_t s = C.stream;
     const int n = (int)N, e = (int)E, r = (int)R;
-    // ---- device arena -----------------------------------------------------------------------------------
-    size_t bytes = 0;
-    {
-        Carver c{nullptr};
-        c.take<float>(N * E);
-        c.take<double>(N * E);       // embd
-        c.take<double>(N * R);       // rho
-        c.take<unsigned char>(N);
-        c.take<int>(N);              // train idx
-        c.take<double>(N * E);       // train
-        c.take<double>(N * R);       // train rho
-        c.take<double>(N * E);       // normalised train
-        c.take<int>(N);              // init labels
-        c.take<int>(N);              // hard
-        c.take<int>(N);              // labels
-        c.take<int>(64);
-        bytes = c.off + 4096;
-    }
-    int st = C.reserve(bytes, N * (sizeof(int) * 4 + 8) + (N > 1 ? (N - 1) * 4 * sizeof(double) : 0) + 4096);
+    // ---- device arena and pinned host arena --------------------------------------------------------------------
+    float *d_emb32;
+    double *d_emb, *d_rho, *d_train, *d_train_rho, *d_norm;
+    unsigned char *d_ok;
+    int *d_idx, *d_init, *d_hard, *d_labels, *d_count;
+    int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        d_emb32 = c.take<float>(N * E);
+        d_emb = c.take<double>(N * E);
+        d_rho = c.take<double>(N * R);
+        d_ok = c.take<unsigned char>(N);
+        d_idx = c.take<int>(N);               // train idx
+        d_train = c.take<double>(N * E);
+        d_train_rho = c.take<double>(N * R);
+        d_norm = c.take<double>(N * E);       // normalised train
+        d_init = c.take<int>(N);              // init labels
+        d_hard = c.take<int>(N);
+        d_labels = c.take<int>(N);
+        d_count = c.take<int>(64);
+    }, 4096);
     if (st != FA_OK) return st;
-    Carver c{static_cast<char *>(C.d_buf)};
-    float *d_emb32 = c.take<float>(N * E);
-    double *d_emb = c.take<double>(N * E);
-    double *d_rho = c.take<double>(N * R);
-    unsigned char *d_ok = c.take<unsigned char>(N);
-    int *d_idx = c.take<int>(N);
-    double *d_train = c.take<double>(N * E);
-    double *d_train_rho = c.take<double>(N * R);
-    double *d_norm = c.take<double>(N * E);
-    int *d_init = c.take<int>(N);
-    int *d_hard = c.take<int>(N);
-    int *d_labels = c.take<int>(N);
-    int *d_count = c.take<int>(64);
-    Carver hc{static_cast<char *>(C.h_buf)};
-    unsigned char *h_ok = hc.take<unsigned char>(N);
-    int *h_idx = hc.take<int>(N);
-    int32_t *h_init = hc.take<int32_t>(N);
-    int *h_count = hc.take<int>(16);
-    double *h_Z = hc.take<double>(N > 1 ? (N - 1) * 4 : 4);
+    unsigned char *h_ok;
+    int *h_idx, *h_count;
+    int32_t *h_init;
+    double *h_Z;
+    st = carve_arena(C.h_buf, C.h_bytes, [&](Carver &c) {
+        h_ok = c.take<unsigned char>(N);
+        h_idx = c.take<int>(N);
+        h_init = c.take<int32_t>(N);
+        h_count = c.take<int>(16);
+        h_Z = c.take<double>(N > 1 ? (N - 1) * 4 : 4);
+    }, 4096, true);
+    if (st != FA_OK) return st;
 
     FA_CUDA_TRY(cudaEventRecord(C.ev[0], s));
     FA_CUDA_TRY(cudaMemcpyAsync(d_emb32, emb, N * E * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -202,7 +222,6 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     if (st != FA_OK) return st;
     st = vbx::finite_rows_device(d_emb32, n, e, d_ok, s);               // :591-611
     if (st != FA_OK) return st;
-    g_launches += 2;
     FA_CUDA_TRY(cudaMemcpyAsync(h_ok, d_ok, N, cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     int Tn = 0;
@@ -219,7 +238,6 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
         if (st != FA_OK) return st;
         st = vbx::gather_rows_device(d_rho, d_idx, Tn, r, d_train_rho, s);
         if (st != FA_OK) return st;
-        g_launches += 2;
         d_tr = d_train;
         d_tr_rho = d_train_rho;
     }
@@ -229,11 +247,8 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     if (Tn >= 2) {
         st = ahc::launch_normalize_rows(d_tr, d_norm, Tn, e, s);
         if (st != FA_OK) return st;
-        g_launches += 1;
         FA_CUDA_TRY(cudaEventRecord(C.ev[2], s));
-        const long long before = C.solver.launches;
         st = C.solver.linkage_device(d_norm, Tn, e, h_Z);
-        g_launches += C.solver.launches - before;
         FA_CUDA_TRY(cudaEventRecord(C.ev[3], s));
         FA_CUDA_TRY(cudaEventSynchronize(C.ev[3]));
         ms_norm = ms_between(C.ev[1], C.ev[2]);
@@ -260,31 +275,26 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     // ---- VBx (:311-343) -----------------------------------------------------------------------------------
     FA_CUDA_TRY(cudaEventRecord(C.ev[4], s));
     FA_CUDA_TRY(cudaMemcpyAsync(d_init, h_init, Tn * sizeof(int), cudaMemcpyHostToDevice, s));
-    // arena for gamma / pi / elbos / centroids (depends on S, known only now)
-    vbx::Config vc;
-    vc.Fa = cfg.vbx.Fa;
-    vc.Fb = cfg.vbx.Fb;
-    vc.max_iterations = cfg.vbx.max_iterations;
-    vc.epsilon = cfg.vbx.epsilon;
-    vc.init_smoothing = cfg.vbx.init_smoothing;
-    const size_t gbytes = ((size_t)Tn * S + 2 * (size_t)S + std::max(vc.max_iterations, 1) + 2 * ((size_t)S * E + E)) *
-                              sizeof(double) + 8192;
-    st = C.cent_ws.reserve(std::max(gbytes, (size_t)1 << 20));
+    // arena for gamma / pi / elbos / centroids (depends on S, known only now), at least 1 MB
+    const vbx::Config vc = to_vbx(cfg.vbx);
+    st = grow_buffer(C.cent_ws.pool, C.cent_ws.pool_bytes, (size_t)1 << 20);
     if (st != FA_OK) return st;
-    Carver gc{static_cast<char *>(C.cent_ws.pool)};
-    double *d_gamma = gc.take<double>((size_t)Tn * S);
-    double *d_pi = gc.take<double>(S);
-    double *d_elbos = gc.take<double>(std::max(vc.max_iterations, 1));
-    double *d_cent = gc.take<double>((size_t)S * E + E);
-    double *d_cent_n = gc.take<double>((size_t)S * E + E);
+    double *d_gamma, *d_pi, *d_elbos, *d_cent, *d_cent_n;
+    st = carve_arena(C.cent_ws.pool, C.cent_ws.pool_bytes, [&](Carver &c) {
+        d_gamma = c.take<double>((size_t)Tn * S);
+        d_pi = c.take<double>(S);
+        d_elbos = c.take<double>(std::max(vc.max_iterations, 1));
+        d_cent = c.take<double>((size_t)S * E + E);
+        d_cent_n = c.take<double>((size_t)S * E + E);
+    }, 8192);
+    if (st != FA_OK) return st;
     int iterations = 0;
     std::vector<double> psi_eff(R, 1.0);   // VBxClustering.swift:71-76: identity when psi does not match
     if (psi) std::memcpy(psi_eff.data(), psi, R * sizeof(double));
     bool used_vbx = false;
-    long long lc = 0;
     if (Tn > 0) {
         st = vbx::refine_device(C.vbx_ws, d_tr_rho, Tn, r, psi_eff.data(), d_init, S, vc, d_gamma, d_pi, d_elbos, d_hard,
-                                &iterations, s, &lc);
+                                &iterations, s);
         if (st != FA_OK) return st;
         used_vbx = true;
     }
@@ -295,30 +305,22 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
         std::vector<int> hard(Tn);
         FA_CUDA_TRY(cudaMemcpyAsync(hard.data(), d_hard, sizeof(int) * Tn, cudaMemcpyDeviceToHost, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));
-        std::vector<char> seen(S, 0);
-        detected = 0;                                       // VBxOutput.assignedClusterCount: row-argmax winners
-        for (int i = 0; i < Tn; ++i)
-            if (hard[i] >= 0 && hard[i] < S && !seen[hard[i]]) {
-                seen[hard[i]] = 1;
-                ++detected;
-            }
+        detected = distinct_winners(hard, S);
         long long lo = 1, hi = Tn;
         kmeans::resolve_constraints(Tn, cfg.num_speakers, cfg.min_speakers, cfg.max_speakers, &lo, &hi);
         if (detected < lo || detected > hi) {
             const int target = (int)(detected < lo ? lo : hi);
-            st = C.cent_ws.reserve(std::max(C.cent_ws.pool_bytes, gbytes + 2 * (size_t)target * E * sizeof(double)));
-            if (st != FA_OK) return st;
             // the arena may have moved: re-carve (gamma / pi are not needed any more on this path)
-            Carver kc{static_cast<char *>(C.cent_ws.pool)};
-            d_cent = kc.take<double>((size_t)target * E + E);
-            d_cent_n = kc.take<double>((size_t)target * E + E);
+            st = carve_arena(C.cent_ws.pool, C.cent_ws.pool_bytes, [&](Carver &c) {
+                d_cent = c.take<double>((size_t)target * E + E);
+                d_cent_n = c.take<double>((size_t)target * E + E);
+            }, 8192);
+            if (st != FA_OK) return st;
             int rows = 0;
-            st = kmeans::cluster_ninit_device(C.vbx_ws, d_tr, Tn, e, target, 100, 10, 0ull, d_hard, d_cent, &rows, nullptr,
-                                              s, &lc);
+            st = kmeans::cluster_ninit_device(C.vbx_ws, d_tr, Tn, e, target, 100, 10, 0ull, d_hard, d_cent, &rows, nullptr, s);
             if (st != FA_OK) return st;
             st = ahc::launch_normalize_rows_keep(d_cent, d_cent_n, rows, e, s);   // normalize (:824-860) for the cosine
             if (st != FA_OK) return st;
-            lc += 1;
             K = rows;
             adjusted = true;
         }
@@ -326,7 +328,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     FA_CUDA_TRY(cudaEventRecord(C.ev[5], s));
     // ---- centroids (:345-353) + assignment (:371-374) -----------------------------------------------------
     if (!adjusted) {
-        st = vbx::centroids_device(C.vbx_ws, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s, &lc);
+        st = vbx::centroids_device(C.vbx_ws, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));
@@ -335,9 +337,8 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
             // no speaker with pi > 1e-7: computeCentroidsFromClusters(initialClusters) (:687-690)
             st = vbx::onehot_device(d_init, Tn, S, d_gamma, d_pi, s);
             if (st != FA_OK) return st;
-            st = vbx::centroids_device(C.vbx_ws, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s, &lc);
+            st = vbx::centroids_device(C.vbx_ws, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
             if (st != FA_OK) return st;
-            lc += 1;
             FA_CUDA_TRY(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
             FA_CUDA_TRY(cudaStreamSynchronize(s));
             K = *h_count;
@@ -352,21 +353,18 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
         // OfflineDiarizerManager.normalize on the one centroid (:824-860: a zero row is kept)
         st = ahc::launch_normalize_rows_keep(d_cent, d_cent_n, 1, e, s);
         if (st != FA_OK) return st;
-        ++lc;
         K = 1;
-        lc += 2;
     }
     // constrained assignment (:357-369) needs the full N x K score matrix on the host; plain argmax (:371-374) does not
     const bool constrained = chunk_index != nullptr && K > 1 && !adjusted;   // :357-360
     double *d_scores = nullptr;
     if (constrained) {
-        st = C.vbx_ws.reserve(std::max(C.vbx_ws.pool_bytes, N * (size_t)K * sizeof(double) + 1024));
+        st = carve_arena(C.vbx_ws.pool, C.vbx_ws.pool_bytes, [&](Carver &c) { d_scores = c.take<double>(N * (size_t)K); },
+                         1024);
         if (st != FA_OK) return st;
-        d_scores = static_cast<double *>(C.vbx_ws.pool);
     }
-    st = vbx::assign_device(d_emb, n, e, d_cent_n, nullptr, K, d_labels, d_scores, s, &lc);
+    st = vbx::assign_device(d_emb, n, e, d_cent_n, nullptr, K, d_labels, d_scores, s);
     if (st != FA_OK) return st;
-    g_launches += lc;
     if (constrained) {
         std::vector<double> h_scores(N * (size_t)K);
         FA_CUDA_TRY(cudaMemcpyAsync(h_scores.data(), d_scores, h_scores.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -390,15 +388,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
         FA_CUDA_TRY(cudaMemcpyAsync(hard_info.data(), d_hard, sizeof(int) * Tn, cudaMemcpyDeviceToHost, s));
     }
     FA_CUDA_TRY(cudaStreamSynchronize(s));
-    if (count_winners) {
-        std::vector<char> seen(S, 0);
-        detected = 0;
-        for (int i = 0; i < Tn; ++i)
-            if (hard_info[i] >= 0 && hard_info[i] < S && !seen[hard_info[i]]) {
-                seen[hard_info[i]] = 1;
-                ++detected;
-            }
-    }
+    if (count_winners) detected = distinct_winners(hard_info, S);
     if (info) {
         info->training_count = Tn;
         info->initial_clusters = S;
@@ -649,12 +639,10 @@ FA_API fa_status fa_mel_compute(fa_mel *mel, const float *audio, size_t n, float
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
     long long ml = 0, nf = 0;
-    const long long before = h->plan.launches;
     const double rate = h->plan.cfg.sample_rate;
     const resample::AudioFormat mono_f32{rate, rate, 1, resample::kPcmF32, 1, resample::kAlgoAuto};
     const int st = h->plan.compute_host(audio, (long long)n, mono_f32, last, mode, expected, layout, out,
                                         (long long)out_len, &ml, &nf, nullptr);
-    g_launches += h->plan.launches - before;
     if (mel_length) *mel_length = ml;
     if (num_frames) *num_frames = nf;
     return (fa_status)st;
@@ -668,10 +656,8 @@ FA_API fa_status fa_mel_compute_device(fa_mel *mel, const float *d_audio, size_t
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
     long long ml = 0, nf = 0;
-    const long long before = h->plan.launches;
     const int st = h->plan.compute_device(d_audio, (long long)n, last, mode, expected, layout, d_out, (long long)out_len,
                                           &ml, &nf, h->plan.streams[1]);
-    g_launches += h->plan.launches - before;
     if (mel_length) *mel_length = ml;
     if (num_frames) *num_frames = nf;
     return (fa_status)st;
@@ -685,13 +671,11 @@ FA_API fa_status fa_mel_compute_batch(fa_mel *mel, const float *audio, const int
         return FA_STATUS_INVALID_ARGUMENT;
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
-    const long long before = h->plan.launches;
     static_assert(sizeof(long long) == sizeof(int64_t), "int64 layout");
     const int st = h->plan.compute_batch_host(audio, reinterpret_cast<const long long *>(offsets), count, last, mode, layout,
                                               out, reinterpret_cast<const long long *>(out_offsets),
                                               reinterpret_cast<long long *>(mel_lengths),
                                               reinterpret_cast<long long *>(num_frames));
-    g_launches += h->plan.launches - before;
     return (fa_status)st;
     FA_GUARD_END
 }
@@ -703,12 +687,10 @@ FA_API fa_status fa_mel_compute_batch_device(fa_mel *mel, const float *d_audio, 
         return FA_STATUS_INVALID_ARGUMENT;
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
-    const long long before = h->plan.launches;
     const int st = h->plan.compute_batch_device(d_audio, reinterpret_cast<const long long *>(offsets), count, last, mode,
                                                 layout, d_out, reinterpret_cast<const long long *>(out_offsets),
                                                 reinterpret_cast<long long *>(mel_lengths),
                                                 reinterpret_cast<long long *>(num_frames), h->plan.streams[1]);
-    g_launches += h->plan.launches - before;
     return (fa_status)st;
     FA_GUARD_END
 }
@@ -764,10 +746,8 @@ static fa_status mel_stream_push(fa_mel *mel, int32_t count, const int32_t *sess
     if (!mel) return FA_STATUS_INVALID_ARGUMENT;
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
-    const long long before = h->plan.launches;
     const int st = h->sessions.push(h->plan, count, sessions, audio, reinterpret_cast<const long long *>(offsets), finish,
                                     device, out, (long long)out_len, reinterpret_cast<long long *>(frames));
-    g_launches += h->plan.launches - before;
     return (fa_status)st;
     FA_GUARD_END
 }
@@ -791,12 +771,10 @@ FA_API fa_status fa_mel_unified_features(fa_mel *mel, const float *window, size_
     if (!mel || !out || (!window && window_samples)) return FA_STATUS_INVALID_ARGUMENT;
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
-    const long long before = h->plan.launches;
     long long T = 0;
     int valid = 0;
     const int st = fa::mel::unified_features(h->plan, window, (long long)window_samples, (long long)valid_count, out,
                                              (long long)out_len, &T, &valid);
-    g_launches += h->plan.launches - before;
     if (total_frames) *total_frames = T;
     if (valid_frames) *valid_frames = valid;
     return (fa_status)st;
@@ -811,10 +789,8 @@ FA_API fa_status fa_mel_lseend_features(fa_mel *mel, const float *chunk, size_t 
         return FA_STATUS_INVALID_ARGUMENT;
     FA_GUARD_BEGIN
     auto *h = reinterpret_cast<MelHandle *>(mel);
-    const long long before = h->plan.launches;
     long long T = 0, count = *cmn_count;
     const int st = fa::mel::lseend_features(h->plan, chunk, (long long)n, cmn_mean, &count, out, (long long)out_len, &T);
-    g_launches += h->plan.launches - before;
     *cmn_count = count;
     if (frames) *frames = T;
     return (fa_status)st;
@@ -833,9 +809,7 @@ FA_API fa_status fa_mel_normalize_per_feature(float *x, int64_t frames, int32_t 
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    const int st = mel::normalize_per_feature_host(x, (long long)frames, n_mels, (long long)valid);
-    if (st == FA_OK) ++g_launches;
-    return (fa_status)st;
+    return (fa_status)mel::normalize_per_feature_host(x, (long long)frames, n_mels, (long long)valid);
     FA_GUARD_END
 }
 
@@ -897,9 +871,7 @@ FA_API fa_status fa_audio_resample(const void *pcm, int64_t frames, const fa_aud
         FA_CUDA_TRY(cudaMemcpyAsync(b.tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice, b.s));
     }
     FA_CUDA_TRY(cudaMemcpyAsync(b.pcm, pcm, bytes, cudaMemcpyHostToDevice, b.s));
-    long long launches = 0;
-    const int st = resample::launch_convert(b.pcm, frames, f, d, b.tab, b.out, 0, n, b.s, &launches);
-    g_launches += launches;
+    const int st = resample::launch_convert(b.pcm, frames, f, d, b.tab, b.out, 0, n, b.s);
     if (st != FA_OK) return (fa_status)st;
     FA_CUDA_TRY(cudaMemcpyAsync(out, b.out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, b.s));
     FA_CUDA_TRY(cudaStreamSynchronize(b.s));
@@ -920,10 +892,8 @@ FA_API fa_status fa_audio_to_mel(fa_mel *mel, const void *pcm, int64_t frames, c
         return FA_STATUS_INVALID_ARGUMENT;
     }
     long long ml = 0, nf = 0, rs = 0;
-    const long long before = h->plan.launches;
     const int st = h->plan.compute_host(pcm, (long long)frames, to_format(fmt), last, mode, -1, layout, out,
                                         (long long)out_len, &ml, &nf, &rs);
-    g_launches += h->plan.launches - before;
     if (mel_length) *mel_length = ml;
     if (num_frames) *num_frames = nf;
     if (resampled_count) *resampled_count = rs;
@@ -973,13 +943,9 @@ FA_API fastcluster_wrapper_status fastcluster_compute_centroid_linkage(const dou
     if (pointCount == 1) return FASTCLUSTER_WRAPPER_SUCCESS;
     try {
         if (require_device() != FA_OK) return FASTCLUSTER_WRAPPER_RUNTIME_ERROR;
-        Lease lease;
-        if (lease.status != FA_OK) return to_fc(lease.status);
-        const long long before = lease.ctx->solver.launches;
-        const int st = lease.ctx->solver.linkage_host(data, pointCount, dimension, dendrogramOut, dendrogramLength);
-        g_launches += lease.ctx->solver.launches - before;
-        lease.status = st == FA_CUDA_ERROR ? FA_CUDA_ERROR : FA_OK;
-        return to_fc(st);
+        return to_fc(with_context(0, [&](ClusterContext &C) {
+            return C.solver.linkage_host(data, pointCount, dimension, dendrogramOut, dendrogramLength);
+        }));
     } catch (const std::bad_alloc &) {
         return FASTCLUSTER_WRAPPER_ALLOCATION_FAILURE;
     } catch (const std::exception &) {
@@ -1000,20 +966,20 @@ FA_API fa_status fa_l2_normalize_rows(const double *x, size_t rows, size_t dim, 
     if (rows == 0 || dim == 0) return FA_STATUS_OK;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    ClusterContext &C = *lease.ctx;
-    int st = C.reserve(2 * rows * dim * sizeof(double) + 512, 64);
-    if (st != FA_OK) return (fa_status)st;
-    double *d_in = static_cast<double *>(C.d_buf);
-    double *d_out = d_in + rows * dim;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_in, x, rows * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    st = ahc::launch_normalize_rows(d_in, d_out, (int)rows, (int)dim, C.stream);
-    if (st != FA_OK) return (fa_status)st;
-    g_launches += 1;
-    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, rows * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-    return FA_STATUS_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
+        double *d_in, *d_out;
+        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+            d_in = c.take<double>(rows * dim);
+            d_out = c.take<double>(rows * dim);
+        }, 512);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(d_in, x, rows * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        st = ahc::launch_normalize_rows(d_in, d_out, (int)rows, (int)dim, C.stream);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, rows * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
@@ -1040,27 +1006,27 @@ FA_API fa_status fa_ahc_cluster(const double *features, size_t count, size_t dim
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    ClusterContext &C = *lease.ctx;
-    int st = C.reserve(2 * count * dim * sizeof(double) + 512, (count - 1) * 4 * sizeof(double) + 512);
-    if (st != FA_OK) return (fa_status)st;
-    double *d_in = static_cast<double *>(C.d_buf);
-    double *d_norm = d_in + count * dim;
-    double *h_Z = static_cast<double *>(C.h_buf);
-    FA_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    st = ahc::launch_normalize_rows(d_in, d_norm, (int)count, (int)dim, C.stream);
-    if (st != FA_OK) return (fa_status)st;
-    const long long before = C.solver.launches;
-    st = C.solver.linkage_device(d_norm, (int)count, (int)dim, h_Z);
-    g_launches += 1 + C.solver.launches - before;
-    if (st == FA_RUNTIME_ERROR || st == FA_UNSUPPORTED) {      // FFI failure -> Array(0..<count) (:52-55)
-        for (size_t i = 0; i < count; ++i) labels[i] = (int32_t)i;
-        return FA_STATUS_OK;
-    }
-    if (st != FA_OK) return (fa_status)st;
-    ahc::dendrogram_cut(h_Z, (long long)count, threshold, labels);
-    return FA_STATUS_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
+        double *d_in, *d_norm, *h_Z;
+        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+            d_in = c.take<double>(count * dim);
+            d_norm = c.take<double>(count * dim);
+        }, 512);
+        if (st != FA_OK) return st;
+        st = carve_arena(C.h_buf, C.h_bytes, [&](Carver &c) { h_Z = c.take<double>((count - 1) * 4); }, 512, true);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        st = ahc::launch_normalize_rows(d_in, d_norm, (int)count, (int)dim, C.stream);
+        if (st != FA_OK) return st;
+        st = C.solver.linkage_device(d_norm, (int)count, (int)dim, h_Z);
+        if (st == FA_RUNTIME_ERROR || st == FA_UNSUPPORTED) {      // FFI failure -> Array(0..<count) (:52-55)
+            for (size_t i = 0; i < count; ++i) labels[i] = (int32_t)i;
+            return FA_OK;
+        }
+        if (st != FA_OK) return st;
+        ahc::dendrogram_cut(h_Z, (long long)count, threshold, labels);
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
@@ -1163,32 +1129,27 @@ FA_API fa_status fa_kmeans_cluster(const double *emb, size_t N, size_t D, int32_
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    ClusterContext &C = *lease.ctx;
-    Carver sz{nullptr};
-    sz.take<double>(N * D);
-    sz.take<double>((size_t)rows_needed * D);
-    sz.take<int>(N);
-    int st = C.reserve(sz.off + 1024, 64);
-    if (st != FA_OK) return (fa_status)st;
-    Carver c{static_cast<char *>(C.d_buf)};
-    double *d_emb = c.take<double>(N * D);
-    double *d_cent = c.take<double>((size_t)rows_needed * D);
-    int *d_labels = c.take<int>(N);
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    long long lc = 0;
-    int rows = 0, best = 0;
-    st = kmeans::cluster_ninit_device(C.vbx_ws, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
-                                      d_labels, d_cent, &rows, &best, C.stream, &lc);
-    g_launches += lc;
-    if (st != FA_OK) return (fa_status)st;
-    FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)rows * D * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-    if (centroid_rows) *centroid_rows = rows;
-    if (best_init) *best_init = best;
-    return FA_STATUS_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
+        double *d_emb, *d_cent;
+        int *d_labels;
+        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+            d_emb = c.take<double>(N * D);
+            d_cent = c.take<double>((size_t)rows_needed * D);
+            d_labels = c.take<int>(N);
+        }, 1024);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        int rows = 0, best = 0;
+        st = kmeans::cluster_ninit_device(C.vbx_ws, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
+                                          d_labels, d_cent, &rows, &best, C.stream);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)rows * D * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        if (centroid_rows) *centroid_rows = rows;
+        if (best_init) *best_init = best;
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
@@ -1198,49 +1159,35 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
     if (!rho || !cfg || !gamma || !pi || !elbos || !hard || T == 0 || D == 0 || S <= 0) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    ClusterContext &C = *lease.ctx;
-    const int cap = std::max(cfg->max_iterations, 1);
-    Carver sz{nullptr};
-    sz.take<double>(T * D);
-    sz.take<int>(T);
-    sz.take<double>(T * (size_t)S);
-    sz.take<double>(S);
-    sz.take<double>(cap);
-    sz.take<int>(T);
-    int st = C.reserve(sz.off + 1024, 64);
-    if (st != FA_OK) return (fa_status)st;
-    Carver c{static_cast<char *>(C.d_buf)};
-    double *d_x = c.take<double>(T * D);
-    int *d_init = c.take<int>(T);
-    double *d_gamma = c.take<double>(T * (size_t)S);
-    double *d_pi = c.take<double>(S);
-    double *d_elbos = c.take<double>(cap);
-    int *d_hard = c.take<int>(T);
-    std::vector<double> psi_eff(D, 1.0);
-    if (psi && psi_len == D) std::memcpy(psi_eff.data(), psi, D * sizeof(double));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    if (initial) FA_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
-    vbx::Config vc;
-    vc.Fa = cfg->Fa;
-    vc.Fb = cfg->Fb;
-    vc.max_iterations = cfg->max_iterations;
-    vc.epsilon = cfg->epsilon;
-    vc.init_smoothing = cfg->init_smoothing;
-    int its = 0;
-    long long lc = 0;
-    st = vbx::refine_device(C.vbx_ws, d_x, (int)T, (int)D, psi_eff.data(), initial ? d_init : nullptr, S, vc, d_gamma,
-                            d_pi, d_elbos, d_hard, &its, C.stream, &lc);
-    g_launches += lc;
-    if (st != FA_OK) return (fa_status)st;
-    FA_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(pi, d_pi, S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(elbos, d_elbos, cap * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(hard, d_hard, T * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-    if (iterations) *iterations = its;
-    return FA_STATUS_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
+        const int cap = std::max(cfg->max_iterations, 1);
+        double *d_x, *d_gamma, *d_pi, *d_elbos;
+        int *d_init, *d_hard;
+        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+            d_x = c.take<double>(T * D);
+            d_init = c.take<int>(T);
+            d_gamma = c.take<double>(T * (size_t)S);
+            d_pi = c.take<double>(S);
+            d_elbos = c.take<double>(cap);
+            d_hard = c.take<int>(T);
+        }, 1024);
+        if (st != FA_OK) return st;
+        std::vector<double> psi_eff(D, 1.0);
+        if (psi && psi_len == D) std::memcpy(psi_eff.data(), psi, D * sizeof(double));
+        FA_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        if (initial) FA_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
+        int its = 0;
+        st = vbx::refine_device(C.vbx_ws, d_x, (int)T, (int)D, psi_eff.data(), initial ? d_init : nullptr, S, to_vbx(*cfg),
+                                d_gamma, d_pi, d_elbos, d_hard, &its, C.stream);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(pi, d_pi, S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(elbos, d_elbos, cap * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(hard, d_hard, T * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        if (iterations) *iterations = its;
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
@@ -1250,41 +1197,33 @@ FA_API fa_status fa_compute_centroids(const double *emb, size_t T, size_t dim, c
         return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    ClusterContext &C = *lease.ctx;
-    Carver sz{nullptr};
-    sz.take<double>(T * dim);
-    sz.take<double>(T * (size_t)S);
-    sz.take<double>(S);
-    sz.take<double>((size_t)S * dim);
-    sz.take<double>((size_t)S * dim);
-    sz.take<int>(64);
-    int st = C.reserve(sz.off + 1024, 64);
-    if (st != FA_OK) return (fa_status)st;
-    Carver c{static_cast<char *>(C.d_buf)};
-    double *d_emb = c.take<double>(T * dim);
-    double *d_gamma = c.take<double>(T * (size_t)S);
-    double *d_pi = c.take<double>(S);
-    double *d_cent = c.take<double>((size_t)S * dim);
-    double *d_cent_n = c.take<double>((size_t)S * dim);
-    int *d_count = c.take<int>(64);
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    long long lc = 0;
-    st = vbx::centroids_device(C.vbx_ws, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream, &lc);
-    g_launches += lc;
-    if (st != FA_OK) return (fa_status)st;
-    int K = 0;
-    FA_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-    *centroid_count = K;
-    if (K > 0) {
-        FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)K * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
+        double *d_emb, *d_gamma, *d_pi, *d_cent, *d_cent_n;
+        int *d_count;
+        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+            d_emb = c.take<double>(T * dim);
+            d_gamma = c.take<double>(T * (size_t)S);
+            d_pi = c.take<double>(S);
+            d_cent = c.take<double>((size_t)S * dim);
+            d_cent_n = c.take<double>((size_t)S * dim);
+            d_count = c.take<int>(64);
+        }, 1024);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        st = vbx::centroids_device(C.vbx_ws, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream);
+        if (st != FA_OK) return st;
+        int K = 0;
+        FA_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
         FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-    }
-    return FA_STATUS_OK;
+        *centroid_count = K;
+        if (K > 0) {
+            FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)K * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+            FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        }
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
@@ -1298,43 +1237,37 @@ FA_API fa_status fa_assign_embeddings(const double *emb, size_t N, size_t dim, c
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    ClusterContext &C = *lease.ctx;
-    Carver sz{nullptr};
-    sz.take<double>(N * dim);
-    sz.take<double>((size_t)K * dim);
-    sz.take<double>((size_t)K * dim);
-    sz.take<int>(N);
-    sz.take<double>(scores ? N * (size_t)K : 1);
-    int st = C.reserve(sz.off + 1024, 64);
-    if (st != FA_OK) return (fa_status)st;
-    Carver c{static_cast<char *>(C.d_buf)};
-    double *d_emb = c.take<double>(N * dim);
-    double *d_craw = c.take<double>((size_t)K * dim);
-    double *d_cn = c.take<double>((size_t)K * dim);
-    int *d_labels = c.take<int>(N);
-    double *d_scores = c.take<double>(scores ? N * (size_t)K : 1);
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_craw, centroids, (size_t)K * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    // centroid normalisation (:793, :824-860; zero rows kept) with the same kernel the pipeline uses
-    st = ahc::launch_normalize_rows_keep(d_craw, d_cn, K, (int)dim, C.stream);
-    if (st != FA_OK) return (fa_status)st;
-    ++g_launches;
-    long long lc = 0;
-    st = vbx::assign_device(d_emb, (int)N, (int)dim, d_cn, nullptr, K, d_labels, scores ? d_scores : nullptr, C.stream, &lc);
-    g_launches += lc;
-    if (st != FA_OK) return (fa_status)st;
-    FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    if (scores) FA_CUDA_TRY(cudaMemcpyAsync(scores, d_scores, N * (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-    return FA_STATUS_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
+        double *d_emb, *d_craw, *d_cn, *d_scores;
+        int *d_labels;
+        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+            d_emb = c.take<double>(N * dim);
+            d_craw = c.take<double>((size_t)K * dim);
+            d_cn = c.take<double>((size_t)K * dim);
+            d_labels = c.take<int>(N);
+            d_scores = c.take<double>(scores ? N * (size_t)K : 1);
+        }, 1024);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(d_craw, centroids, (size_t)K * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
+        // centroid normalisation (:793, :824-860; zero rows kept) with the same kernel the pipeline uses
+        st = ahc::launch_normalize_rows_keep(d_craw, d_cn, K, (int)dim, C.stream);
+        if (st != FA_OK) return st;
+        st = vbx::assign_device(d_emb, (int)N, (int)dim, d_cn, nullptr, K, d_labels, scores ? d_scores : nullptr, C.stream);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+        if (scores)
+            FA_CUDA_TRY(cudaMemcpyAsync(scores, d_scores, N * (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
-FA_API fa_status fa_diarize_cluster(const float *emb256, const double *rho, size_t N, size_t emb_dim, size_t rho_dim,
-                                    const double *psi, const fa_cluster_config *cfg, int32_t *labels, int32_t *initial,
-                                    double *centroids, int32_t max_centroids, fa_cluster_info *info) {
+static fa_status diarize_cluster(const float *emb256, const double *rho, size_t N, size_t emb_dim, size_t rho_dim,
+                                 const double *psi, const fa_cluster_config *cfg, const int32_t *chunk_index,
+                                 int32_t *labels, int32_t *initial, double *centroids, int32_t max_centroids,
+                                 fa_cluster_info *info) {
     if (!emb256 || !rho || !cfg || !labels || N == 0 || emb_dim == 0 || rho_dim == 0) {
         fa::set_error("fa_diarize_cluster: null or empty input (the reference throws noSpeechDetected for N == 0)");
         return FA_STATUS_INVALID_ARGUMENT;
@@ -1342,30 +1275,26 @@ FA_API fa_status fa_diarize_cluster(const float *emb256, const double *rho, size
     if (N > 0x7fffffffull / 4) return FA_STATUS_INDEX_OVERFLOW;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    const int st = cluster_pipeline(*lease.ctx, emb256, rho, N, emb_dim, rho_dim, psi, *cfg, labels, initial, centroids,
-                                    max_centroids, info);
-    lease.status = st == FA_CUDA_ERROR ? FA_CUDA_ERROR : FA_OK;
-    return (fa_status)st;
+    return (fa_status)with_context(0, [&](ClusterContext &C) {
+        return cluster_pipeline(C, emb256, rho, N, emb_dim, rho_dim, psi, *cfg, labels, initial, centroids, max_centroids,
+                                info, chunk_index);
+    });
     FA_GUARD_END
+}
+
+FA_API fa_status fa_diarize_cluster(const float *emb256, const double *rho, size_t N, size_t emb_dim, size_t rho_dim,
+                                    const double *psi, const fa_cluster_config *cfg, int32_t *labels, int32_t *initial,
+                                    double *centroids, int32_t max_centroids, fa_cluster_info *info) {
+    return diarize_cluster(emb256, rho, N, emb_dim, rho_dim, psi, cfg, nullptr, labels, initial, centroids, max_centroids,
+                           info);
 }
 
 FA_API fa_status fa_diarize_cluster_chunks(const float *emb256, const double *rho, size_t N, size_t emb_dim,
                                            size_t rho_dim, const double *psi, const fa_cluster_config *cfg,
                                            const int32_t *chunk_index, int32_t *labels, int32_t *initial,
                                            double *centroids, int32_t max_centroids, fa_cluster_info *info) {
-    if (!emb256 || !rho || !cfg || !labels || N == 0 || emb_dim == 0 || rho_dim == 0) return FA_STATUS_INVALID_ARGUMENT;
-    if (N > 0x7fffffffull / 4) return FA_STATUS_INDEX_OVERFLOW;
-    API_REQUIRE_DEVICE();
-    FA_GUARD_BEGIN
-    Lease lease;
-    if (lease.status != FA_OK) return (fa_status)lease.status;
-    const int st = cluster_pipeline(*lease.ctx, emb256, rho, N, emb_dim, rho_dim, psi, *cfg, labels, initial, centroids,
-                                    max_centroids, info, chunk_index);
-    lease.status = st == FA_CUDA_ERROR ? FA_CUDA_ERROR : FA_OK;
-    return (fa_status)st;
-    FA_GUARD_END
+    return diarize_cluster(emb256, rho, N, emb_dim, rho_dim, psi, cfg, chunk_index, labels, initial, centroids,
+                           max_centroids, info);
 }
 
 FA_API fa_status fa_hungarian_solve(const int64_t *cost, int32_t n, int32_t *assignment) {
@@ -1443,26 +1372,21 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
             status[lane] = FA_CUDA_ERROR;
             return;
         }
-        Lease lease(worker_limit);
-        if (lease.status != FA_OK) {
-            status[lane] = lease.status;
-            messages[lane] = fa::last_error();
-            return;
-        }
-        for (;;) {
-            const int m = next.fetch_add(1);
-            if (m >= set_count) break;
-            const int64_t a = set_offsets[m], b = set_offsets[m + 1];
-            if (b <= a) continue;
-            const int st = cluster_pipeline(*lease.ctx, emb256 + (size_t)a * emb_dim, rho + (size_t)a * rho_dim,
-                                            (size_t)(b - a), emb_dim, rho_dim, psi, *cfg, labels + a, nullptr, nullptr,
-                                            0, infos ? infos + m : nullptr, chunk_index ? chunk_index + a : nullptr);
-            if (st != FA_OK) {
-                status[lane] = st;
-                messages[lane] = fa::last_error();
-                lease.status = st == FA_CUDA_ERROR ? FA_CUDA_ERROR : FA_OK;
-                break;
+        const int st = with_context(worker_limit, [&](ClusterContext &C) {
+            for (;;) {
+                const int m = next.fetch_add(1);
+                if (m >= set_count) return (int)FA_OK;
+                const int64_t a = set_offsets[m], b = set_offsets[m + 1];
+                if (b <= a) continue;
+                const int st = cluster_pipeline(C, emb256 + (size_t)a * emb_dim, rho + (size_t)a * rho_dim, (size_t)(b - a),
+                                                emb_dim, rho_dim, psi, *cfg, labels + a, nullptr, nullptr, 0,
+                                                infos ? infos + m : nullptr, chunk_index ? chunk_index + a : nullptr);
+                if (st != FA_OK) return st;
             }
+        });
+        if (st != FA_OK) {
+            status[lane] = st;
+            messages[lane] = fa::last_error();
         }
     };
     auto run = [&](int lane) noexcept {

@@ -5,6 +5,8 @@
 #include <cstdint>
 
 #if defined(__CUDACC__)
+#include <atomic>
+#include <utility>
 #include <cuda_runtime.h>
 #define FA_HD __host__ __device__ __forceinline__
 #else
@@ -33,17 +35,16 @@ void set_error(const char *fmt, ...);
 const char *last_error();
 
 // Slices one allocation into 256-byte aligned arrays.  Carver{nullptr} is a dry run: `off` then holds the bytes the
-// arrays need, and at<T>() returns offsets for layouts computed before the allocation exists.
+// arrays need (carve_arena below runs a layout both ways).
 struct Carver {
     char *base = nullptr;
     size_t off = 0;
-    template <typename T> size_t at(size_t count) {
+    template <typename T> T *take(size_t count) {
         off = (off + 255) & ~size_t(255);
-        const size_t p = off;
+        T *p = reinterpret_cast<T *>(base + off);
         off += count * sizeof(T);
         return p;
     }
-    template <typename T> T *take(size_t count) { return reinterpret_cast<T *>(base + at<T>(count)); }
 };
 
 #if defined(__CUDACC__)
@@ -75,6 +76,45 @@ template <typename T> int grow_buffer(T *&p, size_t &cap, size_t bytes, bool pin
     p = static_cast<T *>(q);
     cap = bytes;
     return FA_OK;
+}
+
+// Lays out one scratch arena in a grow-only buffer.  `layout(Carver &)` takes every array of the arena in order and
+// only assigns the pointers it gets, so it is safe to run twice: once over a null base to size the arena (plus `slack`
+// bytes), then, after the buffer has grown to that size, over the buffer itself.
+template <typename T, typename Layout>
+int carve_arena(T *&buf, size_t &cap, Layout &&layout, size_t slack = 0, bool pinned = false) {
+    Carver size{nullptr};
+    layout(size);
+    const int st = grow_buffer(buf, cap, size.off + slack, pinned);
+    if (st != FA_OK) return st;
+    Carver c{static_cast<char *>(static_cast<void *>(buf))};
+    layout(c);
+    return FA_OK;
+}
+
+// Kernel launches of the whole process (fa_kernel_launch_count), defined in capi.cu.  Every launch of the library goes
+// through launch() or launch_cooperative(), which count it where it is issued and return its error:
+// FA_CUDA_TRY(fa::launch(kernel, grid, block, smem, stream, args...)).
+extern std::atomic<long long> g_launches;
+
+template <typename... Params, typename... Args>
+cudaError_t launch(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args &&...args) {
+    kernel<<<grid, block, smem, stream>>>(std::forward<Args>(args)...);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
+}
+
+// The same for a kernel whose CTAs must all be resident at once (grid-wide synchronisation).  The arguments are
+// converted to the kernel's parameter types (the kernel alone fixes them), since the launch passes their addresses.
+template <typename T> struct kernel_param { using type = T; };
+template <typename... Params>
+cudaError_t launch_cooperative(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                               typename kernel_param<Params>::type... args) {
+    void *argv[] = {&args...};
+    const cudaError_t e =
+        cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kernel), grid, block, argv, smem, stream);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 // Properties of device `dev`, which must be sm_90: the library carries sm_90a code only.

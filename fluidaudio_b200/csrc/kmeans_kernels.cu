@@ -221,8 +221,7 @@ void resolve_constraints(long long num_embeddings, long long num_speakers, long 
 
 int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, int num_clusters, int max_iterations,
                          int n_init, unsigned long long base_seed, int *d_labels, double *d_centroids, int *rows,
-                         int *best_init, cudaStream_t s, long long *launches) {
-    long long lc = 0;
+                         int *best_init, cudaStream_t s) {
     if (rows) *rows = 0;
     if (best_init) *best_init = 0;
     if (N <= 0) return FA_OK;
@@ -236,11 +235,9 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
         return FA_OK;
     }
     if (N <= k) {                                             // :60-62: identity, centroids = the raw embeddings
-        iota_kernel<<<(N + 255) / 256, 256, 0, s>>>(d_labels, N);
-        FA_CUDA_TRY(cudaGetLastError());
+        FA_CUDA_TRY(fa::launch(iota_kernel, (N + 255) / 256, 256, 0, s, d_labels, N));
         FA_CUDA_TRY(cudaMemcpyAsync(d_centroids, d_emb, sizeof(double) * (size_t)N * D, cudaMemcpyDeviceToDevice, s));
         if (rows) *rows = N;
-        if (launches) *launches += 1;
         return FA_OK;
     }
     if (k > 1024) {
@@ -248,35 +245,24 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
         return FA_UNSUPPORTED;
     }
     const int runs = (N > num_clusters && n_init > 1) ? n_init : 1;   // :106-110
-    size_t need;
-    {
-        Carver c{nullptr};
-        c.take<double>((size_t)N * D);
-        c.take<double>((size_t)N * D);
-        c.take<double>((size_t)k * D);
-        c.take<double>((size_t)N);
-        c.take<int>((size_t)N * 3);
-        c.take<int>((size_t)k);
-        c.take<RunState>(1);
-        need = c.off + 4096;
-    }
-    int st = ws.reserve(std::max(ws.pool_bytes, need));
+    double *d_x, *d_xt, *d_cent, *d_pp;
+    int *d_perm, *d_lab[2], *d_counts;
+    RunState *d_state;
+    const int st = carve_arena(ws.pool, ws.pool_bytes, [&](Carver &c) {
+        d_x = c.take<double>((size_t)N * D);
+        d_xt = c.take<double>((size_t)N * D);
+        d_cent = c.take<double>((size_t)k * D);
+        d_pp = c.take<double>((size_t)N);
+        d_perm = c.take<int>(N);
+        d_lab[0] = c.take<int>(N);
+        d_lab[1] = c.take<int>(N);
+        d_counts = c.take<int>(k);
+        d_state = c.take<RunState>(1);
+    }, 4096);
     if (st != FA_OK) return st;
-    Carver c{static_cast<char *>(ws.pool)};
-    double *d_x = c.take<double>((size_t)N * D);
-    double *d_xt = c.take<double>((size_t)N * D);
-    double *d_cent = c.take<double>((size_t)k * D);
-    double *d_pp = c.take<double>((size_t)N);
-    int *d_perm = c.take<int>(N);
-    int *d_lab[2] = {c.take<int>(N), c.take<int>(N)};
-    int *d_counts = c.take<int>(k);
-    RunState *d_state = c.take<RunState>(1);
 
-    normalize_kernel<<<(N + 127) / 128, 128, 0, s>>>(d_emb, N, D, d_x);
-    FA_CUDA_TRY(cudaGetLastError());
-    transpose_kernel<<<dim3((N + 31) / 32, (D + 31) / 32), dim3(32, 8), 0, s>>>(d_x, N, D, d_xt);
-    FA_CUDA_TRY(cudaGetLastError());
-    lc += 2;
+    FA_CUDA_TRY(fa::launch(normalize_kernel, (N + 127) / 128, 128, 0, s, d_emb, N, D, d_x));
+    FA_CUDA_TRY(fa::launch(transpose_kernel, dim3((N + 31) / 32, (D + 31) / 32), dim3(32, 8), 0, s, d_x, N, D, d_xt));
 
     double best = DBL_MAX;
     RunState h{};
@@ -292,21 +278,18 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
         }
         FA_CUDA_TRY(cudaMemcpyAsync(d_perm, perm.data(), sizeof(int) * k, cudaMemcpyHostToDevice, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));   // perm is reused by the next run
-        init_run_kernel<<<1, 256, 0, s>>>(d_x, N, D, k, d_perm, g.state, d_cent, d_lab[1], d_state);
-        FA_CUDA_TRY(cudaGetLastError());
-        lc += 1;
+        FA_CUDA_TRY(fa::launch(init_run_kernel, 1, 256, 0, s, d_x, N, D, k, d_perm, g.state, d_cent, d_lab[1], d_state));
         int it = 0;
         bool done = false;
         while (it < max_iterations && !done) {
             const int batch = std::min(8, max_iterations - it);
             for (int b = 0; b < batch; ++b, ++it) {
                 int *fresh = d_lab[it & 1], *prev = d_lab[(it & 1) ^ 1];
-                assign_kernel<<<(N + 127) / 128, 128, 0, s>>>(d_xt, N, D, d_cent, k, prev, fresh, d_state);
-                update_kernel<<<dim3((D + 127) / 128, k), 128, 0, s>>>(d_x, N, D, fresh, k, d_cent, d_counts, d_state);
-                finish_iteration_kernel<<<1, 256, 0, s>>>(d_x, N, D, k, d_cent, d_counts, d_state);
-                lc += 3;
+                FA_CUDA_TRY(fa::launch(assign_kernel, (N + 127) / 128, 128, 0, s, d_xt, N, D, d_cent, k, prev, fresh, d_state));
+                FA_CUDA_TRY(fa::launch(update_kernel, dim3((D + 127) / 128, k), 128, 0, s, d_x, N, D, fresh, k, d_cent, d_counts,
+                                       d_state));
+                FA_CUDA_TRY(fa::launch(finish_iteration_kernel, 1, 256, 0, s, d_x, N, D, k, d_cent, d_counts, d_state));
             }
-            FA_CUDA_TRY(cudaGetLastError());
             FA_CUDA_TRY(cudaMemcpyAsync(&h, d_state, sizeof(RunState), cudaMemcpyDeviceToHost, s));
             FA_CUDA_TRY(cudaStreamSynchronize(s));
             done = h.done != 0;
@@ -315,10 +298,8 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
         // in iteration `iterations` (equal to the previous one); after max_iterations full rounds it is the last.
         const int last = h.done ? h.iterations : (max_iterations - 1);
         const int *final_labels = max_iterations > 0 ? d_lab[last & 1] : d_lab[1];
-        point_inertia_kernel<<<(N + 127) / 128, 128, 0, s>>>(d_xt, N, D, d_cent, k, final_labels, d_pp);
-        sum_inertia_kernel<<<1, 1, 0, s>>>(d_pp, N, d_state);
-        lc += 2;
-        FA_CUDA_TRY(cudaGetLastError());
+        FA_CUDA_TRY(fa::launch(point_inertia_kernel, (N + 127) / 128, 128, 0, s, d_xt, N, D, d_cent, k, final_labels, d_pp));
+        FA_CUDA_TRY(fa::launch(sum_inertia_kernel, 1, 1, 0, s, d_pp, N, d_state));
         FA_CUDA_TRY(cudaMemcpyAsync(&h, d_state, sizeof(RunState), cudaMemcpyDeviceToHost, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));
         // :122-125: strictly lower inertia wins.  Run 0 (the base seed) is always taken first, so a NaN inertia in every
@@ -334,7 +315,6 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
     }
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     if (rows) *rows = k;
-    if (launches) *launches += lc;
     return FA_OK;
 }
 

@@ -13,7 +13,7 @@ namespace kmeans {
 // *best_init the index of the winning seed.  Scratch comes from `ws`.
 int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, int num_clusters, int max_iterations,
                          int n_init, unsigned long long base_seed, int *d_labels, double *d_centroids, int *rows,
-                         int *best_init, cudaStream_t stream, long long *launches);
+                         int *best_init, cudaStream_t stream);
 
 // SpeakerCountConstraints.resolve; absent options are FA_NO_VALUE (INT32_MIN).
 void resolve_constraints(long long num_embeddings, long long num_speakers, long long min_speakers, long long max_speakers,

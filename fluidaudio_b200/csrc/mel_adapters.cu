@@ -85,8 +85,8 @@ int normalize_per_feature_host(float *x, long long T, int M, long long valid) {
     const size_t bytes = sizeof(float) * (size_t)T * M;
     FA_CUDA_TRY(cudaMalloc(&b.d, bytes));
     FA_CUDA_TRY(cudaMemcpy(b.d, x, bytes, cudaMemcpyHostToDevice));
-    per_feature_norm_inplace_kernel<<<(M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta>>>(b.d, T, M, valid);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(per_feature_norm_inplace_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, 0, b.d, T,
+                           M, valid));
     FA_CUDA_TRY(cudaMemcpy(x, b.d, bytes, cudaMemcpyDeviceToHost));
     return FA_OK;
 }
@@ -127,9 +127,8 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
     if (valid <= 0) {
         FA_CUDA_TRY(cudaMemsetAsync(d_pack, 0, sizeof(float) * T * M, s));
     } else {
-        per_feature_norm_kernel<<<(M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, s>>>(d_flat, T, M, valid, d_pack);
-        FA_CUDA_TRY(cudaGetLastError());
-        ++p.launches;
+        FA_CUDA_TRY(fa::launch(per_feature_norm_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, s, d_flat, T, M,
+                               valid, d_pack));
     }
     FA_CUDA_TRY(cudaMemcpyAsync(out, d_pack, sizeof(float) * T * M, cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));
@@ -156,9 +155,7 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
     st = p.compute_device(p.d_audio, n, 0.0f, 1, -1, 0, d_flat, T * M, &ml, &nf, s);
     if (st != FA_OK) return st;
     const float scale = 1.0f / logf(10.0f);   // LSEENDPreprocessor.swift:36, Float arithmetic
-    lseend_scale_cmn_kernel<<<(M + 127) / 128, 128, 0, s>>>(d_flat, T, M, d_mean, *cmn_count, scale);
-    FA_CUDA_TRY(cudaGetLastError());
-    ++p.launches;
+    FA_CUDA_TRY(fa::launch(lseend_scale_cmn_kernel, (M + 127) / 128, 128, 0, s, d_flat, T, M, d_mean, *cmn_count, scale));
     FA_CUDA_TRY(cudaMemcpyAsync(out, d_flat, sizeof(float) * T * M, cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaMemcpyAsync(cmn_mean, d_mean, sizeof(float) * M, cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));

@@ -776,22 +776,14 @@ int MelPlan::launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, con
         GenericParams G{cfg.n_fft, generic_log2n, cfg.n_fft / 2 + 1, generic_prow, reinterpret_cast<const cpxd *>(d_generic_tw),
                         generic_warps};
         const int ggrid = std::min(total_tiles, num_sms * std::max(1, 16 / generic_warps));
-        mel_generic_kernel<<<ggrid, generic_warps * 32, smem_bytes, stream>>>(P, G);
-        FA_CUDA_TRY(cudaGetLastError());
-        ++launches;
+        FA_CUDA_TRY(fa::launch(mel_generic_kernel, ggrid, generic_warps * 32, smem_bytes, stream, P, G));
         return FA_OK;
     }
     const int grid = std::min(total_tiles, num_sms * kCtasPerSm);
     const dim3 blk(kWarpsPerCta * 32);
-    if (precision == 1) {
-        if (layout == 0) mel512_kernel<kWarpsPerCta, f32x2, 0><<<grid, blk, smem_bytes, stream>>>(P);
-        else mel512_kernel<kWarpsPerCta, f32x2, 1><<<grid, blk, smem_bytes, stream>>>(P);
-    } else {
-        if (layout == 0) mel512_kernel<kWarpsPerCta, double, 0><<<grid, blk, smem_bytes, stream>>>(P);
-        else mel512_kernel<kWarpsPerCta, double, 1><<<grid, blk, smem_bytes, stream>>>(P);
-    }
-    FA_CUDA_TRY(cudaGetLastError());
-    ++launches;
+    auto kernel = precision == 1 ? (layout == 0 ? mel512_kernel<kWarpsPerCta, f32x2, 0> : mel512_kernel<kWarpsPerCta, f32x2, 1>)
+                                 : (layout == 0 ? mel512_kernel<kWarpsPerCta, double, 0> : mel512_kernel<kWarpsPerCta, double, 1>);
+    FA_CUDA_TRY(fa::launch(kernel, grid, blk, smem_bytes, stream, P));
     return FA_OK;
 }
 
@@ -1062,7 +1054,7 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
                 fa::set_error("internal: resampler window accounting (%lld < %lld)", ready, s_end);
                 return FA_RUNTIME_ERROR;
             }
-            st = resample::launch_convert(d_pcm, frames, f, D, d_rs_tab, d_audio, converted, s_end, s_k, &launches);
+            st = resample::launch_convert(d_pcm, frames, f, D, d_rs_tab, d_audio, converted, s_end, s_k);
             if (st != FA_OK) return st;
             converted = std::max(converted, s_end);
         }

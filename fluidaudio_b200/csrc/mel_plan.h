@@ -80,7 +80,6 @@ struct MelPlan {
     int pt_len = 0, pt_cap = 0, raw_cap = 0;
     size_t smem_bytes = 0;
     int num_sms = 0;
-    long long launches = 0;          // kernels launched through this plan (bench.py reports it)
     int precision = 0;               // transform arithmetic: 0 = FP64 (one frame per warp), 1 = float32 frame pairs
     int pipeline_chunks = 24;        // units a long host-buffer call is cut into (H2D / kernel / D2H overlap)
     bool zero_copy_out = false;      // time-major output in a pinned host buffer: the kernel stores straight into it

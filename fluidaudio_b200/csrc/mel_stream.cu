@@ -312,9 +312,8 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         desc_in_flight = true;
     }
     if (jobs) {
-        mel_stream_ingest_kernel<<<jobs, kIngestThreads, 0, s>>>(dj, src, d_carry, d_last, d_arena, du, capacity, c.preemph);
-        FA_CUDA_TRY(cudaGetLastError());
-        ++p.launches;
+        FA_CUDA_TRY(fa::launch(mel_stream_ingest_kernel, jobs, kIngestThreads, 0, s, dj, src, d_carry, d_last, d_arena, du,
+                               capacity, c.preemph));
     }
     float *k_out = device ? out : p.d_out;
     if (units) {

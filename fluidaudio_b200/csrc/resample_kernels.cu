@@ -239,28 +239,24 @@ static int launch_sinc(const Source &s, const Design &d, const float *d_tab, flo
     const size_t smem = sizeof(float) * (size_t)sinc_smem_floats(d.L, d.M, d.taps);
     if (smem > 48 * 1024)
         FA_CUDA_TRY(cudaFuncSetAttribute(sinc_kernel<Idx>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sinc_kernel<Idx><<<grid, kSincBlock, smem, stream>>>(s, d.L, d.M, d.half, d.phases, d.exact ? 1 : 0, d.row_stride,
-                                                          d_tab, d_out, o_begin, o_end);
+    FA_CUDA_TRY(fa::launch(sinc_kernel<Idx>, grid, kSincBlock, smem, stream, s, d.L, d.M, d.half, d.phases, d.exact ? 1 : 0,
+                           d.row_stride, d_tab, d_out, o_begin, o_end));
     return FA_OK;
 }
 
 int launch_convert(const void *d_pcm, long long frames, const AudioFormat &f, const Design &d, const float *d_tab,
-                   float *d_out, long long o_begin, long long o_end, cudaStream_t stream, long long *launches) {
+                   float *d_out, long long o_begin, long long o_end, cudaStream_t stream) {
     if (o_end <= o_begin) return FA_OK;
     Source s{d_pcm, frames, f.channels, f.format, f.interleaved, 1.0f / (float)f.channels};
     const unsigned grid = (unsigned)((o_end - o_begin + 255) / 256);
     if (f.in_rate == f.out_rate) {
-        mixdown_kernel<<<grid, 256, 0, stream>>>(s, d_out, o_begin, o_end);
+        FA_CUDA_TRY(fa::launch(mixdown_kernel, grid, 256, 0, stream, s, d_out, o_begin, o_end));
     } else if (resolve_algorithm(f) == kAlgoLinear) {
-        linear_kernel<<<grid, 256, 0, stream>>>(s, f.in_rate / f.out_rate, d_out, o_begin, o_end);
+        FA_CUDA_TRY(fa::launch(linear_kernel, grid, 256, 0, stream, s, f.in_rate / f.out_rate, d_out, o_begin, o_end));
     } else {
-        const int st = sinc_narrow_index(d.L, d.M)
-                           ? launch_sinc<unsigned>(s, d, d_tab, d_out, o_begin, o_end, grid, stream)
-                           : launch_sinc<unsigned long long>(s, d, d_tab, d_out, o_begin, o_end, grid, stream);
-        if (st != FA_OK) return st;
+        return sinc_narrow_index(d.L, d.M) ? launch_sinc<unsigned>(s, d, d_tab, d_out, o_begin, o_end, grid, stream)
+                                           : launch_sinc<unsigned long long>(s, d, d_tab, d_out, o_begin, o_end, grid, stream);
     }
-    FA_CUDA_TRY(cudaGetLastError());
-    if (launches) ++*launches;
     return FA_OK;
 }
 

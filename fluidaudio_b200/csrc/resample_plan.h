@@ -81,7 +81,7 @@ int resolve_algorithm(const AudioFormat &f);
 // tab: device copy of Design::table (sinc only).  `frames_avail`: input frames already resident (<= frames): outputs
 // whose filter window reaches beyond it must not be requested yet (see outputs_ready).
 int launch_convert(const void *d_pcm, long long frames, const AudioFormat &f, const Design &d, const float *d_tab,
-                   float *d_out, long long o_begin, long long o_end, cudaStream_t stream, long long *launches);
+                   float *d_out, long long o_begin, long long o_end, cudaStream_t stream);
 // number of leading outputs computable when only the first `frames_avail` input frames are resident
 long long outputs_ready(const AudioFormat &f, const Design &d, long long frames, long long frames_avail,
                         long long out_total);

@@ -768,37 +768,6 @@ void Workspace::release() {
     pool_bytes = 0;
 }
 
-int Workspace::reserve(size_t bytes) { return grow_buffer(pool, pool_bytes, bytes); }
-
-size_t refine_bytes(int T, int D, int S, int max_it) {
-    Carver c{nullptr};
-    const int Tp = (T + 31) & ~31;
-    const int eblocks = (T + kEThreads - 1) / kEThreads;
-    c.take<double>((size_t)T * D);
-    c.take<double>((size_t)D * Tp);
-    c.take<double>(T);
-    c.take<double>(D);
-    c.take<double>((size_t)S * D);
-    c.take<double>((size_t)S * D);
-    c.take<double>(S);
-    c.take<double>(S);
-    c.take<double>(S);
-    c.take<double>((size_t)chunks_for(S) * S * D);
-    c.take<double>((size_t)chunks_for(S) * S);
-    c.take<double>(eblocks);
-    c.take<double>((size_t)eblocks * S);
-    c.take<double>(std::max(max_it, 1));
-    c.take<double>(8);
-    c.take<int>(8);
-    if (S <= kFusedMaxS) {
-        c.take<double>((size_t)eblocks * S * D);
-        c.take<double>((size_t)eblocks * S);
-        c.take<double>(eblocks);
-        for (int i = 0; i < 2; ++i) c.take<double>(3 * (size_t)S);
-    }
-    return c.off + 512;
-}
-
 static size_t fused_smem_bytes(int S, int D) {
     return sizeof(double) * ((size_t)S * D + 2 * (size_t)S + (size_t)kEThreads * S + kEThreads);
 }
@@ -808,12 +777,9 @@ static bool fused_path(int S, int D) { return S <= kFusedMaxS && fused_smem_byte
 // d_init: [T] device labels (or nullptr), d_gamma [T x S], d_pi [S], d_elbos [max(max_it,1)], d_hard [T].
 int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *h_psi, const int *d_init, int S,
                   const Config &cfg, double *d_gamma, double *d_pi, double *d_elbos, int *d_hard, int *iterations_host,
-                  cudaStream_t stream, long long *launches) {
+                  cudaStream_t stream) {
     if (T <= 0 || D <= 0 || S <= 0) return FA_INVALID_ARGUMENT;
     const int max_it = cfg.max_iterations;
-    int st = ws.reserve(refine_bytes(T, D, S, max_it));
-    if (st != FA_OK) return st;
-    Carver c{static_cast<char *>(ws.pool)};
     Dev d{};
     d.T = T;
     d.D = D;
@@ -822,29 +788,33 @@ int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *
     d.chunks = chunks_for(S);
     d.eblocks = (T + kEThreads - 1) / kEThreads;
     d.x = d_x;
-    d.rho = c.take<double>((size_t)T * D);
-    d.rhoT = c.take<double>((size_t)D * d.Tp);
-    d.G = c.take<double>(T);
-    double *phi_c = c.take<double>(D);
+    double *phi_c = nullptr;
+    int st = carve_arena(ws.pool, ws.pool_bytes, [&](Carver &c) {
+        d.rho = c.take<double>((size_t)T * D);
+        d.rhoT = c.take<double>((size_t)D * d.Tp);
+        d.G = c.take<double>(T);
+        phi_c = c.take<double>(D);
+        d.invL = c.take<double>((size_t)S * D);
+        d.alpha = c.take<double>((size_t)S * D);
+        d.phiTerm = c.take<double>(S);
+        d.logPi = c.take<double>(S);
+        d.gsum = c.take<double>(S);
+        d.pA = c.take<double>((size_t)d.chunks * S * D);
+        d.pG = c.take<double>((size_t)d.chunks * S);
+        d.pLL = c.take<double>(d.eblocks);
+        d.pPi = c.take<double>((size_t)d.eblocks * S);
+        (void)c.take<double>(std::max(max_it, 1));
+        d.scal = c.take<double>(8);
+        d.state = c.take<int>(8);
+        if (S <= kFusedMaxS) {
+            d.fA = c.take<double>((size_t)d.eblocks * S * D);
+            d.fG = c.take<double>((size_t)d.eblocks * S);
+            d.fLL = c.take<double>(d.eblocks);
+            for (int i = 0; i < 2; ++i) d.fsums[i] = c.take<double>(3 * (size_t)S);
+        }
+    }, 512);
+    if (st != FA_OK) return st;
     d.phi_c = phi_c;
-    d.invL = c.take<double>((size_t)S * D);
-    d.alpha = c.take<double>((size_t)S * D);
-    d.phiTerm = c.take<double>(S);
-    d.logPi = c.take<double>(S);
-    d.gsum = c.take<double>(S);
-    d.pA = c.take<double>((size_t)d.chunks * S * D);
-    d.pG = c.take<double>((size_t)d.chunks * S);
-    d.pLL = c.take<double>(d.eblocks);
-    d.pPi = c.take<double>((size_t)d.eblocks * S);
-    (void)c.take<double>(std::max(max_it, 1));
-    d.scal = c.take<double>(8);
-    d.state = c.take<int>(8);
-    if (S <= kFusedMaxS) {
-        d.fA = c.take<double>((size_t)d.eblocks * S * D);
-        d.fG = c.take<double>((size_t)d.eblocks * S);
-        d.fLL = c.take<double>(d.eblocks);
-        for (int i = 0; i < 2; ++i) d.fsums[i] = c.take<double>(3 * (size_t)S);
-    }
     d.gamma = d_gamma;
     d.pi = d_pi;
     d.elbos = d_elbos;
@@ -865,9 +835,7 @@ int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *
         FA_CUDA_TRY(cudaMemcpyAsync(phi_c, tmp.data(), D * sizeof(double), cudaMemcpyHostToDevice, stream));
         FA_CUDA_TRY(cudaStreamSynchronize(stream));   // tmp, h_pi and h_scal are pageable stack/heap buffers
     }
-    vbx_init_kernel<<<(T + 127) / 128, 128, 0, stream>>>(d, d_init, cfg.init_smoothing);
-    FA_CUDA_TRY(cudaGetLastError());
-    long long n_launch = 1;
+    FA_CUDA_TRY(fa::launch(vbx_init_kernel, (T + 127) / 128, 128, 0, stream, d, d_init, cfg.init_smoothing));
     if (fused_path(S, D)) {
         static std::once_flag once_f;
         static cudaError_t attr_err_f = cudaSuccess;
@@ -880,53 +848,32 @@ int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *
         const size_t tile_bytes = sizeof(double) * (size_t)D * (kEThreads + 1);
         const bool use_tile = fused_smem_bytes(S, D) + tile_bytes <= 200 * 1024;
         const size_t fsmem = fused_smem_bytes(S, D) + (use_tile ? tile_bytes : 0);
-        vbx_partials0_kernel<<<d.eblocks, kEThreads, sizeof(double) * (size_t)kEThreads * S, stream>>>(d);
-        ++n_launch;
+        FA_CUDA_TRY(fa::launch(vbx_partials0_kernel, d.eblocks, kEThreads, sizeof(double) * (size_t)kEThreads * S, stream, d));
         for (int it = 0; it < max_it; ++it) {
-            vbx_update_kernel2<<<S, kEThreads, 0, stream>>>(d, it, 0);
-            vbx_estep_kernel2<<<d.eblocks, kEThreads, fsmem, stream>>>(d, use_tile ? 1 : 0);
-            n_launch += 2;
+            FA_CUDA_TRY(fa::launch(vbx_update_kernel2, S, kEThreads, 0, stream, d, it, 0));
+            FA_CUDA_TRY(fa::launch(vbx_estep_kernel2, d.eblocks, kEThreads, fsmem, stream, d, use_tile ? 1 : 0));
         }
-        if (max_it > 0) {
-            vbx_update_kernel2<<<S, kEThreads, 0, stream>>>(d, max_it, 1);   // books of the last E-step (no-op if converged)
-            ++n_launch;
-        }
-        vbx_hard_kernel<<<(T + 127) / 128, 128, 0, stream>>>(d_gamma, T, S, d_hard);
-        FA_CUDA_TRY(cudaGetLastError());
-        ++n_launch;
-        if (launches) *launches += n_launch;
-        if (iterations_host) {
-            int h_state[2] = {0, 0};
-            FA_CUDA_TRY(cudaMemcpyAsync(h_state, d.state, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-            FA_CUDA_TRY(cudaStreamSynchronize(stream));
-            *iterations_host = h_state[1];
-        }
-        return FA_OK;
-    }
-    const size_t esmem_full = sizeof(double) * ((size_t)S * D + 2 * S + kEThreads);
-    const bool alpha_smem = esmem_full <= 200 * 1024;
-    const size_t esmem = alpha_smem ? esmem_full : sizeof(double) * kEThreads;
-    {
+        if (max_it > 0)   // books of the last E-step (no-op if converged)
+            FA_CUDA_TRY(fa::launch(vbx_update_kernel2, S, kEThreads, 0, stream, d, max_it, 1));
+    } else {
+        const size_t esmem_full = sizeof(double) * ((size_t)S * D + 2 * S + kEThreads);
+        const bool alpha_smem = esmem_full <= 200 * 1024;
+        const size_t esmem = alpha_smem ? esmem_full : sizeof(double) * kEThreads;
         static std::once_flag once;   // per-function attribute shared by concurrent callers: set once to the maximum
         static cudaError_t attr_err = cudaSuccess;
         std::call_once(once, [&]() {
             attr_err = cudaFuncSetAttribute(vbx_estep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         });
         FA_CUDA_TRY(attr_err);
+        for (int it = 0; it < max_it; ++it) {
+            FA_CUDA_TRY(fa::launch(vbx_accumulate_kernel, d.chunks, 256, 0, stream, d));
+            FA_CUDA_TRY(fa::launch(vbx_update_kernel, 1, 256, 0, stream, d));
+            FA_CUDA_TRY(fa::launch(alpha_smem ? vbx_estep_kernel<true> : vbx_estep_kernel<false>, d.eblocks, kEThreads, esmem,
+                                   stream, d));
+            FA_CUDA_TRY(fa::launch(vbx_finish_kernel, 1, 256, 0, stream, d, it));
+        }
     }
-    for (int it = 0; it < max_it; ++it) {
-        vbx_accumulate_kernel<<<d.chunks, 256, 0, stream>>>(d);
-        vbx_update_kernel<<<1, 256, 0, stream>>>(d);
-        if (alpha_smem) vbx_estep_kernel<true><<<d.eblocks, kEThreads, esmem, stream>>>(d);
-        else vbx_estep_kernel<false><<<d.eblocks, kEThreads, esmem, stream>>>(d);
-        vbx_finish_kernel<<<1, 256, 0, stream>>>(d, it);
-        n_launch += 4;
-    }
-    FA_CUDA_TRY(cudaGetLastError());
-    vbx_hard_kernel<<<(T + 127) / 128, 128, 0, stream>>>(d_gamma, T, S, d_hard);
-    FA_CUDA_TRY(cudaGetLastError());
-    ++n_launch;
-    if (launches) *launches += n_launch;
+    FA_CUDA_TRY(fa::launch(vbx_hard_kernel, (T + 127) / 128, 128, 0, stream, d_gamma, T, S, d_hard));
     if (iterations_host) {
         int h_state[2] = {0, 0};
         FA_CUDA_TRY(cudaMemcpyAsync(h_state, d.state, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
@@ -936,20 +883,17 @@ int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *
     return FA_OK;
 }
 
-size_t centroid_bytes(int T, int E, int S) {
-    const size_t parts = S <= kFusedMaxS ? (size_t)((T + kCBlock - 1) / kCBlock) : (size_t)chunks_for(S);
-    return (parts * S * E + parts * S) * sizeof(double) + (size_t)S * sizeof(int) + 2048;
-}
-
 int centroids_device(Workspace &ws, const double *d_emb, int T, int E, const double *d_gamma, const double *d_pi, int S,
-                     double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream, long long *launches) {
+                     double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream) {
     const int chunks = S <= kFusedMaxS ? (T + kCBlock - 1) / kCBlock : chunks_for(S);
-    int st = ws.reserve(centroid_bytes(T, E, S));
+    double *pnum = nullptr, *pden = nullptr;
+    int *map = nullptr;
+    int st = carve_arena(ws.pool, ws.pool_bytes, [&](Carver &c) {
+        pnum = c.take<double>((size_t)chunks * S * E);
+        pden = c.take<double>((size_t)chunks * S);
+        map = c.take<int>(S);
+    }, 2048);
     if (st != FA_OK) return st;
-    Carver c{static_cast<char *>(ws.pool)};
-    double *pnum = c.take<double>((size_t)chunks * S * E);
-    double *pden = c.take<double>((size_t)chunks * S);
-    int *map = c.take<int>(S);
     if (S <= kFusedMaxS) {
         static std::once_flag once_c;
         static cudaError_t attr_err_c = cudaSuccess;
@@ -959,54 +903,46 @@ int centroids_device(Workspace &ws, const double *d_emb, int T, int E, const dou
         });
         FA_CUDA_TRY(attr_err_c);
         const unsigned tiles = (unsigned)((S * E + 255) / 256);
-        centroid_acc16_kernel<<<chunks, 256, sizeof(double) * (size_t)kCBlock * S, stream>>>(d_emb, d_gamma, T, E, S, pnum, pden);
-        centroid_fold_kernel<<<tiles, 256, 0, stream>>>(pnum, pden, d_pi, E, S, chunks, d_cent);
-        centroid_norm_kernel<<<1, 64, 0, stream>>>(d_pi, E, S, d_cent, d_cent_n, d_count);
-        FA_CUDA_TRY(cudaGetLastError());
-        if (launches) *launches += 3;
+        FA_CUDA_TRY(fa::launch(centroid_acc16_kernel, chunks, 256, sizeof(double) * (size_t)kCBlock * S, stream, d_emb, d_gamma,
+                               T, E, S, pnum, pden));
+        FA_CUDA_TRY(fa::launch(centroid_fold_kernel, tiles, 256, 0, stream, pnum, pden, d_pi, E, S, chunks, d_cent));
+        FA_CUDA_TRY(fa::launch(centroid_norm_kernel, 1, 64, 0, stream, d_pi, E, S, d_cent, d_cent_n, d_count));
         return FA_OK;
     }
-    centroid_accumulate_kernel<<<chunks, 256, 0, stream>>>(d_emb, d_gamma, T, E, S, chunks, pnum, pden);
-    centroid_finish_kernel<<<1, 256, 0, stream>>>(pnum, pden, d_pi, E, S, chunks, map, d_cent, d_cent_n, d_count);
-    FA_CUDA_TRY(cudaGetLastError());
-    if (launches) *launches += 2;
+    FA_CUDA_TRY(fa::launch(centroid_accumulate_kernel, chunks, 256, 0, stream, d_emb, d_gamma, T, E, S, chunks, pnum, pden));
+    FA_CUDA_TRY(fa::launch(centroid_finish_kernel, 1, 256, 0, stream, pnum, pden, d_pi, E, S, chunks, map, d_cent, d_cent_n,
+                           d_count));
     return FA_OK;
 }
 
 int assign_device(const double *d_emb, int N, int E, const double *d_cent_n, const int *d_count, int K_fixed,
-                  int *d_labels, double *d_scores, cudaStream_t stream, long long *launches) {
+                  int *d_labels, double *d_scores, cudaStream_t stream) {
     if (N <= 0) return FA_OK;
-    assign_tiled_kernel<<<(N + kARows - 1) / kARows, kARows, 0, stream>>>(d_emb, N, E, d_cent_n, d_count, K_fixed, d_labels,
-                                                                          d_scores);
-    FA_CUDA_TRY(cudaGetLastError());
-    if (launches) *launches += 1;
+    FA_CUDA_TRY(fa::launch(assign_tiled_kernel, (N + kARows - 1) / kARows, kARows, 0, stream, d_emb, N, E, d_cent_n, d_count,
+                           K_fixed, d_labels, d_scores));
     return FA_OK;
 }
 
 int onehot_device(const int *d_labels, int T, int S, double *d_gamma, double *d_pi, cudaStream_t stream) {
     const int n = std::max(T, S);
-    onehot_kernel<<<(n + 127) / 128, 128, 0, stream>>>(d_labels, T, S, d_gamma, d_pi);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(onehot_kernel, (n + 127) / 128, 128, 0, stream, d_labels, T, S, d_gamma, d_pi));
     return FA_OK;
 }
 
 int finite_rows_device(const float *d_emb, int N, int E, unsigned char *d_ok, cudaStream_t stream) {
-    finite_rows_kernel<<<(N + 127) / 128, 128, 0, stream>>>(d_emb, N, E, d_ok);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(finite_rows_kernel, (N + 127) / 128, 128, 0, stream, d_emb, N, E, d_ok));
     return FA_OK;
 }
 
 int gather_rows_device(const double *d_src, const int *d_idx, int rows, int dim, double *d_dst, cudaStream_t stream) {
     const long long total = (long long)rows * dim;
     if (total <= 0) return FA_OK;
-    gather_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_src, d_idx, rows, dim, d_dst);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(gather_rows_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, d_src, d_idx, rows, dim, d_dst));
     return FA_OK;
 }
 
 int mean_rows_device(const double *d_src, int rows, int dim, double *d_out, cudaStream_t stream) {
-    mean_rows_kernel<<<(dim + 127) / 128, 128, 0, stream>>>(d_src, rows, dim, d_out);
-    FA_CUDA_TRY(cudaGetLastError());
+    FA_CUDA_TRY(fa::launch(mean_rows_kernel, (dim + 127) / 128, 128, 0, stream, d_src, rows, dim, d_out));
     return FA_OK;
 }
 

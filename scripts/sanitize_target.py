@@ -56,7 +56,19 @@ rng = np.random.default_rng(0)
 emb, _ = synth.speaker_embeddings(320, 256, 4, seed=5)
 rho, psi = synth.synthetic_plda(emb)
 init = np.concatenate([np.arange(260), rng.integers(0, 260, 60)]).astype(np.int32)
-cl.VBxClustering(psi=psi).refine(rho, init)
+vbx = cl.VBxClustering(psi=psi).refine(rho, init)
+# the standalone clustering entry points, each on its own scratch arena: normalisation, AHC, K-Means (identity and
+# n_init runs), centroids on both sides of the fused-path limit (64 speakers), assignment with and without scores
+x = emb.astype(np.float64)
+cl.l2_normalize_rows(x)
+cl.AHCClustering().cluster(x[:120], 0.6)
+cl.KMeansClustering.cluster_with_centroids_n_init(x, 6, max_iterations=20, n_init=3)
+cl.KMeansClustering.cluster_with_centroids_n_init(x[:5], 6)
+cents = cl.compute_centroids(x, vbx)
+small = cl.VBxClustering(psi=psi).refine(rho, init % 8)
+cl.compute_centroids(x, small)
+cl.assign_embeddings(x, cents)
+cl.assign_embeddings(x, cents[:7], want_scores=True)
 emb, _ = synth.speaker_embeddings(900, 256, 4, seed=6)
 rho, psi = synth.synthetic_plda(emb)
 cl.OfflineClusterer(psi=psi).cluster_batch(emb, rho, np.array([0, 300, 600, 900], np.int64))
