@@ -505,8 +505,6 @@ __global__ void ahc_filter_finish_kernel(int N, FilterBufs F, double *key, int *
 }
 
 // ------------------------------------------------------------------------------------------------ merge loop
-constexpr int kMergeThreads = 128;
-constexpr int kMaxRounds = 16;    // streamed mode only: slots per thread
 enum { CMD_MERGE = 1, CMD_RESCAN = 2, CMD_EXIT = 3 };
 typedef unsigned long long u64;
 
@@ -1149,45 +1147,8 @@ int Solver::init(cudaStream_t s, int worker_limit) {
     return FA_OK;
 }
 
-namespace {
-// bytes of master state staged in shared memory at each level (must mirror ahc_master's carving)
-size_t master_smem_bytes(int N, int level) {
-    auto up = [](size_t b) { return (b + 15) & ~size_t(15); };
-    const size_t words = (size_t)(2 * N - 1 + 31) >> 5;
-    size_t b = up(sizeof(double) * N) + 2 * up(sizeof(uint16_t) * N) + up(sizeof(unsigned) * words);
-    if (level >= 2) b += up(sizeof(int) * N);
-    if (level >= 3) b += up(sizeof(int) * N);
-    return b;
-}
-
-// Dynamic shared memory the merge kernel may use: leaves room for its static shared memory.
-constexpr size_t kMergeSmemCap = 227 * 1024 - 2048;
-
-// Shared memory of one worker CTA before any resident node vector: the target vector and the reduction scratch.
-size_t worker_fixed_smem(int D) {
-    return 3 * sizeof(double) * (size_t)((D + 1) & ~1) + 2 * sizeof(double) * (kMergeThreads / 32) + 64;
-}
-
-// Node vectors one worker CTA can keep in shared memory (at most one per thread), 0 if not even one fits.
-int resident_slot_capacity(int D) {
-    const size_t fixed = worker_fixed_smem(D);
-    if (fixed + sizeof(double) * D > kMergeSmemCap) return 0;
-    return (int)std::min<size_t>(kMergeThreads, (kMergeSmemCap - fixed) / (sizeof(double) * (size_t)D));
-}
-} // namespace
-
-// Worker CTAs a problem needs to keep every node vector in shared memory (the fast placement), or 0 if a single CTA
-// cannot hold even one vector.
-int resident_workers_needed(int N, int D) {
-    const int cap_slots = resident_slot_capacity(D);
-    return cap_slots ? (N + cap_slots - 1) / cap_slots : 0;
-}
-
-// FA_AHC_* environment hooks (tests only: fall-back placements and the float32 filter at small N), read once.
-struct Hooks {
-    bool force_global = false, force_stream = false;
-    int filter_min_n = 2048;   // FA_AHC_FILTER_MIN_N: problems at least this large take the float32 filter (0 = never)
-};
+// FA_AHC_* environment hooks (tests only: fall-back placements and the float32 filter at small N), read ONCE per
+// process: stray variables cannot change behaviour mid-run.
 static const Hooks &hooks() {
     static const Hooks h = [] {
         Hooks x;
@@ -1203,49 +1164,23 @@ static const Hooks &hooks() {
 int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     if (N < 2) return FA_OK;
     const int Ns = (N + 31) & ~31;
-    // master placement: slot-indexed heap (+ nn, + node_of) in shared memory when it fits
-    int level = 0;
-    if (N <= 65535)
-        for (int l = 1; l <= 3; ++l)
-            if (master_smem_bytes(N, l) <= kMergeSmemCap) level = l;
-    // test hooks: exercise the fall-back placements at small N (tests/test_gpu_parity.py)
-    // (all FA_AHC_* hooks are read ONCE per process, see hooks(): stray variables cannot change behaviour mid-run)
-    const Hooks &hk = hooks();
-    const bool force_global = hk.force_global, force_stream = hk.force_stream;
-    if (force_global) level = 0;
-    const bool idx16 = level >= 1;
-    // worker placement: resident (each CTA keeps <= 128 node vectors in shared memory) when the whole problem fits
-    // into max_workers CTAs, else streamed from the k-major global copy
-    const int cap_slots = resident_slot_capacity(D);
-    if (cap_slots == 0) {
-        fa::set_error("dimension %d too large for the merge kernel's shared-memory target vector", D);
-        return FA_RUNTIME_ERROR;
+    const Placement pl = plan_linkage(N, D, max_workers, hooks());
+    if (pl.status != FA_OK) {
+        if (pl.cap_slots == 0)
+            fa::set_error("dimension %d too large for the merge kernel's shared-memory target vector", D);
+        else
+            fa::set_error("point count %d exceeds the capacity of the merge kernel (%lld)", N, pl.capacity);
+        return pl.status;
     }
-    bool resident = (long long)cap_slots * max_workers >= N;
-    if (force_stream) resident = false;
-    int workers, slots_per_cta = 0;
-    size_t worker_smem = worker_fixed_smem(D);
-    if (resident) {
-        // enough CTAs to hold every node, but no more than needed: the per-step barrier cost grows with CTA count
-        workers = std::min(max_workers, std::max(1, (N + cap_slots - 1) / cap_slots));
-        slots_per_cta = (N + workers - 1) / workers;
-        worker_smem += sizeof(double) * (size_t)D * slots_per_cta;
-    } else {
-        workers = std::max(1, std::min(max_workers, (Ns + kMergeThreads - 1) / kMergeThreads));
-        if ((long long)workers * kMergeThreads * kMaxRounds < Ns) {
-            fa::set_error("point count %d exceeds the capacity of the merge kernel (%lld)", N,
-                          (long long)workers * kMergeThreads * kMaxRounds);
-            return FA_RUNTIME_ERROR;
-        }
-    }
-    const size_t smem = std::max(worker_smem, level ? master_smem_bytes(N, level) : (size_t)0);
+    const int level = pl.level, workers = pl.workers;
+    const bool idx16 = pl.idx16, keep_tmin = pl.keep_tmin;
+    const size_t smem = pl.smem;
 
     // device arena: problem state, then the float32 filter of the initial nearest-neighbour pass (N >= filter_min_n
     // only, but sized unconditionally: small)
     const int ranges = (N + kJR - 1) / kJR;
     const int filter_cap = (int)std::min<long long>(64LL * N, 1 << 24);
     const long long nt = (N + 63) / 64;
-    const bool keep_tmin = (long long)N * nt <= (16LL << 20);   // <= 64 MB
     Problem P{};
     FilterBufs F{};
     Cand *init_partial = nullptr;
@@ -1300,8 +1235,8 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     P.D = D;
     P.Ns = Ns;
     P.result_stride = (max_workers + 1) << kSlotShift;
-    P.resident = resident ? 1 : 0;
-    P.slots_per_cta = slots_per_cta;
+    P.resident = pl.resident ? 1 : 0;
+    P.slots_per_cta = pl.slots_per_cta;
     P.idx16 = idx16 ? 1 : 0;
     P.smem_level = level;
 
@@ -1330,9 +1265,8 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
                                P.node_weight));
         return FA_OK;
     };
-    const bool use_filter = hk.filter_min_n > 0 && N >= hk.filter_min_n;
     int *h_fc = h_err + 1;   // [3] filter counters (pinned)
-    if (use_filter) {
+    if (pl.filter) {
         F.cap = filter_cap;
         F.nt = (N + kFT - 1) / kFT;
         F.c1 = 2.02 * (double)(D + 3) * 5.9604644775390625e-08;   // 2^-24
@@ -1341,7 +1275,7 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
         FA_CUDA_TRY(fa::launch(ahc_filter_prep_kernel, (Ns + 127) / 128, 128, 0, stream, P.cols, N, D, Ns, F));
         const int nt2 = (N + kGT - 1) / kGT;
         FA_CUDA_TRY(fa::launch(ahc_filter_tile128_kernel, (unsigned)((long long)nt2 * (nt2 + 1) / 2), 256, 0, stream, N, D, Ns, F));
-        if (F.tmin && (size_t)8 * D * sizeof(float) <= 48 * 1024) {
+        if (pl.filter_rows) {
             FA_CUDA_TRY(fa::launch(ahc_filter_rows_kernel, (N + 7) / 8, 256, (size_t)8 * D * sizeof(float), stream, N, D, Ns, F));
         } else {
             const unsigned tiles = (unsigned)((long long)F.nt * (F.nt + 1) / 2);

@@ -2,6 +2,7 @@
 #pragma once
 
 #include "ahc_core.cuh"
+#include "ahc_placement.h"
 #include <cuda_runtime.h>
 #include <vector>
 
@@ -83,7 +84,6 @@ const float *last_stage_ms();
 
 // Standalone kernels used by the clustering pipeline
 int launch_normalize_rows(const double *d_in, double *d_out, int rows, int dim, cudaStream_t s);
-int resident_workers_needed(int N, int D);   // worker CTAs for the shared-memory-resident placement (0: impossible)
 int launch_normalize_rows_keep(const double *d_in, double *d_out, int rows, int dim, cudaStream_t s);   // zero rows kept
 int launch_widen_rows(const float *d_in, double *d_out, long long count, cudaStream_t s);
 

@@ -1352,16 +1352,11 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
     FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    // Concurrency: as many sets at a time as still leaves each of them enough SMs to keep its node vectors in shared
-    // memory (the merge loop is ~3x slower when they are streamed from L2): 5 000 x 256 needs 46 workers + 1 master,
-    // so two sets run side by side on an H100's 132 SMs; small sets run four at a time.
+    // Concurrency: see ahc::plan_batch_lanes
     long long n_max = 0;
     for (int m = 0; m < set_count; ++m) n_max = std::max<long long>(n_max, set_offsets[m + 1] - set_offsets[m]);
-    int lanes = std::max(1, std::min(set_count, 4));
-    const int need = ahc::resident_workers_needed((int)std::min<long long>(n_max, INT32_MAX), (int)emb_dim);
-    if (need > 0 && need + 1 <= prop.multiProcessorCount)
-        lanes = std::max(1, std::min(lanes, prop.multiProcessorCount / (need + 1)));
-    const int worker_limit = lanes == 1 ? 0 : std::max(1, prop.multiProcessorCount / lanes - 1);
+    const ahc::BatchLanes plan = ahc::plan_batch_lanes(set_count, n_max, (int)emb_dim, prop.multiProcessorCount);
+    const int lanes = plan.lanes, worker_limit = plan.worker_limit;
     std::atomic<int> next{0};
     std::vector<int> status(lanes, FA_OK);
     std::vector<std::string> messages(lanes);

@@ -77,4 +77,8 @@ m.compute_batch([a[:30000], a[:1000], a[:48077]])
 # the float32 filter of the AHC nearest-neighbour pass is on from N = 2048 (FA_AHC_FILTER_MIN_N lowers it for this run)
 emb, _ = synth.speaker_embeddings(700, 64, 3, seed=8)
 cl.centroid_linkage(emb.astype(np.float64))
+# merge kernel placements (ahc_placement.h): master heap + nn in shared memory (level 2), and node vectors streamed in two
+# rounds per scan thread with the heap alone in shared memory (level 1; two rounds on 131 worker CTAs)
+cl.centroid_linkage(rng.standard_normal((12000, 4)))
+cl.centroid_linkage(rng.standard_normal((16769, 4)))
 print("sanitize target done")

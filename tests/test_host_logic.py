@@ -379,6 +379,111 @@ def test_merge_control_plane_matches_reference_goldens(tmp_path, golden_dir, ora
     assert L.ahc_emul(bad.ctypes.data_as(C.c_void_p), 10, 3, np.zeros((9, 4)).ctypes.data_as(C.c_void_p)) == 5
 
 
+PLACEMENT_FIELDS = ("status", "level", "idx16", "cap_slots", "resident", "workers", "slots_per_cta", "rounds", "capacity",
+                    "smem", "filter", "keep_tmin", "filter_rows")
+
+
+@pytest.fixture(scope="module")
+def placement_lib(tmp_path_factory):
+    """ahc_placement.h compiled on the host, and the GPU sweep's restatement of it"""
+    import importlib.util
+    L = _compile("ahc_placement_emul.cpp", str(tmp_path_factory.mktemp("placement") / "libahc_placement.so"))
+    spec = importlib.util.spec_from_file_location("ahc_sweep", os.path.join(ROOT, "tests", "test_gpu_ahc_sweep.py"))
+    sweep = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(sweep)
+
+    def plan(N, D, W, force_global=False, force_stream=False, filter_min_n=2048):
+        out = (C.c_longlong * 13)()
+        L.ahc_placement(N, D, W, int(force_global), int(force_stream), filter_min_n, out)
+        return dict(zip(PLACEMENT_FIELDS, out))
+
+    def lanes(set_count, n_max, D, sms):
+        out = (C.c_int * 2)()
+        L.ahc_batch_lanes(set_count, C.c_longlong(n_max), D, sms, out)
+        return tuple(out)
+
+    return plan, lanes, sweep
+
+
+def test_merge_kernel_placement_boundaries(placement_lib):
+    """plan_linkage at every boundary of the placement table (DESIGN.md section 4.2), for a 132-SM H100 SXM (131
+    worker CTAs) and a 114-SM H100 PCIe (113)."""
+    plan, _, sweep = placement_lib
+    for W in (131, 113):
+        # master state in shared memory: level 3 (heap + nn + node_of), 2 (heap + nn), 1 (heap), 0 (global)
+        for N, level in ((11376, 3), (11377, 2), (14176, 2), (14177, 1), (18808, 1), (18809, 0), (65535, 0)):
+            p = plan(N, 4, W)
+            assert (p["level"], p["idx16"]) == (level, int(level > 0)), (W, N, p)
+        assert plan(1500, 4, W, force_global=True)["level"] == 0
+        # node vectors per worker CTA, and the resident -> streamed flip at cap(D) * W
+        for D, cap in ((1, 128), (219, 128), (220, 127), (256, 109), (512, 53), (1024, 25), (1536, 15), (2048, 11),
+                       (4096, 4), (7196, 1), (7197, 0)):
+            assert plan(4, D, W)["cap_slots"] == cap, (D, cap)
+            if cap:
+                assert plan(cap * W, D, W)["resident"] == 1 and plan(cap * W + 1, D, W)["resident"] == 0, (W, D)
+                assert plan(cap * W, D, W, force_stream=True)["resident"] == 0
+            else:
+                assert plan(4, D, W)["status"] == 5                         # D >= 7 197: FA_RUNTIME_ERROR
+        assert plan(min(16768, 128 * W), 4, W)["smem"] <= 227 * 1024 - 2048
+        # streamed rounds: 2 from 128 W + 1, 16 at the capacity W * 2 048, refused one point past it
+        assert plan(128 * W + 1, 4, W)["rounds"] == 2
+        assert plan(256 * W + 1, 4, W)["rounds"] == 3
+        top = plan(W * 2048, 1, W)
+        assert (top["status"], top["rounds"], top["workers"], top["capacity"]) == (0, 16, W, W * 2048)
+        assert plan(W * 2048 + 1, 1, W)["status"] == 5 and plan(W * 2048 + 1, 4096, W)["status"] == 5
+        # float32 filter from N = 2 048; its pass 2 is the rows kernel while the bounds are kept and D <= 1 536
+        assert plan(2047, 16, W)["filter"] == 0 and plan(2048, 16, W)["filter"] == 1
+        assert plan(2048, 16, W, filter_min_n=0)["filter"] == 0 and plan(3, 16, W, filter_min_n=2)["filter"] == 1
+        assert plan(32768, 4, W)["keep_tmin"] == 1 and plan(32769, 4, W)["keep_tmin"] == 0
+        assert plan(32768, 4, W)["filter_rows"] == 1 and plan(32769, 4, W)["filter_rows"] == 0
+        assert plan(2048, 1536, W)["filter_rows"] == 1 and plan(2048, 1537, W)["filter_rows"] == 0
+    # the sweep's formulas for a 132-SM device are these numbers
+    assert sweep.level_limits() == [11376, 14176, 18808] and sweep.d_limit() == 7196
+
+
+def test_merge_kernel_placement_restatement_is_exact(placement_lib):
+    """The GPU sweep computes its shapes from a Python restatement of ahc_placement.h: it must agree field for field."""
+    plan, lanes, sweep = placement_lib
+    rng = np.random.default_rng(3)
+    Ns = {2, 3, 31, 32, 33, 2047, 2048, 11376, 11377, 14176, 14177, 14279, 14280, 16637, 16638, 16768, 16769, 18808,
+          18809, 32768, 32769, 33537, 65535, 65536, 65537, 231424, 231425, 268288, 268289, 300000}
+    Ns |= set(rng.integers(2, 300000, 40).tolist())
+    Ds = {1, 2, 3, 7, 8, 9, 15, 16, 17, 31, 33, 219, 220, 256, 1023, 1024, 1536, 1537, 2048, 4096, 7196, 7197, 9000}
+    for W in (1, 2, 32, 43, 65, 113, 131):
+        for N in sorted(Ns):
+            for D in sorted(Ds):
+                for hooks in ({}, {"force_global": True, "force_stream": True}, {"filter_min_n": 0}):
+                    want = plan(N, D, W, **hooks)
+                    assert sweep.placement(N, D, W, **hooks) == want, (N, D, W, hooks, want)
+    for sms in (8, 66, 114, 132):
+        for count in (1, 2, 3, 4, 7):
+            for n_max in sorted(Ns):
+                for D in (4, 256, 2048, 7197):
+                    assert sweep.batch_lanes(count, n_max, D, sms) == lanes(count, n_max, D, sms), (sms, count, n_max, D)
+
+
+def test_batch_lanes_keep_every_set_within_its_lane(placement_lib):
+    """fa_diarize_cluster_batch runs sets side by side in lanes of SMs / lanes - 1 worker CTAs.  Whatever lane count
+    the rule picks, a set the single call accepts must fit its lane's streamed capacity; otherwise the lane's linkage
+    fails and the pipeline turns that set into identity labels (a 65 537-row set among four on 132 SMs: 32 workers hold
+    65 536 slots)."""
+    plan, lanes, _ = placement_lib
+    for sms in (132, 114, 66, 8):
+        W = sms - 1
+        sizes = {2, 300, 5000, 14279, 14280, 16768, 16769, 65536, 65537, 88064, 88065, 133120, 133121, W * 2048 - 31,
+                 W * 2048, W * 2048 + 1}
+        for D in (1, 4, 220, 256, 1024, 2048, 7196, 7197):
+            for n_max in sorted(sizes):
+                single = plan(n_max, D, W)["status"]
+                for count in range(1, 7):
+                    n_lanes, limit = lanes(count, n_max, D, sms)
+                    assert 1 <= n_lanes <= min(count, 4) and (limit == 0) == (n_lanes == 1)
+                    lane = plan(n_max, D, min(W, limit) if limit else W)
+                    assert lane["status"] == single, (sms, D, n_max, count, n_lanes, limit)
+    assert lanes(4, 65537, 4, 132) == (3, 43) and lanes(4, 20000, 4, 132) == (4, 32) and lanes(4, 5000, 256, 132)[0] == 2
+    assert lanes(4, 132 * 2048, 4, 132) == (1, 0)
+
+
 # ------------------------------------------------------------------------------------------------ sharding
 def test_float32_filter_bound_is_rigorous():
     """The AHC initial pass trusts E_ij = c1 r_i r_j + c2 (n_i + n_j), c1 = 2.02 (D + 3) 2^-24, c2 = 2e-12
