@@ -1117,18 +1117,6 @@ int launch_widen_rows(const float *d_in, double *d_out, long long count, cudaStr
 thread_local float g_last_ms[4] = {0, 0, 0, 0};
 const float *last_stage_ms() { return g_last_ms; }
 
-Solver::~Solver() { release(); }
-
-void Solver::release() {
-    if (d_pool) cudaFree(d_pool);
-    if (d_input) cudaFree(d_input);
-    if (h_pool) cudaFreeHost(h_pool);
-    d_pool = nullptr;
-    d_input = nullptr;
-    h_pool = nullptr;
-    pool_bytes = h_pool_bytes = input_bytes = 0;
-}
-
 int Solver::init(cudaStream_t s, int worker_limit) {
     stream = s;
     int dev = 0;
@@ -1185,7 +1173,7 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     FilterBufs F{};
     Cand *init_partial = nullptr;
     Problem *d_prob = nullptr;
-    int st = carve_arena(d_pool, pool_bytes, [&](Carver &c) {
+    int st = carve_arena(d_pool, [&](Carver &c) {
         P.rows = c.take<double>((size_t)(2 * N - 1) * D);
         P.cols = c.take<double>((size_t)D * Ns);
         P.node_weight = c.take<int>((size_t)2 * N);
@@ -1221,7 +1209,7 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     // pinned host mirrors
     double *h_key = nullptr, *h_md = nullptr;
     int *h_at = nullptr, *h_where = nullptr, *h_ma = nullptr, *h_mb = nullptr, *h_err = nullptr;
-    st = carve_arena(h_pool, h_pool_bytes, [&](Carver &c) {
+    st = carve_arena(h_pool, [&](Carver &c) {
         h_key = c.take<double>((size_t)N + 4);
         h_md = c.take<double>((size_t)N + 4);
         h_at = c.take<int>((size_t)N + 2);   // reused as uint16 when idx16
@@ -1229,7 +1217,7 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
         h_ma = c.take<int>((size_t)N);
         h_mb = c.take<int>((size_t)N);
         h_err = c.take<int>(4);          // error flag, then the filter's three counters
-    }, 0, true);
+    });
     if (st != FA_OK) return st;
     P.N = N;
     P.D = D;
@@ -1240,16 +1228,11 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     P.idx16 = idx16 ? 1 : 0;
     P.smem_level = level;
 
-    // timing events live in a guard: every early return below (FA_CUDA_TRY) releases them
-    struct Events {
-        cudaEvent_t e[4] = {nullptr, nullptr, nullptr, nullptr};
-        ~Events() {
-            for (auto x : e)
-                if (x) cudaEventDestroy(x);
-        }
-        cudaEvent_t &operator[](int i) { return e[i]; }
-    } ev;
-    for (int i = 0; i < 4; ++i) FA_CUDA_TRY(cudaEventCreate(&ev.e[i]));
+    Event ev[4];   // stage timing
+    for (auto &e : ev) {
+        st = e.create();
+        if (st != FA_OK) return st;
+    }
 
     FA_CUDA_TRY(cudaMemsetAsync(P.cmd, 0, 256, stream));
     FA_CUDA_TRY(cudaMemsetAsync(P.threshold, 0, 256, stream));
@@ -1367,10 +1350,10 @@ int Solver::linkage_host(const double *rows_host, size_t N, size_t D, double *Z,
     if (z_len < (N > 1 ? (N - 1) * 4 : 0)) return FA_OUTPUT_TOO_SMALL;
     if (N == 1) return FA_OK;
     const size_t count = N * D;
-    const int st = grow_buffer(d_input, input_bytes, count * sizeof(double));
+    const int st = d_input.grow(count * sizeof(double));
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_input, rows_host, count * sizeof(double), cudaMemcpyHostToDevice, stream));
-    return linkage_device(d_input, (int)N, (int)D, Z);
+    FA_CUDA_TRY(cudaMemcpyAsync(d_input.data(), rows_host, count * sizeof(double), cudaMemcpyHostToDevice, stream));
+    return linkage_device(d_input.data(), (int)N, (int)D, Z);
 }
 
 // Swift-side cut (AHCClustering.swift:112-121 clamp, :124-197 traversal, :200-210 relabel)

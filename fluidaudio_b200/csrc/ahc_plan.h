@@ -61,16 +61,10 @@ struct Solver {
     int max_workers = 0;      // worker CTAs available for one problem (grid = workers + 1)
     cudaStream_t stream = nullptr;
     // device storage (grown on demand, reused across calls)
-    void *d_pool = nullptr;
-    size_t pool_bytes = 0;
-    double *d_input = nullptr;   // staging of the caller's [N x D] rows when they come from the host
-    size_t input_bytes = 0;
-    // pinned host mirrors
-    void *h_pool = nullptr;
-    size_t h_pool_bytes = 0;
+    DeviceBuffer<> d_pool;
+    DeviceBuffer<double> d_input;   // staging of the caller's [N x D] rows when they come from the host
+    PinnedBuffer<> h_pool;          // pinned host mirrors
 
-    ~Solver();
-    void release();
     int init(cudaStream_t s, int worker_limit);
     // rows: device pointer to N x D row-major doubles (already normalised by the caller, as the reference requires).
     // Z: host buffer of (N-1) x 4 doubles.  Status codes follow FastClusterWrapper.h.

@@ -71,34 +71,28 @@ static int require_device() {
 // synchronous, stateless and re-entrant: FastClusterWrapper.cpp keeps no state, SURVEY §8b) -------------
 struct ClusterContext {
     int device = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;   // declared first, so destroyed last: after every buffer
     ahc::Solver solver;
-    vbx::Workspace vbx_ws, cent_ws;
+    DeviceBuffer<> vbx_pool;    // scratch of VBx refinement, centroids and K-Means
+    DeviceBuffer<> cent_pool;   // the pipeline's gamma / pi / ELBOs / centroids
     // pipeline buffers
-    void *d_buf = nullptr;
-    size_t d_bytes = 0;
-    void *h_buf = nullptr;
-    size_t h_bytes = 0;
-    cudaEvent_t ev[8] = {};
+    DeviceBuffer<> d_buf;
+    PinnedBuffer<> h_buf;
+    Event ev[8];
     bool ready = false;
     int worker_limit = 0;
 
     int init(int worker_lim) {
         FA_CUDA_TRY(cudaGetDevice(&device));
-        FA_CUDA_TRY(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-        for (auto &e : ev) FA_CUDA_TRY(cudaEventCreate(&e));
+        int st = stream.create();
+        for (auto &e : ev)
+            if (st == FA_OK) st = e.create();
+        if (st != FA_OK) return st;
         worker_limit = worker_lim;
-        const int st = solver.init(stream, worker_lim);
+        st = solver.init(stream, worker_lim);
         if (st != FA_OK) return st;
         ready = true;
         return FA_OK;
-    }
-    ~ClusterContext() {
-        if (d_buf) cudaFree(d_buf);
-        if (h_buf) cudaFreeHost(h_buf);
-        for (auto &e : ev)
-            if (e) cudaEventDestroy(e);
-        if (stream) cudaStreamDestroy(stream);
     }
 };
 
@@ -187,7 +181,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     double *d_emb, *d_rho, *d_train, *d_train_rho, *d_norm;
     unsigned char *d_ok;
     int *d_idx, *d_init, *d_hard, *d_labels, *d_count;
-    int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+    int st = carve_arena(C.d_buf, [&](Carver &c) {
         d_emb32 = c.take<float>(N * E);
         d_emb = c.take<double>(N * E);
         d_rho = c.take<double>(N * R);
@@ -206,13 +200,13 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     int *h_idx, *h_count;
     int32_t *h_init;
     double *h_Z;
-    st = carve_arena(C.h_buf, C.h_bytes, [&](Carver &c) {
+    st = carve_arena(C.h_buf, [&](Carver &c) {
         h_ok = c.take<unsigned char>(N);
         h_idx = c.take<int>(N);
         h_init = c.take<int32_t>(N);
         h_count = c.take<int>(16);
         h_Z = c.take<double>(N > 1 ? (N - 1) * 4 : 4);
-    }, 4096, true);
+    }, 4096);
     if (st != FA_OK) return st;
 
     FA_CUDA_TRY(cudaEventRecord(C.ev[0], s));
@@ -277,10 +271,10 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     FA_CUDA_TRY(cudaMemcpyAsync(d_init, h_init, Tn * sizeof(int), cudaMemcpyHostToDevice, s));
     // arena for gamma / pi / elbos / centroids (depends on S, known only now), at least 1 MB
     const vbx::Config vc = to_vbx(cfg.vbx);
-    st = grow_buffer(C.cent_ws.pool, C.cent_ws.pool_bytes, (size_t)1 << 20);
+    st = C.cent_pool.grow((size_t)1 << 20);
     if (st != FA_OK) return st;
     double *d_gamma, *d_pi, *d_elbos, *d_cent, *d_cent_n;
-    st = carve_arena(C.cent_ws.pool, C.cent_ws.pool_bytes, [&](Carver &c) {
+    st = carve_arena(C.cent_pool, [&](Carver &c) {
         d_gamma = c.take<double>((size_t)Tn * S);
         d_pi = c.take<double>(S);
         d_elbos = c.take<double>(std::max(vc.max_iterations, 1));
@@ -293,7 +287,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     if (psi) std::memcpy(psi_eff.data(), psi, R * sizeof(double));
     bool used_vbx = false;
     if (Tn > 0) {
-        st = vbx::refine_device(C.vbx_ws, d_tr_rho, Tn, r, psi_eff.data(), d_init, S, vc, d_gamma, d_pi, d_elbos, d_hard,
+        st = vbx::refine_device(C.vbx_pool, d_tr_rho, Tn, r, psi_eff.data(), d_init, S, vc, d_gamma, d_pi, d_elbos, d_hard,
                                 &iterations, s);
         if (st != FA_OK) return st;
         used_vbx = true;
@@ -311,13 +305,13 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
         if (detected < lo || detected > hi) {
             const int target = (int)(detected < lo ? lo : hi);
             // the arena may have moved: re-carve (gamma / pi are not needed any more on this path)
-            st = carve_arena(C.cent_ws.pool, C.cent_ws.pool_bytes, [&](Carver &c) {
+            st = carve_arena(C.cent_pool, [&](Carver &c) {
                 d_cent = c.take<double>((size_t)target * E + E);
                 d_cent_n = c.take<double>((size_t)target * E + E);
             }, 8192);
             if (st != FA_OK) return st;
             int rows = 0;
-            st = kmeans::cluster_ninit_device(C.vbx_ws, d_tr, Tn, e, target, 100, 10, 0ull, d_hard, d_cent, &rows, nullptr, s);
+            st = kmeans::cluster_ninit_device(C.vbx_pool, d_tr, Tn, e, target, 100, 10, 0ull, d_hard, d_cent, &rows, nullptr, s);
             if (st != FA_OK) return st;
             st = ahc::launch_normalize_rows_keep(d_cent, d_cent_n, rows, e, s);   // normalize (:824-860) for the cosine
             if (st != FA_OK) return st;
@@ -328,7 +322,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     FA_CUDA_TRY(cudaEventRecord(C.ev[5], s));
     // ---- centroids (:345-353) + assignment (:371-374) -----------------------------------------------------
     if (!adjusted) {
-        st = vbx::centroids_device(C.vbx_ws, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
+        st = vbx::centroids_device(C.vbx_pool, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));
@@ -337,7 +331,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
             // no speaker with pi > 1e-7: computeCentroidsFromClusters(initialClusters) (:687-690)
             st = vbx::onehot_device(d_init, Tn, S, d_gamma, d_pi, s);
             if (st != FA_OK) return st;
-            st = vbx::centroids_device(C.vbx_ws, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
+            st = vbx::centroids_device(C.vbx_pool, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
             if (st != FA_OK) return st;
             FA_CUDA_TRY(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
             FA_CUDA_TRY(cudaStreamSynchronize(s));
@@ -359,8 +353,7 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     const bool constrained = chunk_index != nullptr && K > 1 && !adjusted;   // :357-360
     double *d_scores = nullptr;
     if (constrained) {
-        st = carve_arena(C.vbx_ws.pool, C.vbx_ws.pool_bytes, [&](Carver &c) { d_scores = c.take<double>(N * (size_t)K); },
-                         1024);
+        st = carve_arena(C.vbx_pool, [&](Carver &c) { d_scores = c.take<double>(N * (size_t)K); }, 1024);
         if (st != FA_OK) return st;
     }
     st = vbx::assign_device(d_emb, n, e, d_cent_n, nullptr, K, d_labels, d_scores, s);
@@ -407,8 +400,16 @@ static int cluster_pipeline(ClusterContext &C, const float *emb, const double *r
     return FA_OK;
 }
 
-// timer state for fa_timer_*
-static thread_local cudaEvent_t t_ev0 = nullptr, t_ev1 = nullptr;
+// timer state for fa_timer_*, per thread
+static thread_local Event t_ev[2];
+
+// Creates both timer events, or neither: a failed creation leaves the timer unset, so the next start tries again.
+static int create_timer(Event (&ev)[2]) {
+    int st = ev[0].create();
+    if (st == FA_OK) st = ev[1].create();
+    if (st != FA_OK) ev[0].reset();
+    return st;
+}
 
 struct MelHandle {
     mel::MelPlan plan;
@@ -500,27 +501,22 @@ FA_API fa_status fa_memcpy_probe(const void *host_src, size_t h2d_bytes, void *h
                                  float *ms_per_round) {
     if (!ms_per_round || reps < 1 || (!host_src && h2d_bytes) || (!host_dst && d2h_bytes)) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
-    struct R {
-        void *a = nullptr, *b = nullptr;
-        cudaStream_t s[2] = {nullptr, nullptr};
-        ~R() {
-            if (a) cudaFree(a);
-            if (b) cudaFree(b);
-            for (auto x : s)
-                if (x) cudaStreamDestroy(x);
-        }
-    } r;
-    FA_CUDA_TRY(cudaMalloc(&r.a, h2d_bytes + 16));
-    FA_CUDA_TRY(cudaMalloc(&r.b, d2h_bytes + 16));
-    FA_CUDA_TRY(cudaMemset(r.b, 0, d2h_bytes + 16));
-    for (auto &x : r.s) FA_CUDA_TRY(cudaStreamCreateWithFlags(&x, cudaStreamNonBlocking));
+    Stream s[2];
+    DeviceBuffer<> a, b;
+    int st = a.grow(h2d_bytes + 16);
+    if (st == FA_OK) st = b.grow(d2h_bytes + 16);
+    if (st != FA_OK) return (fa_status)st;
+    FA_CUDA_TRY(cudaMemset(b.data(), 0, d2h_bytes + 16));
+    for (auto &x : s)
+        if (st == FA_OK) st = x.create();
+    if (st != FA_OK) return (fa_status)st;
     FA_CUDA_TRY(cudaDeviceSynchronize());
     const auto t0 = std::chrono::steady_clock::now();
     for (int i = 0; i < reps; ++i) {
-        if (h2d_bytes) FA_CUDA_TRY(cudaMemcpyAsync(r.a, host_src, h2d_bytes, cudaMemcpyHostToDevice, r.s[0]));
-        if (d2h_bytes) FA_CUDA_TRY(cudaMemcpyAsync(host_dst, r.b, d2h_bytes, cudaMemcpyDeviceToHost, r.s[1]));
-        FA_CUDA_TRY(cudaStreamSynchronize(r.s[0]));
-        FA_CUDA_TRY(cudaStreamSynchronize(r.s[1]));
+        if (h2d_bytes) FA_CUDA_TRY(cudaMemcpyAsync(a.data(), host_src, h2d_bytes, cudaMemcpyHostToDevice, s[0]));
+        if (d2h_bytes) FA_CUDA_TRY(cudaMemcpyAsync(host_dst, b.data(), d2h_bytes, cudaMemcpyDeviceToHost, s[1]));
+        FA_CUDA_TRY(cudaStreamSynchronize(s[0]));
+        FA_CUDA_TRY(cudaStreamSynchronize(s[1]));
     }
     const auto t1 = std::chrono::steady_clock::now();
     *ms_per_round = (float)(std::chrono::duration<double, std::milli>(t1 - t0).count() / reps);
@@ -532,20 +528,20 @@ FA_API fa_status fa_memcpy_probe(const void *host_src, size_t h2d_bytes, void *h
 // are timed by the caller bracketing fa_device_synchronize()).
 FA_API fa_status fa_timer_start(void) {
     API_REQUIRE_DEVICE();
-    if (!t_ev0) {
-        FA_CUDA_TRY(cudaEventCreate(&t_ev0));
-        FA_CUDA_TRY(cudaEventCreate(&t_ev1));
+    if (!t_ev[0]) {
+        const int st = create_timer(t_ev);
+        if (st != FA_OK) return (fa_status)st;
     }
     FA_CUDA_TRY(cudaDeviceSynchronize());
-    FA_CUDA_TRY(cudaEventRecord(t_ev0, 0));
+    FA_CUDA_TRY(cudaEventRecord(t_ev[0], 0));
     return FA_STATUS_OK;
 }
 FA_API fa_status fa_timer_stop_ms(float *elapsed_ms) {
-    if (!elapsed_ms || !t_ev0) return FA_STATUS_INVALID_ARGUMENT;
+    if (!elapsed_ms || !t_ev[0]) return FA_STATUS_INVALID_ARGUMENT;
     FA_CUDA_TRY(cudaDeviceSynchronize());
-    FA_CUDA_TRY(cudaEventRecord(t_ev1, 0));
-    FA_CUDA_TRY(cudaEventSynchronize(t_ev1));
-    FA_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, t_ev0, t_ev1));
+    FA_CUDA_TRY(cudaEventRecord(t_ev[1], 0));
+    FA_CUDA_TRY(cudaEventSynchronize(t_ev[1]));
+    FA_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, t_ev[0], t_ev[1]));
     return FA_STATUS_OK;
 }
 
@@ -700,8 +696,8 @@ FA_API fa_status fa_mel_timer_start(fa_mel *mel) {
     if (!mel) return FA_STATUS_INVALID_ARGUMENT;
     auto *h = reinterpret_cast<MelHandle *>(mel);
     if (!h->plan.timer[0]) {
-        FA_CUDA_TRY(cudaEventCreate(&h->plan.timer[0]));
-        FA_CUDA_TRY(cudaEventCreate(&h->plan.timer[1]));
+        const int st = create_timer(h->plan.timer);
+        if (st != FA_OK) return (fa_status)st;
     }
     FA_CUDA_TRY(cudaStreamSynchronize(h->plan.streams[1]));
     FA_CUDA_TRY(cudaEventRecord(h->plan.timer[0], h->plan.streams[1]));
@@ -852,29 +848,21 @@ FA_API fa_status fa_audio_resample(const void *pcm, int64_t frames, const fa_aud
         if (st != FA_OK) return (fa_status)st;
     }
     const size_t bytes = (size_t)frames * f.channels * (f.format == resample::kPcmI16 ? 2 : 4);
-    struct Bufs {
-        void *pcm = nullptr;
-        float *tab = nullptr, *out = nullptr;
-        cudaStream_t s = nullptr;
-        ~Bufs() {
-            if (pcm) cudaFree(pcm);
-            if (tab) cudaFree(tab);
-            if (out) cudaFree(out);
-            if (s) cudaStreamDestroy(s);
-        }
-    } b;
-    FA_CUDA_TRY(cudaStreamCreateWithFlags(&b.s, cudaStreamNonBlocking));
-    FA_CUDA_TRY(cudaMalloc(&b.pcm, bytes + 16));
-    FA_CUDA_TRY(cudaMalloc(&b.out, (size_t)n * sizeof(float)));
-    if (!d.table.empty()) {
-        FA_CUDA_TRY(cudaMalloc(&b.tab, d.table.size() * sizeof(float)));
-        FA_CUDA_TRY(cudaMemcpyAsync(b.tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice, b.s));
-    }
-    FA_CUDA_TRY(cudaMemcpyAsync(b.pcm, pcm, bytes, cudaMemcpyHostToDevice, b.s));
-    const int st = resample::launch_convert(b.pcm, frames, f, d, b.tab, b.out, 0, n, b.s);
+    Stream s;
+    DeviceBuffer<> d_pcm;
+    DeviceBuffer<float> d_tab, d_out;
+    int st = s.create();
+    if (st == FA_OK) st = d_pcm.grow(bytes + 16);
+    if (st == FA_OK) st = d_out.grow((size_t)n * sizeof(float));
+    if (st == FA_OK) st = d_tab.grow(d.table.size() * sizeof(float));
     if (st != FA_OK) return (fa_status)st;
-    FA_CUDA_TRY(cudaMemcpyAsync(out, b.out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, b.s));
-    FA_CUDA_TRY(cudaStreamSynchronize(b.s));
+    if (!d.table.empty())
+        FA_CUDA_TRY(cudaMemcpyAsync(d_tab.data(), d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_pcm.data(), pcm, bytes, cudaMemcpyHostToDevice, s));
+    st = resample::launch_convert(d_pcm.data(), frames, f, d, d_tab.data(), d_out.data(), 0, n, s);
+    if (st != FA_OK) return (fa_status)st;
+    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out.data(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    FA_CUDA_TRY(cudaStreamSynchronize(s));
     return FA_STATUS_OK;
     FA_GUARD_END
 }
@@ -968,7 +956,7 @@ FA_API fa_status fa_l2_normalize_rows(const double *x, size_t rows, size_t dim, 
     FA_GUARD_BEGIN
     return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
         double *d_in, *d_out;
-        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
             d_in = c.take<double>(rows * dim);
             d_out = c.take<double>(rows * dim);
         }, 512);
@@ -1008,12 +996,12 @@ FA_API fa_status fa_ahc_cluster(const double *features, size_t count, size_t dim
     FA_GUARD_BEGIN
     return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
         double *d_in, *d_norm, *h_Z;
-        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
             d_in = c.take<double>(count * dim);
             d_norm = c.take<double>(count * dim);
         }, 512);
         if (st != FA_OK) return st;
-        st = carve_arena(C.h_buf, C.h_bytes, [&](Carver &c) { h_Z = c.take<double>((count - 1) * 4); }, 512, true);
+        st = carve_arena(C.h_buf, [&](Carver &c) { h_Z = c.take<double>((count - 1) * 4); }, 512);
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
         st = ahc::launch_normalize_rows(d_in, d_norm, (int)count, (int)dim, C.stream);
@@ -1132,7 +1120,7 @@ FA_API fa_status fa_kmeans_cluster(const double *emb, size_t N, size_t D, int32_
     return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
         double *d_emb, *d_cent;
         int *d_labels;
-        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
             d_emb = c.take<double>(N * D);
             d_cent = c.take<double>((size_t)rows_needed * D);
             d_labels = c.take<int>(N);
@@ -1140,7 +1128,7 @@ FA_API fa_status fa_kmeans_cluster(const double *emb, size_t N, size_t D, int32_
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
         int rows = 0, best = 0;
-        st = kmeans::cluster_ninit_device(C.vbx_ws, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
+        st = kmeans::cluster_ninit_device(C.vbx_pool, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
                                           d_labels, d_cent, &rows, &best, C.stream);
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
@@ -1163,7 +1151,7 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
         const int cap = std::max(cfg->max_iterations, 1);
         double *d_x, *d_gamma, *d_pi, *d_elbos;
         int *d_init, *d_hard;
-        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
             d_x = c.take<double>(T * D);
             d_init = c.take<int>(T);
             d_gamma = c.take<double>(T * (size_t)S);
@@ -1177,7 +1165,7 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
         FA_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
         if (initial) FA_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
         int its = 0;
-        st = vbx::refine_device(C.vbx_ws, d_x, (int)T, (int)D, psi_eff.data(), initial ? d_init : nullptr, S, to_vbx(*cfg),
+        st = vbx::refine_device(C.vbx_pool, d_x, (int)T, (int)D, psi_eff.data(), initial ? d_init : nullptr, S, to_vbx(*cfg),
                                 d_gamma, d_pi, d_elbos, d_hard, &its, C.stream);
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
@@ -1200,7 +1188,7 @@ FA_API fa_status fa_compute_centroids(const double *emb, size_t T, size_t dim, c
     return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
         double *d_emb, *d_gamma, *d_pi, *d_cent, *d_cent_n;
         int *d_count;
-        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
             d_emb = c.take<double>(T * dim);
             d_gamma = c.take<double>(T * (size_t)S);
             d_pi = c.take<double>(S);
@@ -1212,7 +1200,7 @@ FA_API fa_status fa_compute_centroids(const double *emb, size_t T, size_t dim, c
         FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
         FA_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
         FA_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        st = vbx::centroids_device(C.vbx_ws, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream);
+        st = vbx::centroids_device(C.vbx_pool, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream);
         if (st != FA_OK) return st;
         int K = 0;
         FA_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
@@ -1240,7 +1228,7 @@ FA_API fa_status fa_assign_embeddings(const double *emb, size_t N, size_t dim, c
     return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
         double *d_emb, *d_craw, *d_cn, *d_scores;
         int *d_labels;
-        int st = carve_arena(C.d_buf, C.d_bytes, [&](Carver &c) {
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
             d_emb = c.take<double>(N * dim);
             d_craw = c.take<double>((size_t)K * dim);
             d_cn = c.take<double>((size_t)K * dim);

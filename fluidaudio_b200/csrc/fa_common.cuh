@@ -6,6 +6,9 @@
 
 #if defined(__CUDACC__)
 #include <atomic>
+#include <cstdio>
+#include <memory>
+#include <type_traits>
 #include <utility>
 #include <cuda_runtime.h>
 #define FA_HD __host__ __device__ __forceinline__
@@ -64,33 +67,118 @@ inline CudaStatus cuda_failure(cudaError_t e, const char *expr, const char *file
         if (e__ != cudaSuccess) return fa::cuda_failure(e__, #expr, __FILE__, __LINE__); \
     } while (0)
 
-// Grow-only device (or pinned host) buffer: keeps `p` when it already holds `bytes`, otherwise replaces it.  It never
-// shrinks, and a failed allocation leaves `p` null and `cap` zero.
-template <typename T> int grow_buffer(T *&p, size_t &cap, size_t bytes, bool pinned = false) {
-    if (bytes <= cap) return FA_OK;
-    if (p) pinned ? cudaFreeHost(p) : cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    void *q = nullptr;
-    FA_CUDA_TRY(pinned ? cudaMallocHost(&q, bytes) : cudaMalloc(&q, bytes));
-    p = static_cast<T *>(q);
-    cap = bytes;
-    return FA_OK;
-}
+// Owners of the library's CUDA resources.  Every cudaMalloc / cudaMallocHost, stream and event of the library is made
+// here and released by a destructor, which ignores errors: the static context pool is torn down at process exit, when
+// the runtime may already be gone.
+template <bool Pinned> struct CudaFree {
+    void operator()(void *p) const { Pinned ? cudaFreeHost(p) : cudaFree(p); }
+};
+
+// Grow-only device (or pinned host) buffer of T: grow() keeps the allocation when it already holds `bytes`, otherwise
+// frees it before allocating the larger one (peak memory is the larger size alone).  It never shrinks, and a failed
+// allocation leaves it empty.
+template <typename T, bool Pinned> class GrowBuffer {
+  public:
+    GrowBuffer() = default;
+    GrowBuffer(GrowBuffer &&o) noexcept : p_(std::move(o.p_)), cap_(std::exchange(o.cap_, 0)) {}
+    GrowBuffer &operator=(GrowBuffer &&o) noexcept {
+        p_ = std::move(o.p_);
+        cap_ = std::exchange(o.cap_, 0);
+        return *this;
+    }
+    int grow(size_t bytes) {
+        if (bytes <= cap_) return FA_OK;
+        p_.reset();
+        cap_ = 0;
+        void *q = nullptr;
+        const cudaError_t e = Pinned ? cudaMallocHost(&q, bytes) : cudaMalloc(&q, bytes);
+        if (e != cudaSuccess) {
+            char what[64];
+            std::snprintf(what, sizeof(what), "%s(%zu bytes)", Pinned ? "cudaMallocHost" : "cudaMalloc", bytes);
+            return cuda_failure(e, what, __FILE__, __LINE__);
+        }
+        p_.reset(q);
+        cap_ = bytes;
+        return FA_OK;
+    }
+    T *data() const { return static_cast<T *>(p_.get()); }
+    size_t capacity() const { return cap_; }
+
+  private:
+    std::unique_ptr<void, CudaFree<Pinned>> p_;
+    size_t cap_ = 0;
+};
+template <typename T = void> using DeviceBuffer = GrowBuffer<T, false>;
+template <typename T = void> using PinnedBuffer = GrowBuffer<T, true>;
 
 // Lays out one scratch arena in a grow-only buffer.  `layout(Carver &)` takes every array of the arena in order and
 // only assigns the pointers it gets, so it is safe to run twice: once over a null base to size the arena (plus `slack`
 // bytes), then, after the buffer has grown to that size, over the buffer itself.
-template <typename T, typename Layout>
-int carve_arena(T *&buf, size_t &cap, Layout &&layout, size_t slack = 0, bool pinned = false) {
+template <typename T, bool Pinned, typename Layout>
+int carve_arena(GrowBuffer<T, Pinned> &buf, Layout &&layout, size_t slack = 0) {
     Carver size{nullptr};
     layout(size);
-    const int st = grow_buffer(buf, cap, size.off + slack, pinned);
+    const int st = buf.grow(size.off + slack);
     if (st != FA_OK) return st;
-    Carver c{static_cast<char *>(static_cast<void *>(buf))};
+    Carver c{static_cast<char *>(static_cast<void *>(buf.data()))};
     layout(c);
     return FA_OK;
 }
+
+// Owned stream and event: empty until create() succeeds, and usable wherever the raw handle is.
+struct StreamDestroy {
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+struct EventDestroy {
+    void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+struct Stream : std::unique_ptr<std::remove_pointer_t<cudaStream_t>, StreamDestroy> {
+    operator cudaStream_t() const { return get(); }
+    int create(unsigned flags = cudaStreamNonBlocking) {
+        cudaStream_t s = nullptr;
+        FA_CUDA_TRY(cudaStreamCreateWithFlags(&s, flags));
+        reset(s);
+        return FA_OK;
+    }
+};
+struct Event : std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDestroy> {
+    operator cudaEvent_t() const { return get(); }
+    int create(unsigned flags = cudaEventDefault) {
+        cudaEvent_t e = nullptr;
+        FA_CUDA_TRY(cudaEventCreateWithFlags(&e, flags));
+        reset(e);
+        return FA_OK;
+    }
+};
+
+// Launch descriptors written in a pinned buffer and uploaded to its device twin.  An asynchronous call returns with its
+// upload still queued, so the pinned copy may be rewritten (or replaced) only once that upload has read it: reserve()
+// waits for the last upload before it grows the buffers, and upload() records the event reserve() waits on.
+template <typename T = void> struct UploadStage {
+    PinnedBuffer<T> host;
+    DeviceBuffer<T> device;
+    Event uploaded;
+    bool in_flight = false;
+
+    int reserve(size_t bytes) {
+        if (in_flight) {
+            FA_CUDA_TRY(cudaEventSynchronize(uploaded));
+            in_flight = false;
+        }
+        const int st = device.grow(bytes);
+        return st != FA_OK ? st : host.grow(bytes);
+    }
+    int upload(size_t bytes, cudaStream_t stream) {
+        if (!uploaded) {
+            const int st = uploaded.create(cudaEventDisableTiming);
+            if (st != FA_OK) return st;
+        }
+        FA_CUDA_TRY(cudaMemcpyAsync(device.data(), host.data(), bytes, cudaMemcpyHostToDevice, stream));
+        FA_CUDA_TRY(cudaEventRecord(uploaded, stream));
+        in_flight = true;
+        return FA_OK;
+    }
+};
 
 // Kernel launches of the whole process (fa_kernel_launch_count), defined in capi.cu.  Every launch of the library goes
 // through launch() or launch_cooperative(), which count it where it is issued and return its error:

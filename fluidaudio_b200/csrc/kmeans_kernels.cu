@@ -219,7 +219,7 @@ void resolve_constraints(long long num_embeddings, long long num_speakers, long 
     *hi_out = hi;
 }
 
-int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, int num_clusters, int max_iterations,
+int cluster_ninit_device(DeviceBuffer<> &pool, const double *d_emb, int N, int D, int num_clusters, int max_iterations,
                          int n_init, unsigned long long base_seed, int *d_labels, double *d_centroids, int *rows,
                          int *best_init, cudaStream_t s) {
     if (rows) *rows = 0;
@@ -248,7 +248,7 @@ int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, 
     double *d_x, *d_xt, *d_cent, *d_pp;
     int *d_perm, *d_lab[2], *d_counts;
     RunState *d_state;
-    const int st = carve_arena(ws.pool, ws.pool_bytes, [&](Carver &c) {
+    const int st = carve_arena(pool, [&](Carver &c) {
         d_x = c.take<double>((size_t)N * D);
         d_xt = c.take<double>((size_t)N * D);
         d_cent = c.take<double>((size_t)k * D);

@@ -2,7 +2,6 @@
 #pragma once
 
 #include "fa_common.cuh"
-#include "vbx_plan.h"
 #include <cuda_runtime.h>
 
 namespace fa {
@@ -10,8 +9,8 @@ namespace kmeans {
 
 // KMeansClustering.clusterWithCentroidsNInit on device-resident raw embeddings d_emb [N x D] (row-major doubles).
 // d_labels [N] and d_centroids [min(k, N) x D] receive the winning run; *rows the number of centroid rows,
-// *best_init the index of the winning seed.  Scratch comes from `ws`.
-int cluster_ninit_device(vbx::Workspace &ws, const double *d_emb, int N, int D, int num_clusters, int max_iterations,
+// *best_init the index of the winning seed.  Scratch comes from `pool`.
+int cluster_ninit_device(DeviceBuffer<> &pool, const double *d_emb, int N, int D, int num_clusters, int max_iterations,
                          int n_init, unsigned long long base_seed, int *d_labels, double *d_centroids, int *rows,
                          int *best_init, cudaStream_t stream);
 

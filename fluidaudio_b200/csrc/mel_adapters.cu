@@ -78,16 +78,14 @@ __global__ void per_feature_norm_inplace_kernel(float *x, long long T, int M, lo
 
 // host buffer in, host buffer out (x: [T x M] time-major, normalised in place); valid >= 1
 int normalize_per_feature_host(float *x, long long T, int M, long long valid) {
-    struct Buf {
-        float *d = nullptr;
-        ~Buf() { if (d) cudaFree(d); }
-    } b;
+    DeviceBuffer<float> d;
     const size_t bytes = sizeof(float) * (size_t)T * M;
-    FA_CUDA_TRY(cudaMalloc(&b.d, bytes));
-    FA_CUDA_TRY(cudaMemcpy(b.d, x, bytes, cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(fa::launch(per_feature_norm_inplace_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, 0, b.d, T,
-                           M, valid));
-    FA_CUDA_TRY(cudaMemcpy(x, b.d, bytes, cudaMemcpyDeviceToHost));
+    const int st = d.grow(bytes);
+    if (st != FA_OK) return st;
+    FA_CUDA_TRY(cudaMemcpy(d.data(), x, bytes, cudaMemcpyHostToDevice));
+    FA_CUDA_TRY(fa::launch(per_feature_norm_inplace_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, 0, d.data(),
+                           T, M, valid));
+    FA_CUDA_TRY(cudaMemcpy(x, d.data(), bytes, cudaMemcpyDeviceToHost));
     return FA_OK;
 }
 
@@ -119,10 +117,10 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
     int st = p.ensure_staging((size_t)n + 16, (size_t)(2 * T * M));
     if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
-    float *d_flat = p.d_out, *d_pack = p.d_out + T * M;
-    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio, window, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
+    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), window, sizeof(float) * n, cudaMemcpyHostToDevice, s));
     long long ml = 0, nf = 0;
-    st = p.compute_device(p.d_audio, n, 0.0f, 0, T, 0, d_flat, T * M, &ml, &nf, s);
+    st = p.compute_device(p.d_audio.data(), n, 0.0f, 0, T, 0, d_flat, T * M, &ml, &nf, s);
     if (st != FA_OK) return st;
     if (valid <= 0) {
         FA_CUDA_TRY(cudaMemsetAsync(d_pack, 0, sizeof(float) * T * M, s));
@@ -148,11 +146,11 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
     int st = p.ensure_staging((size_t)n + 16, (size_t)(T * M + M));
     if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
-    float *d_flat = p.d_out, *d_mean = p.d_out + T * M;
-    FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio, chunk, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    float *d_flat = p.d_out.data(), *d_mean = d_flat + T * M;
+    FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), chunk, sizeof(float) * n, cudaMemcpyHostToDevice, s));
     FA_CUDA_TRY(cudaMemcpyAsync(d_mean, cmn_mean, sizeof(float) * M, cudaMemcpyHostToDevice, s));
     long long ml = 0, nf = 0;
-    st = p.compute_device(p.d_audio, n, 0.0f, 1, -1, 0, d_flat, T * M, &ml, &nf, s);
+    st = p.compute_device(p.d_audio.data(), n, 0.0f, 1, -1, 0, d_flat, T * M, &ml, &nf, s);
     if (st != FA_OK) return st;
     const float scale = 1.0f / logf(10.0f);   // LSEENDPreprocessor.swift:36, Float arithmetic
     FA_CUDA_TRY(fa::launch(lseend_scale_cmn_kernel, (M + 127) / 128, 128, 0, s, d_flat, T, M, d_mean, *cmn_count, scale));

@@ -462,44 +462,12 @@ void build_filterbank(int n_fft, int n_mels, int sample_rate, std::vector<float>
 static constexpr int kWarpsPerCta = 8;
 static constexpr int kCtasPerSm = 2;
 
-MelPlan::~MelPlan() { release(); }
-
-void MelPlan::release() {
-    auto fr = [](auto *&p) {
-        if (p) cudaFree(p);
-        p = nullptr;
-    };
-    for (int m = 0; m < 2; ++m) {
-        fr(d_win_tab_mode[m]);
-        fr(d_in_tab_mode[m]);
-        fr(d_lane_tab[m][0]);
-        fr(d_lane_tab[m][1]);
-    }
-    fr(d_fb_w);
-    fr(d_fb_slots);
-    fr(d_fb_lo);
-    fr(d_fb_hi);
-    fr(d_fb_off);
-    fr(d_units);
-    fr(d_audio);
-    fr(d_out);
-    fr(d_pcm);
-    fr(d_rs_tab);
-    fr(d_generic_tw);
-    rs_in = rs_out = 0.0;
-    d_units_bytes = h_units_bytes = d_audio_bytes = d_out_bytes = d_pcm_bytes = rs_tab_bytes = 0;
-    if (h_units) cudaFreeHost(h_units);
-    h_units = nullptr;
-    if (units_uploaded) cudaEventDestroy(units_uploaded);
-    units_uploaded = nullptr;
-    units_in_flight = false;
-    for (auto &s : streams)
-        if (s) cudaStreamDestroy(s), s = nullptr;
-    for (auto &e : events)
-        if (e) cudaEventDestroy(e);
-    events.clear();
-    for (auto &e : timer)
-        if (e) cudaEventDestroy(e), e = nullptr;
+// Device copy of a host table (at least one element, so that an empty table still has an address).
+template <typename T, typename U> static int upload_table(DeviceBuffer<T> &b, const std::vector<U> &v) {
+    const int st = b.grow(std::max<size_t>(1, v.size()) * sizeof(U));
+    if (st != FA_OK) return st;
+    if (!v.empty()) FA_CUDA_TRY(cudaMemcpy(b.data(), v.data(), v.size() * sizeof(U), cudaMemcpyHostToDevice));
+    return FA_OK;
 }
 
 int MelPlan::init(const MelConfig &c) {
@@ -581,7 +549,7 @@ int MelPlan::init(const MelConfig &c) {
     int dev = 0;
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
-    const int st = sm90_device_props(dev, prop);
+    int st = sm90_device_props(dev, prop);
     if (st != FA_OK) return st;
     num_sms = prop.multiProcessorCount;
 
@@ -621,10 +589,9 @@ int MelPlan::init(const MelConfig &c) {
             win_tab[off_w + j] = window[j];
             in_tab[off_w + j] = 1;
         }
-        FA_CUDA_TRY(cudaMalloc(&d_win_tab_mode[mode], n_fft * sizeof(float)));
-        FA_CUDA_TRY(cudaMalloc(&d_in_tab_mode[mode], n_fft));
-        FA_CUDA_TRY(cudaMemcpy(d_win_tab_mode[mode], win_tab.data(), n_fft * sizeof(float), cudaMemcpyHostToDevice));
-        FA_CUDA_TRY(cudaMemcpy(d_in_tab_mode[mode], in_tab.data(), n_fft, cudaMemcpyHostToDevice));
+        st = upload_table(d_win_tab_mode[mode], win_tab);
+        if (st == FA_OK) st = upload_table(d_in_tab_mode[mode], in_tab);
+        if (st != FA_OK) return st;
         if (!generic) {
             std::vector<LaneTables<double>> t64(32);
             std::vector<LaneTables<f32x2>> t32(32);
@@ -632,31 +599,25 @@ int MelPlan::init(const MelConfig &c) {
                 load_lane_tables(l, win_tab.data(), in_tab.data(), t64[l]);
                 load_lane_tables(l, win_tab.data(), in_tab.data(), t32[l]);
             }
-            FA_CUDA_TRY(cudaMalloc(&d_lane_tab[mode][0], 32 * sizeof(LaneTables<double>)));
-            FA_CUDA_TRY(cudaMalloc(&d_lane_tab[mode][1], 32 * sizeof(LaneTables<f32x2>)));
-            FA_CUDA_TRY(cudaMemcpy(d_lane_tab[mode][0], t64.data(), 32 * sizeof(LaneTables<double>), cudaMemcpyHostToDevice));
-            FA_CUDA_TRY(cudaMemcpy(d_lane_tab[mode][1], t32.data(), 32 * sizeof(LaneTables<f32x2>), cudaMemcpyHostToDevice));
+            st = upload_table(d_lane_tab[mode][0], t64);
+            if (st == FA_OK) st = upload_table(d_lane_tab[mode][1], t32);
+            if (st != FA_OK) return st;
         }
     }
-    FA_CUDA_TRY(cudaMalloc(&d_fb_w, std::max<size_t>(1, w.size()) * sizeof(float)));
-    FA_CUDA_TRY(cudaMalloc(&d_fb_slots, std::max<size_t>(1, slots.size()) * sizeof(int4)));
-    if (!slots.empty())
-        FA_CUDA_TRY(cudaMemcpy(d_fb_slots, slots.data(), slots.size() * sizeof(int4), cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(cudaMalloc(&d_fb_lo, cfg.n_mels * sizeof(int)));
-    FA_CUDA_TRY(cudaMalloc(&d_fb_hi, cfg.n_mels * sizeof(int)));
-    FA_CUDA_TRY(cudaMalloc(&d_fb_off, cfg.n_mels * sizeof(int)));
-    if (!w.empty()) FA_CUDA_TRY(cudaMemcpy(d_fb_w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(cudaMemcpy(d_fb_lo, lo.data(), cfg.n_mels * sizeof(int), cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(cudaMemcpy(d_fb_hi, hi.data(), cfg.n_mels * sizeof(int), cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(cudaMemcpy(d_fb_off, off.data(), cfg.n_mels * sizeof(int), cudaMemcpyHostToDevice));
-
-    for (auto &st : streams) FA_CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    st = upload_table(d_fb_w, w);
+    if (st == FA_OK) st = upload_table(d_fb_slots, slots);
+    if (st == FA_OK) st = upload_table(d_fb_lo, lo);
+    if (st == FA_OK) st = upload_table(d_fb_hi, hi);
+    if (st == FA_OK) st = upload_table(d_fb_off, off);
+    for (auto &s : streams)
+        if (st == FA_OK) st = s.create();
+    if (st != FA_OK) return st;
     if (generic) {
         // FP64 twiddle table W_n^k and the shared-memory budget: as many warps per CTA as fit beside it
         std::vector<cpxd> tw(n_fft / 2);
         for (int k = 0; k < n_fft / 2; ++k) tw[k] = unit_root(k, n_fft);
-        FA_CUDA_TRY(cudaMalloc(&d_generic_tw, tw.size() * sizeof(cpxd)));
-        FA_CUDA_TRY(cudaMemcpy(d_generic_tw, tw.data(), tw.size() * sizeof(cpxd), cudaMemcpyHostToDevice));
+        st = upload_table(d_generic_tw, tw);
+        if (st != FA_OK) return st;
         generic_prow = ((bins + 3) & ~3) + 4;
         int log2n = 0;
         while ((1 << log2n) < n_fft) ++log2n;
@@ -687,49 +648,26 @@ long long MelPlan::frame_count(long long n, int mode, long long expected) const 
     return expected >= 0 ? expected : computed;
 }
 
-int MelPlan::ensure_units(int count) {
-    // the device entry points return with their descriptor upload still queued behind earlier work on the stream: the
-    // pinned h_units may be rewritten (or replaced) only once that copy has read it
-    if (units_in_flight) {
-        FA_CUDA_TRY(cudaEventSynchronize(units_uploaded));
-        units_in_flight = false;
-    }
-    const size_t bytes = (size_t)std::max(count, 64) * sizeof(MelUnit);
-    const int st = grow_buffer(d_units, d_units_bytes, bytes);
-    return st != FA_OK ? st : grow_buffer(h_units, h_units_bytes, bytes, true);
-}
-
-int MelPlan::upload_units(int count, cudaStream_t stream) {
-    if (!units_uploaded) FA_CUDA_TRY(cudaEventCreateWithFlags(&units_uploaded, cudaEventDisableTiming));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, count * sizeof(MelUnit), cudaMemcpyHostToDevice, stream));
-    FA_CUDA_TRY(cudaEventRecord(units_uploaded, stream));
-    units_in_flight = true;
-    return FA_OK;
-}
+// bytes of the unit descriptors of a call with `count` units
+static size_t unit_bytes(int count) { return (size_t)std::max(count, 64) * sizeof(MelUnit); }
 
 int MelPlan::ensure_staging(size_t audio_floats, size_t out_floats) {
-    const int st = grow_buffer(d_audio, d_audio_bytes, audio_floats * sizeof(float));
-    return st != FA_OK ? st : grow_buffer(d_out, d_out_bytes, out_floats * sizeof(float));
+    const int st = d_audio.grow(audio_floats * sizeof(float));
+    return st != FA_OK ? st : d_out.grow(out_floats * sizeof(float));
 }
 
 int MelPlan::ensure_events(size_t count) {
     while (events.size() < count) {
-        cudaEvent_t e;
-        FA_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        events.push_back(e);
+        Event e;
+        const int st = e.create(cudaEventDisableTiming);
+        if (st != FA_OK) return st;
+        events.push_back(std::move(e));
     }
     return FA_OK;
 }
 
-int MelPlan::launch(const float *d_audio_base, float *d_out_base, int first, int count, int total_tiles, int mode,
-                    int layout, cudaStream_t stream, bool aligned16) {
-    return launch_units(d_units + first, h_units + first, count, d_audio_base, d_out_base, total_tiles, mode, layout,
-                        stream, aligned16);
-}
-
-int MelPlan::launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, const float *d_audio_base,
-                          float *d_out_base, int total_tiles, int mode, int layout, cudaStream_t stream,
-                          bool aligned16) {
+int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inline_unit, const float *d_audio_base,
+                    float *d_out_base, int total_tiles, int mode, int layout, cudaStream_t stream, bool aligned16) {
     if (total_tiles <= 0) return FA_OK;
     MelLaunch P{};
     P.audio = d_audio_base;
@@ -747,20 +685,20 @@ int MelPlan::launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, con
     P.log_clamped = cfg.log_floor_mode;
     P.ot_stride = (cfg.n_mels & 3) == 0 ? cfg.n_mels + 4 : cfg.n_mels + 1;
     // float4 copy-out only when every destination row is 16-byte aligned: the caller's d_out, a batch's out_offsets or a
-    // pinned output may sit at any 4-byte boundary (h_units mirrors the units of every launch)
+    // pinned output may sit at any 4-byte boundary (h_u mirrors the launch's units)
     P.out_vec4 = (cfg.n_mels & 3) == 0 && (reinterpret_cast<uintptr_t>(d_out_base) & 15) == 0;
     for (int i = 0; i < count && P.out_vec4; ++i) P.out_vec4 = (h_u[i].out_off & 3) == 0;
     P.log_normal = cfg.log_floor >= 1e-37f ? 1 : 0;   // mel energies are >= 0: log's argument is then never a denormal
     P.layout = layout;
-    P.lane_tab = d_lane_tab[mode == 2 ? 1 : 0][precision == 1 ? 1 : 0];
-    P.win_tab = d_win_tab_mode[mode == 2 ? 1 : 0];
-    P.in_tab = d_in_tab_mode[mode == 2 ? 1 : 0];
-    P.fb_w = d_fb_w;
-    P.fb_slots = reinterpret_cast<const int4 *>(d_fb_slots);
+    P.lane_tab = d_lane_tab[mode == 2 ? 1 : 0][precision == 1 ? 1 : 0].data();
+    P.win_tab = d_win_tab_mode[mode == 2 ? 1 : 0].data();
+    P.in_tab = d_in_tab_mode[mode == 2 ? 1 : 0].data();
+    P.fb_w = d_fb_w.data();
+    P.fb_slots = d_fb_slots.data();
     P.n_slots = n_slots;
-    P.fb_lo = d_fb_lo;
-    P.fb_hi = d_fb_hi;
-    P.fb_off = d_fb_off;
+    P.fb_lo = d_fb_lo.data();
+    P.fb_hi = d_fb_hi.data();
+    P.fb_off = d_fb_off.data();
     P.fb_nnz = fb_nnz;
     P.fb_cap = fb_cap;
     P.pt_len = pt_len;
@@ -773,8 +711,8 @@ int MelPlan::launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, con
     }
     P.inv_n_mels = (unsigned)((0x100000000ull + (unsigned)cfg.n_mels - 1) / (unsigned)cfg.n_mels);
     if (generic) {
-        GenericParams G{cfg.n_fft, generic_log2n, cfg.n_fft / 2 + 1, generic_prow, reinterpret_cast<const cpxd *>(d_generic_tw),
-                        generic_warps};
+        GenericParams G{cfg.n_fft, generic_log2n, cfg.n_fft / 2 + 1, generic_prow,
+                        static_cast<const cpxd *>(d_generic_tw.data()), generic_warps};
         const int ggrid = std::min(total_tiles, num_sms * std::max(1, 16 / generic_warps));
         FA_CUDA_TRY(fa::launch(mel_generic_kernel, ggrid, generic_warps * 32, smem_bytes, stream, P, G));
         return FA_OK;
@@ -827,21 +765,23 @@ int MelPlan::compute_device(const float *d_in, long long n, float last, int mode
         if (Tp) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf, 0, cfg.n_mels * sizeof(float), stream));
         return FA_OK;
     }
-    st = ensure_units(1);
+    st = units.reserve(unit_bytes(1));
     if (st != FA_OK) return st;
     if (Tp > T) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf, 0, Tp * cfg.n_mels * sizeof(float), stream));
-    h_units[0] = MelUnit{0, n, 0, Tp, 0, T, last, 0};
-    st = upload_units(1, stream);
+    units.host.data()[0] = MelUnit{0, n, 0, Tp, 0, T, last, 0};
+    st = units.upload(sizeof(MelUnit), stream);
     if (st != FA_OK) return st;
     const bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
-    return launch(d_in, d_out_buf, 0, 1, tiles_of(T), mode, layout, stream, aligned);
+    return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, tiles_of(T), mode, layout, stream,
+                  aligned);
 }
 
 int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, int count, const float *last, int mode,
                                   int layout, float *d_out_buf, const long long *out_offsets, long long *mel_lengths,
                                   long long *num_frames, cudaStream_t stream) {
-    int st = ensure_units(count);
+    int st = units.reserve(unit_bytes(count));
     if (st != FA_OK) return st;
+    MelUnit *h_units = units.host.data();
     int tiles = 0, used = 0;
     bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
     for (int i = 0; i < count; ++i) {
@@ -860,9 +800,9 @@ int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, i
         ++used;
     }
     if (!used) return FA_OK;
-    st = upload_units(used, stream);
+    st = units.upload(used * sizeof(MelUnit), stream);
     if (st != FA_OK) return st;
-    return launch(d_in, d_out_buf, 0, used, tiles, mode, layout, stream, aligned);
+    return launch(units.device.data(), h_units, used, false, d_in, d_out_buf, tiles, mode, layout, stream, aligned);
 }
 
 // A pinned (page-locked, mapped) host buffer has a device alias under UVA: the kernel can then store its output rows
@@ -881,8 +821,8 @@ static float *device_alias_if_pinned(float *host) {
 // host-buffer pipeline (MelPlan::compute_host), printed to stderr after the call.  Off: no events, no cost.
 struct PipelineTrace {
     bool on = false;
-    cudaEvent_t t0 = nullptr;
-    std::vector<cudaEvent_t> ev;
+    Event t0;
+    std::vector<Event> ev;
     std::vector<int> tag;   // unit * 4 + stage (0 H2D done, 1 kernels done, 2 D2H done)
     PipelineTrace() {
         static const bool want = [] { const char *e = std::getenv("FA_MEL_TRACE_PIPELINE"); return e && *e && *e != '0'; }();
@@ -890,15 +830,14 @@ struct PipelineTrace {
     }
     void start(cudaStream_t s) {
         if (!on) return;
-        cudaEventCreate(&t0);
+        t0.create();
         cudaEventRecord(t0, s);
     }
     void mark(cudaStream_t s, int unit, int stage) {
         if (!on) return;
-        cudaEvent_t e;
-        cudaEventCreate(&e);
-        cudaEventRecord(e, s);
-        ev.push_back(e);
+        ev.emplace_back();
+        ev.back().create();
+        cudaEventRecord(ev.back(), s);
         tag.push_back(unit * 4 + stage);
     }
     void dump(const char *what) {
@@ -909,10 +848,8 @@ struct PipelineTrace {
             float ms = 0.0f;
             cudaEventElapsedTime(&ms, t0, ev[i]);
             std::fprintf(stderr, " u%d.%s=%.3f", tag[i] / 4, names[tag[i] & 3], ms);
-            cudaEventDestroy(ev[i]);
         }
         std::fprintf(stderr, "\n");
-        cudaEventDestroy(t0);
     }
 };
 
@@ -945,14 +882,14 @@ static std::vector<long long> unit_bounds(long long T, long long max_units, long
 }
 
 int MelPlan::ensure_resampler(double in_rate, double out_rate) {
-    if (in_rate == out_rate || (in_rate == rs_in && out_rate == rs_out && d_rs_tab)) return FA_OK;
+    if (in_rate == out_rate || (in_rate == rs_in && out_rate == rs_out && d_rs_tab.data())) return FA_OK;
     resample::Design d;
     int st = resample::make_design(in_rate, out_rate, d);
     if (st != FA_OK) return st;
     rs_in = rs_out = 0.0;   // the table is being replaced
-    st = grow_buffer(d_rs_tab, rs_tab_bytes, d.table.size() * sizeof(float));
+    st = d_rs_tab.grow(d.table.size() * sizeof(float));
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpy(d_rs_tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice));
+    FA_CUDA_TRY(cudaMemcpy(d_rs_tab.data(), d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice));
     rs_design = std::move(d);
     rs_in = in_rate;
     rs_out = out_rate;
@@ -985,11 +922,12 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
     if (st != FA_OK) return st;
     const size_t bps = f.format == resample::kPcmI16 ? 2 : 4;
     const size_t pcm_bytes = (size_t)frames * f.channels * bps;
-    char *d_in = reinterpret_cast<char *>(d_audio);   // where the input lands
+    float *const d_f32 = d_audio.data(), *const d_rows = d_out.data();   // kernel input, staged output
+    char *d_in = reinterpret_cast<char *>(d_f32);   // where the input lands
     if (!identity) {
-        st = grow_buffer(d_pcm, d_pcm_bytes, pcm_bytes + 16);
+        st = d_pcm.grow(pcm_bytes + 16);
         if (st != FA_OK) return st;
-        d_in = static_cast<char *>(d_pcm);
+        d_in = static_cast<char *>(d_pcm.data());
     }
     // Units: pipeline_chunks for identity input; converted input keeps ~10 MB of PCM per unit (the copy engines' fixed
     // cost per transfer and the host's enqueue rate make finer units slower there: int16 hour 3.08 ms at 8-12 units,
@@ -1002,15 +940,19 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
     // to overlap, so one stream, no events, the unit descriptor passed in the kernel parameters, one synchronisation.
     const bool single = chunks == 1;
     float *out_alias = (zero_copy_out && layout == 0 && !single) ? device_alias_if_pinned(out) : nullptr;
-    float *k_out = out_alias ? out_alias : d_out;   // where the kernel writes
+    float *k_out = out_alias ? out_alias : d_rows;   // where the kernel writes
     if (out_alias && Tp > T) std::memset(out + T * cfg.n_mels, 0, (size_t)(Tp - T) * cfg.n_mels * sizeof(float));
-    st = ensure_units(chunks);
+    st = units.reserve(unit_bytes(chunks));
     if (st != FA_OK) return st;
     st = ensure_events(2 * (size_t)chunks);
     if (st != FA_OK) return st;
     cudaStream_t s_k = streams[1], s_in = single ? s_k : streams[0], s_out = single ? s_k : streams[2];
+    MelUnit *h_units = units.host.data();
     for (int c = 0; c < chunks; ++c) h_units[c] = MelUnit{0, n, 0, Tp, bounds[c], bounds[c + 1] - bounds[c], last, 0};
-    if (!single) FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, chunks * sizeof(MelUnit), cudaMemcpyHostToDevice, s_k));
+    if (!single) {
+        st = units.upload(chunks * sizeof(MelUnit), s_k);
+        if (st != FA_OK) return st;
+    }
     const long long pad = mode == 0 ? cfg.n_fft / 2 : 0;
     const resample::Design &D = rs_design;
     const bool linear = f.in_rate != f.out_rate && resample::resolve_algorithm(f) == resample::kAlgoLinear;
@@ -1042,7 +984,7 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
             in_copied = in_need;
         }
         // zero the pad rows after the first input copy: a copy from pageable memory first waits for its stream's queue
-        if (c == 0 && Tp > T && !out_alias) FA_CUDA_TRY(cudaMemsetAsync(d_out, 0, need * sizeof(float), s_k));
+        if (c == 0 && Tp > T && !out_alias) FA_CUDA_TRY(cudaMemsetAsync(d_rows, 0, need * sizeof(float), s_k));
         if (!single) {
             FA_CUDA_TRY(cudaEventRecord(events[2 * c], s_in));
             FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * c], 0));
@@ -1054,13 +996,12 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
                 fa::set_error("internal: resampler window accounting (%lld < %lld)", ready, s_end);
                 return FA_RUNTIME_ERROR;
             }
-            st = resample::launch_convert(d_pcm, frames, f, D, d_rs_tab, d_audio, converted, s_end, s_k);
+            st = resample::launch_convert(d_pcm.data(), frames, f, D, d_rs_tab.data(), d_f32, converted, s_end, s_k);
             if (st != FA_OK) return st;
             converted = std::max(converted, s_end);
         }
-        inline_unit = single;
-        st = launch(d_audio, k_out, c, 1, tiles_of(bounds[c + 1] - bounds[c]), mode, layout, s_k, true);
-        inline_unit = false;
+        st = launch(units.device.data() + c, h_units + c, 1, single, d_f32, k_out, tiles_of(bounds[c + 1] - bounds[c]),
+                    mode, layout, s_k, true);
         if (st != FA_OK) return st;
         trace.mark(s_k, c, 1);
         if (out_alias) continue;   // the kernel stored its rows in the caller's pinned buffer: no D2H stage
@@ -1070,10 +1011,10 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
         }
         const long long fb = bounds[c], rows = (tail ? Tp : bounds[c + 1]) - fb;   // the last unit also returns the pad rows
         if (layout == 0 || single) {   // a single unit returns the whole buffer in either layout
-            FA_CUDA_TRY(cudaMemcpyAsync(out + fb * cfg.n_mels, d_out + fb * cfg.n_mels, rows * cfg.n_mels * sizeof(float),
+            FA_CUDA_TRY(cudaMemcpyAsync(out + fb * cfg.n_mels, d_rows + fb * cfg.n_mels, rows * cfg.n_mels * sizeof(float),
                                         cudaMemcpyDeviceToHost, s_out));
         } else {
-            FA_CUDA_TRY(cudaMemcpy2DAsync(out + fb, Tp * sizeof(float), d_out + fb, Tp * sizeof(float),
+            FA_CUDA_TRY(cudaMemcpy2DAsync(out + fb, Tp * sizeof(float), d_rows + fb, Tp * sizeof(float),
                                           rows * sizeof(float), cfg.n_mels, cudaMemcpyDeviceToHost, s_out));
         }
         trace.mark(s_out, c, 2);
@@ -1112,13 +1053,14 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
     dout[count] = o;
     int st = ensure_staging((size_t)a + 8, (size_t)o);
     if (st != FA_OK) return st;
-    st = ensure_units(count);
+    st = units.reserve(unit_bytes(count));
     if (st != FA_OK) return st;
     const int groups = std::min(count, 32);   // one H2D, one launch, one D2H per group: the last group's kernel + D2H is the pipeline's tail
     st = ensure_events(2 * (size_t)groups);
     if (st != FA_OK) return st;
     cudaStream_t s_in = streams[0], s_k = streams[1], s_out = streams[2];
     // all unit descriptors first (one small copy), then per group: H2D, kernel, D2H
+    MelUnit *h_units = units.host.data();
     std::vector<int> g_first(groups + 1), g_units(groups + 1, 0), g_tiles(groups, 0);
     int used = 0;
     for (int g = 0; g < groups; ++g) {
@@ -1134,36 +1076,41 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
         g_tiles[g] = tiles;
     }
     g_first[groups] = used;
-    if (used) FA_CUDA_TRY(cudaMemcpyAsync(d_units, h_units, used * sizeof(MelUnit), cudaMemcpyHostToDevice, s_k));
-    FA_CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)o * sizeof(float), s_k));
+    if (used) {
+        st = units.upload(used * sizeof(MelUnit), s_k);
+        if (st != FA_OK) return st;
+    }
+    float *const d_f32 = d_audio.data(), *const d_rows = d_out.data();
+    FA_CUDA_TRY(cudaMemsetAsync(d_rows, 0, (size_t)o * sizeof(float), s_k));
     for (int g = 0; g < groups; ++g) {
         const int c0 = (int)((long long)count * g / groups), c1 = (int)((long long)count * (g + 1) / groups);
         if (same_layout) {
             const long long n = offsets[c1] - offsets[c0];
             if (n > 0)
-                FA_CUDA_TRY(cudaMemcpyAsync(d_audio + doff[c0], audio + offsets[c0], n * sizeof(float), cudaMemcpyHostToDevice, s_in));
+                FA_CUDA_TRY(cudaMemcpyAsync(d_f32 + doff[c0], audio + offsets[c0], n * sizeof(float), cudaMemcpyHostToDevice, s_in));
         } else {
             for (int i = c0; i < c1; ++i) {
                 const long long n = offsets[i + 1] - offsets[i];
                 if (n > 0)
-                    FA_CUDA_TRY(cudaMemcpyAsync(d_audio + doff[i], audio + offsets[i], n * sizeof(float), cudaMemcpyHostToDevice, s_in));
+                    FA_CUDA_TRY(cudaMemcpyAsync(d_f32 + doff[i], audio + offsets[i], n * sizeof(float), cudaMemcpyHostToDevice, s_in));
             }
         }
         FA_CUDA_TRY(cudaEventRecord(events[2 * g], s_in));
         FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * g], 0));
-        st = launch(d_audio, d_out, g_first[g], g_first[g + 1] - g_first[g], g_tiles[g], mode, layout, s_k, true);
+        st = launch(units.device.data() + g_first[g], h_units + g_first[g], g_first[g + 1] - g_first[g], false, d_f32, d_rows,
+                    g_tiles[g], mode, layout, s_k, true);
         if (st != FA_OK) return st;
         FA_CUDA_TRY(cudaEventRecord(events[2 * g + 1], s_k));
         FA_CUDA_TRY(cudaStreamWaitEvent(s_out, events[2 * g + 1], 0));
         bool out_contiguous = c1 > c0;   // the caller's output offsets follow the packed device layout: one transfer
         for (int i = c0; i < c1 && out_contiguous; ++i) out_contiguous = out_offsets[i] - out_offsets[c0] == dout[i] - dout[c0];
         if (out_contiguous) {
-            FA_CUDA_TRY(cudaMemcpyAsync(out + out_offsets[c0], d_out + dout[c0], (dout[c1] - dout[c0]) * sizeof(float),
+            FA_CUDA_TRY(cudaMemcpyAsync(out + out_offsets[c0], d_rows + dout[c0], (dout[c1] - dout[c0]) * sizeof(float),
                                         cudaMemcpyDeviceToHost, s_out));
         } else {
             for (int i = c0; i < c1; ++i) {
                 const long long len = dout[i + 1] - dout[i];
-                FA_CUDA_TRY(cudaMemcpyAsync(out + out_offsets[i], d_out + dout[i], len * sizeof(float), cudaMemcpyDeviceToHost, s_out));
+                FA_CUDA_TRY(cudaMemcpyAsync(out + out_offsets[i], d_rows + dout[i], len * sizeof(float), cudaMemcpyDeviceToHost, s_out));
             }
         }
     }

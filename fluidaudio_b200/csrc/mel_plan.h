@@ -84,55 +84,40 @@ struct MelPlan {
     int pipeline_chunks = 24;        // units a long host-buffer call is cut into (H2D / kernel / D2H overlap)
     bool zero_copy_out = false;      // time-major output in a pinned host buffer: the kernel stores straight into it
                                      // (opt-in: the staged copy is the default)
-    bool inline_unit = false;        // next launch() passes its (single) unit in the kernel parameters
+    // declared before the buffers, so destroyed after them
+    Stream streams[3];               // h2d, compute, d2h
+    std::vector<Event> events;
+    Event timer[2];                  // fa_mel_timer_*: events on the compute stream
+
     bool generic = false;            // nFFT != 512 or odd hop: mel_generic_kernel (FP64 transform whatever `precision`)
     int generic_warps = 0, generic_prow = 0, generic_log2n = 0;
-    void *d_generic_tw = nullptr;    // FP64 twiddles W_n^k, k < n/2
+    DeviceBuffer<> d_generic_tw;     // FP64 twiddles W_n^k, k < n/2
 
-    void *d_lane_tab[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [window placement][precision]
-    float *d_win_tab_mode[2] = {nullptr, nullptr};
-    uint8_t *d_in_tab_mode[2] = {nullptr, nullptr};
-    float *d_fb_w = nullptr;
-    int *d_fb_lo = nullptr, *d_fb_hi = nullptr, *d_fb_off = nullptr;
-    void *d_fb_slots = nullptr;
+    DeviceBuffer<> d_lane_tab[2][2];   // [window placement][precision]
+    DeviceBuffer<float> d_win_tab_mode[2];
+    DeviceBuffer<uint8_t> d_in_tab_mode[2];
+    DeviceBuffer<float> d_fb_w;
+    DeviceBuffer<int> d_fb_lo, d_fb_hi, d_fb_off;
+    DeviceBuffer<int4> d_fb_slots;
     int n_slots = 0;
 
-    // buffers grown on demand (grow_buffer); the *_bytes members are their capacities
-    MelUnit *d_units = nullptr, *h_units = nullptr;
-    size_t d_units_bytes = 0, h_units_bytes = 0;
-    // recorded after every asynchronous h_units -> d_units copy: ensure_units() waits on it before h_units is rewritten,
-    // so back-to-back device calls never overwrite descriptors whose upload is still queued
-    cudaEvent_t units_uploaded = nullptr;
-    bool units_in_flight = false;
-    float *d_audio = nullptr, *d_out = nullptr;   // staging for the host-buffer entry points
-    size_t d_audio_bytes = 0, d_out_bytes = 0;
+    // buffers grown on demand
+    UploadStage<MelUnit> units;                    // unit descriptors of every launch
+    DeviceBuffer<float> d_audio, d_out;            // staging for the host-buffer entry points
     // AudioConverter stage ahead of the kernel (fa_audio_to_mel): raw PCM staging + the polyphase table of the last ratio
-    void *d_pcm = nullptr;
-    size_t d_pcm_bytes = 0;
+    DeviceBuffer<> d_pcm;
     resample::Design rs_design;
     double rs_in = 0.0, rs_out = 0.0;
-    float *d_rs_tab = nullptr;
-    size_t rs_tab_bytes = 0;
-    cudaStream_t streams[3] = {nullptr, nullptr, nullptr};   // h2d, compute, d2h
-    std::vector<cudaEvent_t> events;
-    cudaEvent_t timer[2] = {nullptr, nullptr};   // fa_mel_timer_*: events on the compute stream
+    DeviceBuffer<float> d_rs_tab;
 
-    ~MelPlan();
-    void release();
     int init(const MelConfig &c);
     long long frame_count(long long n, int mode, long long expected) const;
-    // h_units holds `count` units and may be written (waits for a queued upload of its previous contents)
-    int ensure_units(int count);
-    // queues the copy of h_units[0, count) into d_units on `stream` and records units_uploaded behind it
-    int upload_units(int count, cudaStream_t stream);
     int ensure_staging(size_t audio_floats, size_t out_floats);
     int ensure_events(size_t count);
-    // kernel launch over units [first, first+count) already resident in d_units
-    int launch(const float *d_audio_base, float *d_out_base, int first, int count, int total_tiles, int mode,
-               int layout, cudaStream_t stream, bool aligned16);
-    // the same over `count` units at d_u (device) whose host mirror is h_u (read for the output alignment); never inline
-    int launch_units(const MelUnit *d_u, const MelUnit *h_u, int count, const float *d_audio_base, float *d_out_base,
-                     int total_tiles, int mode, int layout, cudaStream_t stream, bool aligned16);
+    // kernel launch over `count` units at d_u (device) whose host mirror is h_u (read for the output alignment).
+    // inline_unit: a single unit travels in the kernel parameters and d_u is not read.
+    int launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inline_unit, const float *d_audio_base,
+               float *d_out_base, int total_tiles, int mode, int layout, cudaStream_t stream, bool aligned16);
 
     // mode: 0 .center, 1 .prePadded, 2 legacy compute(); layout: 0 time-major, 1 mel-major
     int compute_device(const float *d_in, long long n, float last, int mode, long long expected, int layout,
@@ -162,20 +147,15 @@ struct MelStreamJob;
 struct MelStreamSet {
     int capacity = 0;                    // floats per session in d_carry: round_up4(nFFT/2 + win/2)
     int slots = 0;                       // sessions d_carry / d_last hold
-    float *d_carry = nullptr;            // [slots x capacity]
-    float *d_last = nullptr;             // [slots] lastAudioSample
+    DeviceBuffer<float> d_carry;         // [slots x capacity]
+    DeviceBuffer<float> d_last;          // [slots] lastAudioSample
     std::vector<long long> carry_len, received, emitted;
     std::vector<uint8_t> live, finished;
-    // push staging: descriptors (units, then jobs) in one pinned buffer and its device copy, the pushed samples of a
-    // host push, and the arena the ingest kernel assembles every emitting session's contiguous input in
-    void *h_desc = nullptr, *d_desc = nullptr;
-    size_t h_desc_bytes = 0, d_desc_bytes = 0;
-    float *d_arena = nullptr;
-    size_t d_arena_bytes = 0;
-    cudaEvent_t desc_uploaded = nullptr;   // h_desc may be rewritten once this has completed
-    bool desc_in_flight = false;
+    // push staging: descriptors (units, then jobs) and the arena the ingest kernel assembles every emitting session's
+    // contiguous input in
+    UploadStage<> desc;
+    DeviceBuffer<float> d_arena;
 
-    ~MelStreamSet();
     static int check_config(const MelConfig &c);   // pad_to <= 1 and hop <= win, or FA_INVALID_ARGUMENT
     int open(MelPlan &p, int *session);
     int close(int session);

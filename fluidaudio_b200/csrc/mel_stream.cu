@@ -95,15 +95,6 @@ static void push_frames(const MelConfig &c, long long received, long long emitte
     if (fin && r > 0) second = std::max(0LL, 1 + (r + c.n_fft - c.win_length) / c.hop_length - emitted - first);
 }
 
-MelStreamSet::~MelStreamSet() {
-    if (d_carry) cudaFree(d_carry);
-    if (d_last) cudaFree(d_last);
-    if (d_arena) cudaFree(d_arena);
-    if (d_desc) cudaFree(d_desc);
-    if (h_desc) cudaFreeHost(h_desc);
-    if (desc_uploaded) cudaEventDestroy(desc_uploaded);
-}
-
 int MelStreamSet::check_config(const MelConfig &c) {
     if (c.pad_to > 1) {
         fa::set_error("mel stream: pad_to must be 0 or 1 (an emit returns exactly its frames), got %d", c.pad_to);
@@ -125,32 +116,29 @@ int MelStreamSet::open(MelPlan &p, int *session) {
     int id = 0;
     while (id < slots && live[id]) ++id;   // ids are dense from 0: the lowest closed one is reused
     if (id == slots) {
-        // grow, keeping the live sessions' carries and `last` (queued pushes finish first: same stream)
+        // grow into fresh buffers, keeping the live sessions' carries and `last` (queued pushes finish first: same
+        // stream); a failure leaves the live sessions as they were
         const int grown = std::max(64, 2 * slots);
-        float *c = nullptr, *l = nullptr;
-        cudaError_t e = cudaMalloc(&c, (size_t)grown * capacity * sizeof(float));
-        if (e == cudaSuccess) e = cudaMalloc(&l, (size_t)grown * sizeof(float));
-        if (e != cudaSuccess) {
-            if (c) cudaFree(c);
-            return fa::cuda_failure(e, "cudaMalloc(mel stream state)", __FILE__, __LINE__);
-        }
+        DeviceBuffer<float> c, l;
+        st = c.grow((size_t)grown * capacity * sizeof(float));
+        if (st == FA_OK) st = l.grow((size_t)grown * sizeof(float));
+        if (st != FA_OK) return st;
         if (slots) {
-            FA_CUDA_TRY(cudaMemcpyAsync(c, d_carry, (size_t)slots * capacity * sizeof(float), cudaMemcpyDeviceToDevice, s));
-            FA_CUDA_TRY(cudaMemcpyAsync(l, d_last, (size_t)slots * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            FA_CUDA_TRY(cudaMemcpyAsync(c.data(), d_carry.data(), (size_t)slots * capacity * sizeof(float),
+                                        cudaMemcpyDeviceToDevice, s));
+            FA_CUDA_TRY(cudaMemcpyAsync(l.data(), d_last.data(), (size_t)slots * sizeof(float), cudaMemcpyDeviceToDevice, s));
             FA_CUDA_TRY(cudaStreamSynchronize(s));
-            cudaFree(d_carry);
-            cudaFree(d_last);
         }
-        d_carry = c;
-        d_last = l;
+        d_carry = std::move(c);
+        d_last = std::move(l);
         slots = grown;
         for (auto *v : {&carry_len, &received, &emitted}) v->resize(grown, 0);
         live.resize(grown, 0);
         finished.resize(grown, 0);
     }
     // resetMelStreamLocked (:204-217): the buffer is nFFT/2 zeros, lastAudioSample 0, counters cleared
-    FA_CUDA_TRY(cudaMemsetAsync(d_carry + (size_t)id * capacity, 0, (size_t)half * sizeof(float), s));
-    FA_CUDA_TRY(cudaMemsetAsync(d_last + id, 0, sizeof(float), s));
+    FA_CUDA_TRY(cudaMemsetAsync(d_carry.data() + (size_t)id * capacity, 0, (size_t)half * sizeof(float), s));
+    FA_CUDA_TRY(cudaMemsetAsync(d_last.data() + id, 0, sizeof(float), s));
     carry_len[id] = half;
     received[id] = emitted[id] = 0;
     finished[id] = 0;
@@ -247,25 +235,19 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         return FA_OUTPUT_TOO_SMALL;
     }
 
-    // ---- buffers: h_desc is rewritten only after its previous upload has read it
-    if (desc_in_flight) {
-        FA_CUDA_TRY(cudaEventSynchronize(desc_uploaded));
-        desc_in_flight = false;
-    }
-    if (!desc_uploaded) FA_CUDA_TRY(cudaEventCreateWithFlags(&desc_uploaded, cudaEventDisableTiming));
+    // ---- buffers
     const size_t units_bytes = (((size_t)units * sizeof(MelUnit)) + 15) & ~size_t(15);
     const size_t desc_bytes = units_bytes + (size_t)jobs * sizeof(MelStreamJob);
-    int st = grow_buffer(h_desc, h_desc_bytes, std::max<size_t>(desc_bytes, 4096), true);
-    if (st == FA_OK) st = grow_buffer(d_desc, d_desc_bytes, std::max<size_t>(desc_bytes, 4096));
-    if (st == FA_OK) st = grow_buffer(d_arena, d_arena_bytes, (size_t)std::max(arena, 1024LL) * sizeof(float));
+    int st = desc.reserve(std::max<size_t>(desc_bytes, 4096));
+    if (st == FA_OK) st = d_arena.grow((size_t)std::max(arena, 1024LL) * sizeof(float));
     if (st == FA_OK && !device) st = p.ensure_staging((size_t)std::max(total_new, 0LL) + 8, (size_t)rows * M);
     if (st != FA_OK) return st;
 
-    // ---- descriptors
-    MelUnit *hu = static_cast<MelUnit *>(h_desc);
-    MelStreamJob *hj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(h_desc) + units_bytes);
-    MelUnit *du = static_cast<MelUnit *>(d_desc);
-    MelStreamJob *dj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(d_desc) + units_bytes);
+    // ---- descriptors: units, then jobs
+    MelUnit *hu = static_cast<MelUnit *>(desc.host.data());
+    MelStreamJob *hj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(desc.host.data()) + units_bytes);
+    MelUnit *du = static_cast<MelUnit *>(desc.device.data());
+    MelStreamJob *dj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(desc.device.data()) + units_bytes);
     const long long src0 = device ? 0 : offsets[0];   // a host push's samples land at d_audio[0]
     long long row = 0, a = 0;
     int u = 0, j = 0, tiles = 0;
@@ -302,30 +284,26 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     const float *src = audio;
     if (!device) {
         if (total_new > 0)
-            FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio, audio + offsets[0], (size_t)total_new * sizeof(float),
+            FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio + offsets[0], (size_t)total_new * sizeof(float),
                                         cudaMemcpyHostToDevice, s));
-        src = p.d_audio;
+        src = p.d_audio.data();
     }
     if (desc_bytes) {
-        FA_CUDA_TRY(cudaMemcpyAsync(d_desc, h_desc, desc_bytes, cudaMemcpyHostToDevice, s));
-        FA_CUDA_TRY(cudaEventRecord(desc_uploaded, s));
-        desc_in_flight = true;
+        st = desc.upload(desc_bytes, s);
+        if (st != FA_OK) return st;
     }
     if (jobs) {
-        FA_CUDA_TRY(fa::launch(mel_stream_ingest_kernel, jobs, kIngestThreads, 0, s, dj, src, d_carry, d_last, d_arena, du,
-                               capacity, c.preemph));
+        FA_CUDA_TRY(fa::launch(mel_stream_ingest_kernel, jobs, kIngestThreads, 0, s, dj, src, d_carry.data(), d_last.data(),
+                               d_arena.data(), du, capacity, c.preemph));
     }
-    float *k_out = device ? out : p.d_out;
+    float *k_out = device ? out : p.d_out.data();
     if (units) {
-        // `last` lives in d_units (written by the ingest kernel): the launch must read its units from HBM, never inline
-        const bool saved = p.inline_unit;
-        p.inline_unit = false;
-        st = p.launch_units(du, hu, units, d_arena, k_out, tiles, 1, 0, s, true);
-        p.inline_unit = saved;
+        // `last` lives in the device units (written by the ingest kernel): the launch reads them from HBM, never inline
+        st = p.launch(du, hu, units, false, d_arena.data(), k_out, tiles, 1, 0, s, true);
         if (st != FA_OK) return st;
     }
     if (!device) {
-        if (rows) FA_CUDA_TRY(cudaMemcpyAsync(out, p.d_out, (size_t)rows * M * sizeof(float), cudaMemcpyDeviceToHost, s));
+        if (rows) FA_CUDA_TRY(cudaMemcpyAsync(out, p.d_out.data(), (size_t)rows * M * sizeof(float), cudaMemcpyDeviceToHost, s));
         FA_CUDA_TRY(cudaStreamSynchronize(s));
     }
 

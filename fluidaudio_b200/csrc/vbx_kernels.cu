@@ -761,13 +761,6 @@ __global__ void mean_rows_kernel(const double *__restrict__ src, int rows, int d
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-Workspace::~Workspace() { release(); }
-void Workspace::release() {
-    if (pool) cudaFree(pool);
-    pool = nullptr;
-    pool_bytes = 0;
-}
-
 static size_t fused_smem_bytes(int S, int D) {
     return sizeof(double) * ((size_t)S * D + 2 * (size_t)S + (size_t)kEThreads * S + kEThreads);
 }
@@ -775,7 +768,7 @@ static bool fused_path(int S, int D) { return S <= kFusedMaxS && fused_smem_byte
 
 // d_x: [T x D] device, h_psi: [D] HOST (already identity-substituted by the caller if lengths mismatch),
 // d_init: [T] device labels (or nullptr), d_gamma [T x S], d_pi [S], d_elbos [max(max_it,1)], d_hard [T].
-int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *h_psi, const int *d_init, int S,
+int refine_device(DeviceBuffer<> &pool, const double *d_x, int T, int D, const double *h_psi, const int *d_init, int S,
                   const Config &cfg, double *d_gamma, double *d_pi, double *d_elbos, int *d_hard, int *iterations_host,
                   cudaStream_t stream) {
     if (T <= 0 || D <= 0 || S <= 0) return FA_INVALID_ARGUMENT;
@@ -789,7 +782,7 @@ int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *
     d.eblocks = (T + kEThreads - 1) / kEThreads;
     d.x = d_x;
     double *phi_c = nullptr;
-    int st = carve_arena(ws.pool, ws.pool_bytes, [&](Carver &c) {
+    int st = carve_arena(pool, [&](Carver &c) {
         d.rho = c.take<double>((size_t)T * D);
         d.rhoT = c.take<double>((size_t)D * d.Tp);
         d.G = c.take<double>(T);
@@ -883,12 +876,12 @@ int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *
     return FA_OK;
 }
 
-int centroids_device(Workspace &ws, const double *d_emb, int T, int E, const double *d_gamma, const double *d_pi, int S,
-                     double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream) {
+int centroids_device(DeviceBuffer<> &pool, const double *d_emb, int T, int E, const double *d_gamma, const double *d_pi,
+                     int S, double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream) {
     const int chunks = S <= kFusedMaxS ? (T + kCBlock - 1) / kCBlock : chunks_for(S);
     double *pnum = nullptr, *pden = nullptr;
     int *map = nullptr;
-    int st = carve_arena(ws.pool, ws.pool_bytes, [&](Carver &c) {
+    int st = carve_arena(pool, [&](Carver &c) {
         pnum = c.take<double>((size_t)chunks * S * E);
         pden = c.take<double>((size_t)chunks * S);
         map = c.take<int>(S);

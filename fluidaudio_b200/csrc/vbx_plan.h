@@ -15,19 +15,12 @@ struct Config {
     double init_smoothing = 7.0; // VBxClustering.swift:131
 };
 
-// Scratch arena reused across calls (grown on demand).
-struct Workspace {
-    void *pool = nullptr;
-    size_t pool_bytes = 0;
-    ~Workspace();
-    void release();
-};
-
-int refine_device(Workspace &ws, const double *d_x, int T, int D, const double *h_psi, const int *d_init, int S,
+// `pool`: the scratch arena, reused across calls (grown on demand).
+int refine_device(DeviceBuffer<> &pool, const double *d_x, int T, int D, const double *h_psi, const int *d_init, int S,
                   const Config &cfg, double *d_gamma, double *d_pi, double *d_elbos, int *d_hard, int *iterations_host,
                   cudaStream_t stream);
-int centroids_device(Workspace &ws, const double *d_emb, int T, int E, const double *d_gamma, const double *d_pi, int S,
-                     double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream);
+int centroids_device(DeviceBuffer<> &pool, const double *d_emb, int T, int E, const double *d_gamma, const double *d_pi,
+                     int S, double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream);
 int assign_device(const double *d_emb, int N, int E, const double *d_cent_n, const int *d_count, int K_fixed,
                   int *d_labels, double *d_scores, cudaStream_t stream);
 int onehot_device(const int *d_labels, int T, int S, double *d_gamma, double *d_pi, cudaStream_t stream);
