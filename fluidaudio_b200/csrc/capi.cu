@@ -104,9 +104,9 @@ struct Lease {
     int status = FA_OK;
     explicit Lease(int worker_limit = 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) {
-            set_error("cudaGetDevice failed");
-            status = FA_CUDA_ERROR;
+        const cudaError_t e = cudaGetDevice(&dev);
+        if (e != cudaSuccess) {
+            status = cuda_failure(e, "cudaGetDevice", __FILE__, __LINE__);
             return;
         }
         {
@@ -1334,6 +1334,19 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
     if (!emb256 || !rho || !set_offsets || !cfg || !labels || set_count < 0 || emb_dim == 0 || rho_dim == 0)
         return FA_STATUS_INVALID_ARGUMENT;
     if (set_count == 0) return FA_STATUS_OK;
+    if (set_offsets[0] < 0) {
+        fa::set_error("fa_diarize_cluster_batch: set_offsets[0] = %lld is negative", (long long)set_offsets[0]);
+        return FA_STATUS_INVALID_ARGUMENT;
+    }
+    for (int m = 0; m < set_count; ++m)
+        if (set_offsets[m + 1] < set_offsets[m]) {
+            fa::set_error("fa_diarize_cluster_batch: set_offsets decrease at set %d (%lld -> %lld)", m,
+                          (long long)set_offsets[m], (long long)set_offsets[m + 1]);
+            return FA_STATUS_INVALID_ARGUMENT;
+        }
+    if (infos)   // an empty set is not clustered: its info reads all zeros
+        for (int m = 0; m < set_count; ++m)
+            if (set_offsets[m + 1] == set_offsets[m]) infos[m] = fa_cluster_info{};
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
     int dev = 0;
@@ -1351,8 +1364,10 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
     // Each lane is a plain std::thread: nothing may escape it (an exception leaving a thread function is std::terminate,
     // and FA_GUARD_* only covers the calling thread), so the body is wrapped and failures are reported through status[].
     auto run_lane = [&](int lane) {
-        if (cudaSetDevice(dev) != cudaSuccess) {
-            status[lane] = FA_CUDA_ERROR;
+        const cudaError_t e = cudaSetDevice(dev);
+        if (e != cudaSuccess) {
+            status[lane] = cuda_failure(e, "cudaSetDevice", __FILE__, __LINE__);
+            messages[lane] = fa::last_error();
             return;
         }
         const int st = with_context(worker_limit, [&](ClusterContext &C) {
@@ -1360,7 +1375,7 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
                 const int m = next.fetch_add(1);
                 if (m >= set_count) return (int)FA_OK;
                 const int64_t a = set_offsets[m], b = set_offsets[m + 1];
-                if (b <= a) continue;
+                if (b == a) continue;   // its info was zeroed above
                 const int st = cluster_pipeline(C, emb256 + (size_t)a * emb_dim, rho + (size_t)a * rho_dim, (size_t)(b - a),
                                                 emb_dim, rho_dim, psi, *cfg, labels + a, nullptr, nullptr, 0,
                                                 infos ? infos + m : nullptr, chunk_index ? chunk_index + a : nullptr);

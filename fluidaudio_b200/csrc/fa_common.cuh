@@ -57,8 +57,12 @@ struct CudaStatus {
     int code;
     template <typename T> operator T() const { return static_cast<T>(code); }
 };
+// Reports a failed CUDA call and consumes the runtime's last-error state of this thread.  launch() returns
+// cudaGetLastError(), which also holds the error of any earlier runtime call: without this, a refused cudaMalloc would
+// fail the next, unrelated launch on the thread with the same stale error.  A sticky error is not cleared by this.
 inline CudaStatus cuda_failure(cudaError_t e, const char *expr, const char *file, int line) {
     set_error("%s failed: %s (%s:%d)", expr, cudaGetErrorString(e), file, line);
+    (void)cudaGetLastError();
     return CudaStatus{e == cudaErrorMemoryAllocation ? FA_ALLOCATION_FAILURE : FA_CUDA_ERROR};
 }
 #define FA_CUDA_TRY(expr)                                                                 \

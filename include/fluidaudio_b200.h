@@ -379,7 +379,9 @@ fa_status fa_export_write(const char *path, size_t count, size_t emb_dim, size_t
                           const int32_t *cluster);
 
 /* Many independent embedding sets (meetings) on this GPU.  Set m is rows [set_offsets[m], set_offsets[m+1]).
- * Several sets are clustered concurrently on disjoint SM partitions. */
+ * Several sets are clustered concurrently on disjoint SM partitions.  set_offsets[0] must be >= 0 and the offsets
+ * non-decreasing, else FA_STATUS_INVALID_ARGUMENT before any work.  An empty set (equal offsets) is skipped and its
+ * infos[m] is zeroed; rows outside every set are not written. */
 fa_status fa_diarize_cluster_batch(const float *emb256, const double *rho, const int64_t *set_offsets,
                                    int32_t set_count, size_t emb_dim, size_t rho_dim, const double *psi,
                                    const fa_cluster_config *cfg, int32_t *labels, fa_cluster_info *infos);

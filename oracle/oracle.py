@@ -681,10 +681,12 @@ def speaker_constraints(num_embeddings: int, num_speakers=None, min_speakers=Non
 
 def diarize_cluster(emb256: np.ndarray, rho128: np.ndarray, psi: np.ndarray, threshold=0.6, Fa=0.07, Fb=0.8,
                     max_iterations=20, epsilon=1e-4, use_ref: bool = False, chunk_indices=None, num_speakers=None,
-                    min_speakers=None, max_speakers=None) -> ClusterResult:
+                    min_speakers=None, max_speakers=None, init_smoothing=7.0, initial=None) -> ClusterResult:
     """OfflineDiarizerManager.cluster(_:) lines 286-375.  chunk_indices=None -> plain argmax (:371-374); otherwise
     the reference's default constrained assignment (:357-369) whenever more than one centroid exists and the speaker
-    count was not forced.  num/min/max_speakers: VBxClustering.refineWithConstraints (:685-733)."""
+    count was not forced.  num/min/max_speakers: VBxClustering.refineWithConstraints (:685-733).
+    ``initial`` replaces the AHC labels of the training rows: ``"identity"`` is what AHCClustering returns when the
+    linkage call fails (AHCClustering.swift:52-55), an array is taken as given."""
     emb32 = np.ascontiguousarray(emb256, np.float32)
     feats = emb32.astype(np.float64)                      # :286  Float -> Double
     rho = np.ascontiguousarray(rho128, np.float64)
@@ -693,11 +695,16 @@ def diarize_cluster(emb256: np.ndarray, rho128: np.ndarray, psi: np.ndarray, thr
     if idx.size == 0:
         idx = np.arange(feats.shape[0])
     train, train_rho = feats[idx], rho[idx]
-    if train.shape[0] >= 2:
+    if isinstance(initial, str) and initial == "identity":
+        initial = np.arange(train.shape[0], dtype=np.int32)
+    elif initial is not None:
+        initial = np.ascontiguousarray(initial, np.int32)
+        assert initial.shape == (train.shape[0],)
+    elif train.shape[0] >= 2:
         initial = ahc_cluster(train, threshold, use_ref=use_ref)
     else:
         initial = np.zeros(train.shape[0], np.int32)
-    vbx = vbx_refine(train_rho, psi, initial, Fa, Fb, max_iterations, epsilon)
+    vbx = vbx_refine(train_rho, psi, initial, Fa, Fb, max_iterations, epsilon, init_smoothing)
     adjusted, detected = False, len(set(vbx.hard.tolist())) if vbx.hard.size else 0      # assignedClusterCount
     cents = None
     if (num_speakers is not None or min_speakers is not None or max_speakers is not None) and train_rho.size and initial.size:

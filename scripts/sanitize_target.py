@@ -81,4 +81,15 @@ cl.centroid_linkage(emb.astype(np.float64))
 # rounds per scan thread with the heap alone in shared memory (level 1; two rounds on 131 worker CTAs)
 cl.centroid_linkage(rng.standard_normal((12000, 4)))
 cl.centroid_linkage(rng.standard_normal((16769, 4)))
+# pipeline branches: a non-finite rho row (every E-step row falls back to uniform gamma), AHC refusing D = 7 197
+# (identity labels, one speaker per row), and a batch with empty sets at the start, the middle and the end
+emb, _ = synth.speaker_embeddings(300, 256, 4, seed=10)
+rho, psi = synth.synthetic_plda(emb)
+rho[5, 3] = np.nan
+cl.OfflineClusterer(psi=psi).cluster(emb, rho, chunk_indices=(np.arange(300) // 2).astype(np.int32))
+wide, _ = synth.speaker_embeddings(40, 7197, 3, seed=11)
+cl.OfflineClusterer().cluster(wide, rng.standard_normal((40, 16)))
+emb, _ = synth.speaker_embeddings(900, 256, 4, seed=12)
+rho, psi = synth.synthetic_plda(emb)
+cl.OfflineClusterer(psi=psi).cluster_batch(emb, rho, np.array([0, 0, 300, 300, 600, 900, 900], np.int64))
 print("sanitize target done")
