@@ -103,8 +103,21 @@ __global__ void lseend_scale_cmn_kernel(float *x, long long T, int M, float *mea
     mean_io[m] = mean;
 }
 
+// Both adapters return exactly T rows and size their staging for T; a handle with pad_to > 1 would have the mel kernel
+// write ceil_to(T, pad_to) rows.  The reference builds both extractors with padTo 0, so such a handle is refused up front,
+// before any copy or launch and with the caller's state untouched (as MelStreamSet::check_config does for streams).
+static int check_adapter_config(const MelPlan &p, const char *what) {
+    if (p.cfg.pad_to > 1) {
+        fa::set_error("%s: pad_to must be 0 or 1 (the features hold exactly their frames), got %d", what, p.cfg.pad_to);
+        return FA_INVALID_ARGUMENT;
+    }
+    return FA_OK;
+}
+
 int unified_features(MelPlan &p, const float *window, long long n, long long valid_count, float *out, long long out_len,
                      long long *total_frames, int *valid_frames) {
+    int st = check_adapter_config(p, "unified mel features");
+    if (st != FA_OK) return st;
     const int M = p.cfg.n_mels, hop = p.cfg.hop_length;
     const long long T = n / hop + 1;                                   // UnifiedMelExtractor.swift:30
     const long long valid = std::min<long long>(valid_count / hop, T); // :71
@@ -114,7 +127,7 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
         fa::set_error("unified mel features need %lld floats, buffer has %lld", T * M, out_len);
         return FA_OUTPUT_TOO_SMALL;
     }
-    int st = p.ensure_staging((size_t)n + 16, (size_t)(2 * T * M));
+    st = p.ensure_staging((size_t)n + 16, (size_t)(2 * T * M));
     if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
     float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
@@ -135,6 +148,8 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
 
 int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean, long long *cmn_count, float *out,
                     long long out_len, long long *frames) {
+    int st = check_adapter_config(p, "LS-EEND features");
+    if (st != FA_OK) return st;
     const int M = p.cfg.n_mels;
     const long long T = p.frame_count(n, 1, -1);
     if (frames) *frames = T;
@@ -143,7 +158,7 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
         fa::set_error("LS-EEND features need %lld floats, buffer has %lld", T * M, out_len);
         return FA_OUTPUT_TOO_SMALL;
     }
-    int st = p.ensure_staging((size_t)n + 16, (size_t)(T * M + M));
+    st = p.ensure_staging((size_t)n + 16, (size_t)(T * M + M));
     if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
     float *d_flat = p.d_out.data(), *d_mean = d_flat + T * M;

@@ -190,7 +190,9 @@ fa_status fa_mel_timer_stop_ms(fa_mel *mel, float *elapsed_ms);
  *   per-feature-normalised log-mel packed [n_mels x total_frames] (the MLMultiArray [1, nMels, T]).
  * fa_mel_lseend_features = LSEENDPreprocessor.processAudioQueue (Diarizer/LS-EEND/LSEENDPreprocessor.swift:249-283):
  *   the handle configured as :70-81 (preemph 0, periodic Hann, clamped floor 1e-10); out receives [frames x n_mels]
- *   log10-scaled, cumulative-mean-normalised features; cmn_mean[n_mels] / cmn_count are the running state, updated. */
+ *   log10-scaled, cumulative-mean-normalised features; cmn_mean[n_mels] / cmn_count are the running state, updated.
+ * Both return exactly their frames, so both need a handle with pad_to 0 or 1 (the reference's padTo: 0); any other
+ * pad_to gives FA_STATUS_INVALID_ARGUMENT before any copy or launch, with cmn_mean / cmn_count untouched. */
 fa_status fa_mel_unified_features(fa_mel *mel, const float *window, size_t window_samples, size_t valid_count,
                                   float *out, size_t out_len, int64_t *total_frames, int32_t *valid_frames);
 fa_status fa_mel_lseend_features(fa_mel *mel, const float *chunk, size_t n, float *cmn_mean, int64_t *cmn_count,

@@ -217,14 +217,20 @@ def normalize_per_feature(x: np.ndarray, valid_frames: int) -> np.ndarray:
     return y
 
 
-def unified_mel_features(window: np.ndarray, valid_count: int, n_mels: int = 128, hop: int = 160):
+def unified_mel_features(window: np.ndarray, valid_count: int, n_mels: int = 128, hop: int = 160,
+                         cfg: MelConfig | None = None):
     """UnifiedMelExtractor.features(window:validCount:) (UnifiedMelExtractor.swift:52-86): center-padded log-mel with
     expectedFrameCount = windowSamples / hop + 1, NeMo per-feature normalisation over validCount / hop frames, packed as
-    [nMels x totalFrames].  Returns (mel [n_mels x T], valid_frames)."""
+    [nMels x totalFrames].  ``cfg`` (a full MelConfig) replaces the extractor's own configuration, ``n_mels`` and
+    ``hop`` with it.  Returns (mel [n_mels x T], valid_frames)."""
     window = np.ascontiguousarray(window, np.float32)
+    if cfg is None:
+        cfg = mel_config(n_mels=n_mels)
+    else:
+        hop = cfg.hop_length
     total = window.size // hop + 1
-    cfg = mel_config(n_mels=n_mels)
     flat, _, _ = mel_flat_transposed(cfg, window, 0.0, 0, expected_frames=total)
+    flat = flat.reshape(-1, cfg.n_mels)        # an empty window gives the guard's one flat row of zeros
     valid = min(int(valid_count) // hop, total)
     norm = normalize_per_feature(flat[:total], valid)
     return np.ascontiguousarray(norm.T), valid
@@ -240,8 +246,14 @@ def lseend_features(cfg: MelConfig, chunk: np.ndarray, cmn_mean: np.ndarray, cmn
     """LSEENDPreprocessor.processAudioQueue (:249-283): .prePadded log-mel, log10 scaling, cumulative mean
     normalisation.  Returns (features [T x nMels], cmn_mean', cmn_count')."""
     flat, ml, _ = mel_flat_transposed(cfg, np.ascontiguousarray(chunk, np.float32), 0.0, 1, None)
-    x = np.ascontiguousarray(flat[:ml], np.float32).copy()
+    return lseend_scale_cmn(flat[:ml], cmn_mean, cmn_count)
+
+
+def lseend_scale_cmn(x: np.ndarray, cmn_mean: np.ndarray, cmn_count: int):
+    """The post-processing half of ``lseend_features`` on a given [T x nMels] log-mel: log10 scaling and cumulative mean
+    normalisation from (cmn_mean, cmn_count).  Returns (features [T x nMels], cmn_mean', cmn_count')."""
     mean = np.ascontiguousarray(cmn_mean, np.float32).copy()
+    x = np.ascontiguousarray(x, np.float32).reshape(-1, mean.size).copy()
     cnt = C.c_int64(int(cmn_count))
     lib().oracle_lseend_scale_cmn(x, x.shape[0], x.shape[1], mean, C.byref(cnt))
     return x, mean, cnt.value

@@ -4,7 +4,8 @@ import numpy as np
 sys.path.insert(0, ".")
 from fluidaudio_b200 import synth, clustering as cl
 import os
-from fluidaudio_b200.mel import AudioMelSpectrogram, LSEENDMelFrontend, UnifiedMelExtractor, PaddingMode, Precision
+from fluidaudio_b200.mel import (AudioMelSpectrogram, LSEENDMelFrontend, UnifiedMelExtractor, PaddingMode, Precision,
+                                 normalize_per_feature)
 from fluidaudio_b200.audio_converter import AudioConverter
 
 a = synth.tone_noise_audio(16000 * 3 + 77)
@@ -43,6 +44,11 @@ m.compute_from_pcm(np.ascontiguousarray(np.round(st.T * 32767).astype(np.int16))
 m.compute_from_pcm(np.round(st[0] * 32767).astype(np.int16)[:16000], 16000)
 UnifiedMelExtractor(24000).features(np.concatenate([a[:20000], np.zeros(4000, np.float32)]), 20000)
 LSEENDMelFrontend().process(a[:16000])
+# adapters: a partial last 128-bin CTA and a partial last 32-frame tile with one valid frame, LS-EEND on the 8 kHz model's
+# configuration (nFFT 256, the any-nFFT kernel), the standalone normalisation across two CTAs
+UnifiedMelExtractor(50 * 160 + 37, n_mels=257).features(a[:50 * 160 + 37], 160)
+LSEENDMelFrontend(n_fft=256, hop_length=80, win_length=200, sample_rate=8000).process(a[:8000])
+normalize_per_feature(np.random.default_rng(0).normal(size=(45, 129)).astype(np.float32), 40)
 for n in (2, 3, 50, 400):
     emb, _ = synth.speaker_embeddings(n, 256, 4, seed=n)
     rho, psi = synth.synthetic_plda(emb)
