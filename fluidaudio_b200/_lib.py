@@ -35,6 +35,12 @@ class MelConfig(C.Structure):
                 ("log_floor_mode", C.c_int32), ("window_periodic", C.c_int32)]
 
 
+class MelExConfig(C.Structure):
+    _fields_ = [("base", MelConfig), ("filterbank", C.c_int32), ("filter_sample_rate", C.c_int32), ("f_min", C.c_float),
+                ("f_max", C.c_float), ("center_edge", C.c_int32), ("spectrum_power", C.c_float),
+                ("log_mean", C.c_float), ("log_std", C.c_float)]
+
+
 class AudioFormat(C.Structure):
     _fields_ = [("in_rate", C.c_double), ("out_rate", C.c_double), ("channels", C.c_int32), ("format", C.c_int32),
                 ("interleaved", C.c_int32), ("algorithm", C.c_int32)]
@@ -71,6 +77,8 @@ EXPORTED_SYMBOLS = [
     "fa_mel_destroy", "fa_mel_get_window", "fa_mel_get_filterbank", "fa_mel_frame_count", "fa_mel_compute",
     "fa_mel_compute_device", "fa_mel_compute_batch", "fa_mel_compute_batch_device", "fa_mel_timer_start",
     "fa_mel_timer_stop_ms", "fa_mel_set_precision", "fa_mel_get_precision", "fa_mel_set_pipeline_chunks", "fa_mel_set_zero_copy_output", "fa_mel_normalize_per_feature", "fa_mel_unified_features", "fa_mel_lseend_features",
+    "fa_mel_ex_default_config", "fa_mel_preset_cohere", "fa_mel_preset_styletts2", "fa_mel_preset_luxtts",
+    "fa_mel_create_ex", "fa_mel_cohere_features", "fa_mel_styletts2_features", "fa_mel_luxtts_features",
     "fa_mel_stream_open", "fa_mel_stream_close", "fa_mel_stream_frames", "fa_mel_stream_push", "fa_mel_stream_push_device",
     "fa_resample_output_count", "fa_audio_resample", "fa_audio_to_mel",
     "fa_linear_resample", "fa_l2_normalize_rows", "fa_ahc_cluster", "fa_dendrogram_cut", "fa_vbx_default_config",
@@ -112,6 +120,13 @@ def load():
     L.fa_mel_default_config.argtypes = [C.POINTER(MelConfig)]
     L.fa_mel_default_config.restype = None
     L.fa_mel_create.argtypes = [C.POINTER(MelConfig), C.POINTER(vp)]
+    for name in ("fa_mel_ex_default_config", "fa_mel_preset_cohere", "fa_mel_preset_styletts2", "fa_mel_preset_luxtts"):
+        getattr(L, name).argtypes = [C.POINTER(MelExConfig)]
+        getattr(L, name).restype = None
+    L.fa_mel_create_ex.argtypes = [C.POINTER(MelExConfig), C.POINTER(vp)]
+    L.fa_mel_cohere_features.argtypes = [vp, vp, sz, i64, vp, sz, C.POINTER(i64), C.POINTER(i64)]
+    L.fa_mel_styletts2_features.argtypes = [vp, vp, sz, vp, sz, C.POINTER(i64)]
+    L.fa_mel_luxtts_features.argtypes = [vp, vp, sz, vp, sz, C.POINTER(i64)]
     L.fa_mel_destroy.argtypes = [vp]
     L.fa_mel_destroy.restype = None
     L.fa_mel_get_window.argtypes = [vp, vp, sz]

@@ -560,20 +560,117 @@ FA_API void fa_mel_default_config(fa_mel_config *cfg) {
     cfg->window_periodic = 0;
 }
 
-FA_API fa_status fa_mel_create(const fa_mel_config *cfg, fa_mel **out) {
-    if (!cfg || !out) return FA_STATUS_INVALID_ARGUMENT;
-    *out = nullptr;
+static mel::MelConfig mel_config_of(const fa_mel_config *cfg) {
+    return mel::MelConfig{cfg->sample_rate, cfg->n_mels,  cfg->n_fft,     cfg->hop_length,     cfg->win_length,
+                          cfg->preemph,     cfg->pad_to,  cfg->log_floor, cfg->log_floor_mode, cfg->window_periodic};
+}
+
+static fa_status create_mel(const mel::MelConfig &c, fa_mel **out) {
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
     std::unique_ptr<MelHandle> h(new MelHandle());
-    mel::MelConfig c{cfg->sample_rate, cfg->n_mels, cfg->n_fft, cfg->hop_length, cfg->win_length, cfg->preemph,
-                     cfg->pad_to, cfg->log_floor, cfg->log_floor_mode, cfg->window_periodic};
     FA_CUDA_TRY(cudaGetDevice(&h->device));
     const int st = h->plan.init(c);
     if (st != FA_OK) return (fa_status)st;
     *out = reinterpret_cast<fa_mel *>(h.release());
     return FA_STATUS_OK;
     FA_GUARD_END
+}
+
+FA_API fa_status fa_mel_create(const fa_mel_config *cfg, fa_mel **out) {
+    if (!cfg || !out) return FA_STATUS_INVALID_ARGUMENT;
+    *out = nullptr;
+    return create_mel(mel_config_of(cfg), out);
+}
+
+FA_API void fa_mel_ex_default_config(fa_mel_ex_config *cfg) {
+    if (!cfg) return;
+    fa_mel_default_config(&cfg->base);
+    cfg->filterbank = FA_MEL_FB_AUDIO_MEL;
+    cfg->filter_sample_rate = 0;
+    cfg->f_min = 0.0f;
+    cfg->f_max = 0.0f;
+    cfg->center_edge = FA_MEL_EDGE_ZERO;
+    cfg->spectrum_power = 2.0f;
+    cfg->log_mean = 0.0f;
+    cfg->log_std = 1.0f;
+}
+
+// CohereMelSpectrogram.Config() (CoherePipeline.swift:55-77) with CohereAsrConfig.MelSpec: nFFT = nextPow2(winLength)
+FA_API void fa_mel_preset_cohere(fa_mel_ex_config *cfg) {
+    if (!cfg) return;
+    fa_mel_ex_default_config(cfg);
+    fa_mel_config &b = cfg->base;
+    b.sample_rate = 16000;
+    b.win_length = 400;
+    b.hop_length = 160;
+    b.n_mels = 128;
+    b.n_fft = 1;
+    while (b.n_fft < b.win_length) b.n_fft <<= 1;   // nextPowerOfTwo(atLeast:) (:265-269): 512
+    b.preemph = 0.97f;
+    b.log_floor = 5.9604645e-08f;   // logZeroGuard 2^-24, additive
+    b.log_floor_mode = 0;
+    b.window_periodic = 0;
+    cfg->filterbank = FA_MEL_FB_COHERE;
+    cfg->f_min = 0.0f;
+    cfg->f_max = 8000.0f;
+}
+
+// StyleTTS2Constants (StyleTTS2Constants.swift:13, :43-52): 24 kHz audio, the table built for 16 kHz
+FA_API void fa_mel_preset_styletts2(fa_mel_ex_config *cfg) {
+    if (!cfg) return;
+    fa_mel_ex_default_config(cfg);
+    fa_mel_config &b = cfg->base;
+    b.sample_rate = 24000;
+    b.n_fft = 2048;
+    b.win_length = 1200;
+    b.hop_length = 300;
+    b.n_mels = 80;
+    b.preemph = 0.0f;
+    b.log_floor = 1e-5f;
+    b.log_floor_mode = 0;
+    b.window_periodic = 1;
+    cfg->filterbank = FA_MEL_FB_STYLETTS2;
+    cfg->filter_sample_rate = 16000;
+    cfg->center_edge = FA_MEL_EDGE_REFLECT;
+    cfg->log_mean = -4.0f;
+    cfg->log_std = 4.0f;
+}
+
+// LuxTtsConstants (LuxTtsConstants.swift:11-21): torchaudio MelSpectrogram(24000, 1024, hop 256, 100 mels, power 1)
+FA_API void fa_mel_preset_luxtts(fa_mel_ex_config *cfg) {
+    if (!cfg) return;
+    fa_mel_ex_default_config(cfg);
+    fa_mel_config &b = cfg->base;
+    b.sample_rate = 24000;
+    b.n_fft = 1024;
+    b.win_length = 1024;
+    b.hop_length = 256;
+    b.n_mels = 100;
+    b.preemph = 0.0f;
+    b.log_floor = 1e-7f;
+    b.log_floor_mode = 1;
+    b.window_periodic = 1;
+    cfg->filterbank = FA_MEL_FB_LUXTTS;
+    cfg->center_edge = FA_MEL_EDGE_REFLECT;
+    cfg->spectrum_power = 1.0f;
+}
+
+FA_API fa_status fa_mel_create_ex(const fa_mel_ex_config *cfg, fa_mel **out) {
+    if (!cfg || !out) return FA_STATUS_INVALID_ARGUMENT;
+    *out = nullptr;
+    mel::MelConfig c = mel_config_of(&cfg->base);
+    c.fb_kind = cfg->filterbank;
+    c.filter_sample_rate = cfg->filter_sample_rate;
+    c.f_min = cfg->f_min;
+    c.f_max = cfg->f_max;
+    c.center_edge = cfg->center_edge;
+    c.spectrum_power = cfg->spectrum_power;
+    c.log_mean = cfg->log_mean;
+    c.log_std = cfg->log_std;
+    const int st = mel::check_ex_config(c);   // before the device is touched
+    if (st != FA_OK) return (fa_status)st;
+    return create_mel(c, out);
 }
 
 FA_API void fa_mel_destroy(fa_mel *mel) { delete reinterpret_cast<MelHandle *>(mel); }
@@ -788,6 +885,45 @@ FA_API fa_status fa_mel_lseend_features(fa_mel *mel, const float *chunk, size_t 
     long long T = 0, count = *cmn_count;
     const int st = fa::mel::lseend_features(h->plan, chunk, (long long)n, cmn_mean, &count, out, (long long)out_len, &T);
     *cmn_count = count;
+    if (frames) *frames = T;
+    return (fa_status)st;
+    FA_GUARD_END
+}
+
+// CohereMelSpectrogram.compute + padOrTruncate (CoherePipeline.swift:127-263), StyleTTS2MelExtractor.compute
+// (StyleTTS2MelExtractor.swift:77-141), LuxTtsMelExtractor.extract (LuxTtsMelExtractor.swift:52-132): mel_adapters.cu.
+FA_API fa_status fa_mel_cohere_features(fa_mel *mel, const float *audio, size_t n, int64_t fixed_frames, float *out,
+                                        size_t out_len, int64_t *frames, int64_t *valid_frames) {
+    if (!mel || !out || (!audio && n)) return FA_STATUS_INVALID_ARGUMENT;
+    FA_GUARD_BEGIN
+    long long W = 0, valid = 0;
+    const int st = fa::mel::cohere_features(reinterpret_cast<MelHandle *>(mel)->plan, audio, (long long)n,
+                                            (long long)fixed_frames, out, (long long)out_len, &W, &valid);
+    if (frames) *frames = W;
+    if (valid_frames) *valid_frames = valid;
+    return (fa_status)st;
+    FA_GUARD_END
+}
+
+FA_API fa_status fa_mel_styletts2_features(fa_mel *mel, const float *audio, size_t n, float *out, size_t out_len,
+                                           int64_t *frames) {
+    if (!mel || !out || (!audio && n)) return FA_STATUS_INVALID_ARGUMENT;
+    FA_GUARD_BEGIN
+    long long T = 0;
+    const int st = fa::mel::styletts2_features(reinterpret_cast<MelHandle *>(mel)->plan, audio, (long long)n, out,
+                                               (long long)out_len, &T);
+    if (frames) *frames = T;
+    return (fa_status)st;
+    FA_GUARD_END
+}
+
+FA_API fa_status fa_mel_luxtts_features(fa_mel *mel, const float *audio, size_t n, float *out, size_t out_len,
+                                        int64_t *frames) {
+    if (!mel || (!out && out_len) || (!audio && n)) return FA_STATUS_INVALID_ARGUMENT;
+    FA_GUARD_BEGIN
+    long long T = 0;
+    const int st = fa::mel::luxtts_features(reinterpret_cast<MelHandle *>(mel)->plan, audio, (long long)n, out,
+                                            (long long)out_len, &T);
     if (frames) *frames = T;
     return (fa_status)st;
     FA_GUARD_END

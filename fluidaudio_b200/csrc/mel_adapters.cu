@@ -107,6 +107,10 @@ __global__ void lseend_scale_cmn_kernel(float *x, long long T, int M, float *mea
 // write ceil_to(T, pad_to) rows.  The reference builds both extractors with padTo 0, so such a handle is refused up front,
 // before any copy or launch and with the caller's state untouched (as MelStreamSet::check_config does for streams).
 static int check_adapter_config(const MelPlan &p, const char *what) {
+    if (!p.cfg.neutral()) {   // both restate NeMo-flavoured AudioMelSpectrogram callers
+        fa::set_error("%s: needs an AudioMelSpectrogram handle, not one with fa_mel_ex_config fields set", what);
+        return FA_INVALID_ARGUMENT;
+    }
     if (p.cfg.pad_to > 1) {
         fa::set_error("%s: pad_to must be 0 or 1 (the features hold exactly their frames), got %d", what, p.cfg.pad_to);
         return FA_INVALID_ARGUMENT;
@@ -174,6 +178,131 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     *cmn_count += T;
     return FA_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ torch-style frontends
+// CohereMelSpectrogram.compute's CMVN and padOrTruncate (CoherePipeline.swift:220-263).  x: the log-mel, time-major
+// [T x M] with T > valid; out: mel-major [M x W].  When valid > 1 every mel bin is normalised with the mean and the
+// unbiased std (a non-finite std counts as 0) of ALL its valid frames, even those past W: padOrTruncate runs after
+// compute.  Frames >= valid are zero, and so are the pad columns up to W.
+__global__ void __launch_bounds__(kBinsPerCta) cohere_cmvn_kernel(const float *__restrict__ x, int M, long long valid,
+                                                                  long long W, float eps, float *__restrict__ out) {
+    __shared__ float tile[kBinsPerCta][kTile + 1];
+    const int m0 = blockIdx.x * kBinsPerCta, m = m0 + threadIdx.x;
+    const bool live = m < M, cmvn = valid > 1;
+    float mean = 0.0f, denom = 1.0f;
+    if (live && cmvn) {
+        for (long long t = 0; t < valid; ++t) mean = __fadd_rn(mean, x[t * M + m]);
+        mean = __fdiv_rn(mean, (float)valid);
+        float ssq = 0.0f;
+        for (long long t = 0; t < valid; ++t) {
+            const float d = __fsub_rn(x[t * M + m], mean);
+            ssq = __fadd_rn(ssq, __fmul_rn(d, d));
+        }
+        float sd = __fsqrt_rn(__fdiv_rn(ssq, (float)(valid - 1)));
+        if (!isfinite(sd)) sd = 0.0f;
+        denom = __fadd_rn(sd, eps);
+    }
+    const long long keep = valid < W ? valid : W;
+    const int rows = min(kBinsPerCta, M - m0);
+    for (long long t0 = 0; t0 < W; t0 += kTile) {
+        const int nt = (int)min((long long)kTile, W - t0);
+        if (live)
+            for (int i = 0; i < nt; ++i) {
+                const long long t = t0 + i;
+                float v = 0.0f;
+                if (t < keep) v = cmvn ? __fdiv_rn(__fsub_rn(x[t * M + m], mean), denom) : x[t * M + m];
+                tile[threadIdx.x][i] = v;
+            }
+        __syncthreads();
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        for (int r = warp; r < rows; r += kBinsPerCta / 32)
+            if (lane < nt) out[(long long)(m0 + r) * W + t0 + lane] = tile[r][lane];
+        __syncthreads();
+    }
+}
+
+// Does the handle restate the class?  Filterbank kind, edge, spectrum and log mode, and exactly T rows (pad_to <= 1).
+static int check_class(const MelPlan &p, const char *what, int fb_kind, int edge, float power, int log_mode) {
+    const MelConfig &c = p.cfg;
+    const bool any_power = power < 0.0f;   // CohereMelSpectrogram.Config.magPower is a parameter
+    if (c.fb_kind != fb_kind || c.center_edge != edge || (!any_power && c.spectrum_power != power) ||
+        c.log_floor_mode != log_mode || c.pad_to > 1 || (fb_kind == 1 && c.affine())) {
+        fa::set_error("%s: the handle is not configured as its reference class (see its fa_mel_preset_*)", what);
+        return FA_INVALID_ARGUMENT;
+    }
+    return FA_OK;
+}
+
+static int check_out(const char *what, long long need, long long out_len) {
+    if (out_len < need) {
+        fa::set_error("%s need %lld floats, buffer has %lld", what, need, out_len);
+        return FA_OUTPUT_TOO_SMALL;
+    }
+    return FA_OK;
+}
+
+int cohere_features(MelPlan &p, const float *audio, long long n, long long fixed_frames, float *out, long long out_len,
+                    long long *frames, long long *valid_frames) {
+    const char *what = "Cohere mel features";
+    int st = check_class(p, what, 1, 0, -1.0f, 0);
+    if (st != FA_OK) return st;
+    const int M = p.cfg.n_mels, hop = p.cfg.hop_length;
+    const long long T = 1 + n / hop, valid = n / hop;   // padded.count = n + nFFT: 1 + n / hop frames (:146), :120
+    const long long W = fixed_frames < 0 ? T : fixed_frames;
+    if (frames) *frames = W;
+    if (valid_frames) *valid_frames = std::min(valid, W);
+    st = check_out(what, W * M, out_len);
+    if (st != FA_OK) return st;
+    st = p.ensure_staging((size_t)n + 16, (size_t)((T + W) * M));
+    if (st != FA_OK) return st;
+    cudaStream_t s = p.streams[1];
+    float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
+    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    st = p.launch_clip(p.d_audio.data(), n, T, 0, d_flat, s);
+    if (st != FA_OK) return st;
+    FA_CUDA_TRY(fa::launch(cohere_cmvn_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, s, d_flat, M, valid, W,
+                           1.0e-5f, d_pack));   // Config.cmvnEpsilon
+    if (W) FA_CUDA_TRY(cudaMemcpyAsync(out, d_pack, sizeof(float) * W * M, cudaMemcpyDeviceToHost, s));
+    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    return FA_OK;
+}
+
+// host clip in, one launch of T frames in `layout`, rows out
+static int run_clip(MelPlan &p, const float *audio, long long n, long long T, int layout, float *out) {
+    const long long need = T * p.cfg.n_mels;
+    int st = p.ensure_staging((size_t)n + 16, (size_t)need);
+    if (st != FA_OK) return st;
+    cudaStream_t s = p.streams[1];
+    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    st = p.launch_clip(p.d_audio.data(), n, T, layout, p.d_out.data(), s);
+    if (st != FA_OK) return st;
+    FA_CUDA_TRY(cudaMemcpyAsync(out, p.d_out.data(), sizeof(float) * need, cudaMemcpyDeviceToHost, s));
+    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    return FA_OK;
+}
+
+int styletts2_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames) {
+    const char *what = "StyleTTS2 mel features";
+    int st = check_class(p, what, 2, 1, 2.0f, 0);
+    if (st != FA_OK) return st;
+    const long long T = 1 + n / p.cfg.hop_length;   // reflectPad keeps n + nFFT samples, an empty clip nFFT zeros (:78-87)
+    if (frames) *frames = T;
+    st = check_out(what, T * p.cfg.n_mels, out_len);
+    return st != FA_OK ? st : run_clip(p, audio, n, T, 1, out);
+}
+
+int luxtts_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames) {
+    const char *what = "LuxTTS mel features";
+    int st = check_class(p, what, 3, 1, 1.0f, 1);
+    if (st != FA_OK) return st;
+    // lhotse's count (:44-47).  It never exceeds the STFT's 1 + n / hop (:67), so the reference's replicate-last-frame
+    // branch (:126-130) is never taken and the frames are the first T STFT frames.
+    const long long hop = p.cfg.hop_length, T = n > 0 ? (n + hop / 2) / hop : 0;
+    if (frames) *frames = T;
+    if (T == 0) return FA_OK;
+    st = check_out(what, T * p.cfg.n_mels, out_len);
+    return st != FA_OK ? st : run_clip(p, audio, n, T, 0, out);
 }
 
 } // namespace mel

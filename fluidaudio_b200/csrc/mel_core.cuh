@@ -576,5 +576,16 @@ FA_HD float preemph_first(float x0, float last, float a) {
 }
 FA_HD float preemph_rest(float x, float xprev, float a) { return fmaf(xprev, -a, x); }
 
+// Reflect padding of a clip of n >= 1 samples (FA_MEL_EDGE_REFLECT): the sample index audio index i reads.  These are
+// the reference's clamps (StyleTTS2MelExtractor.swift:226-250, LuxTtsMelExtractor.swift:57-64), not torch's rule:
+// i < 0 reads x[min(-i, n-1)], i >= n reads x[max(2n-2-i, 0)], so a clip shorter than the pad repeats its end samples
+// instead of failing.  [a,b,c,d] padded by 2 reads [c,b,a,b,c,d,c,b].  The any-nFFT kernel and the CPU emulation
+// (tests/emul/mel_reflect_emul.cpp) share this function.
+FA_HD long long reflect_index(long long i, long long n) {
+    if (i < 0) return -i < n - 1 ? -i : n - 1;
+    if (i >= n) return 2 * n - 2 - i > 0 ? 2 * n - 2 - i : 0;
+    return i;
+}
+
 } // namespace mel
 } // namespace fa

@@ -335,12 +335,21 @@ __global__ void __launch_bounds__(kWarps * 32, 2) mel512_kernel(const MelLaunch 
 // unit / tile bookkeeping and the same packed filterbank as mel512_kernel; one warp per frame, the transform an FP64
 // radix-2 decimation-in-time FFT of the real frame in shared memory (twiddles from an FP64 table), power rounded once
 // to float32.  A correctness-first path: ~6x the instructions per frame of the specialised kernel.
+// The torch-style frontends (fa_mel_create_ex) also run here, as three compile-time variants; <false, kSpecPower, false>
+// is AudioMelSpectrogram's kernel:
+//   kReflect   .center reads reflect_index(i, n) (mel_core.cuh) instead of zeros outside the clip; no pre-emphasis;
+//   kSpectrum  kSpecPower: the tile holds 4|X|^2 and the weights 1/4 of the table; kSpecMagnitude: sqrt of the float32
+//              power (rounded once from the FP64 transform), kSpecGeneral: powf(|X|, p); both with unscaled weights;
+//   kAffine    out = (log - log_mean) / log_std, two rounded float32 operations as the Swift states them.
 struct GenericParams {
     int n_fft, log2n, bins, prow;      // prow: floats per power row (bins rounded up to quads + 4)
     const cpxd *tw;                    // W_n^k, k < n/2
     int warps;
+    float spectrum_power;              // kSpecGeneral: p
+    float log_mean, log_std;           // kAffine
 };
 
+template <bool kReflect, int kSpectrum, bool kAffine>
 __global__ void __launch_bounds__(256) mel_generic_kernel(const MelLaunch P, const GenericParams G) {
     extern __shared__ __align__(16) unsigned char smem[];
     cpxd *tw = reinterpret_cast<cpxd *>(smem);                                   // n/2
@@ -366,7 +375,9 @@ __global__ void __launch_bounds__(256) mel_generic_kernel(const MelLaunch P, con
             for (int j = lane; j < G.n_fft; j += 32) {
                 const long long i = base + j;
                 float v = 0.0f;
-                if (i >= 0 && i < u.n && P.in_tab[j]) {
+                if (kReflect) {
+                    if (u.n > 0 && P.in_tab[j]) v = __fmul_rn(__ldg(x + reflect_index(i, u.n)), win[j]);
+                } else if (i >= 0 && i < u.n && P.in_tab[j]) {
                     const float xi = __ldg(x + i);
                     if (a == 0.0f) v = xi;
                     else if (i == 0) v = preemph_first(xi, u.last, a);
@@ -398,14 +409,18 @@ __global__ void __launch_bounds__(256) mel_generic_kernel(const MelLaunch P, con
             }
             for (int b = lane; b < G.bins; b += 32) {
                 const float xr = (float)buf[b].x, xi = (float)buf[b].y;
-                prow[b] = 4.0f * __fadd_rn(__fmul_rn(xr, xr), __fmul_rn(xi, xi));   // the packed weights carry 1/4
+                const float pw = __fadd_rn(__fmul_rn(xr, xr), __fmul_rn(xi, xi));
+                if (kSpectrum == kSpecPower) prow[b] = 4.0f * pw;   // the packed weights carry 1/4
+                else if (kSpectrum == kSpecMagnitude) prow[b] = __fsqrt_rn(pw);
+                else prow[b] = powf(__fsqrt_rn(pw), G.spectrum_power);   // CohereMelSpectrogram's pow(mag, magPower)
             }
             __syncwarp();
             for (int m = lane; m < P.n_mels; m += 32) {
                 const int lo = P.fb_lo[m], nq = (P.fb_hi[m] - lo) >> 2;
-                const float v = log_value(mel_dot_quads(reinterpret_cast<const float4 *>(prow + lo),
-                                                        reinterpret_cast<const float4 *>(P.fb_w + P.fb_off[m]), nq),
-                                          P.log_floor, P.log_clamped);
+                float v = log_value(mel_dot_quads(reinterpret_cast<const float4 *>(prow + lo),
+                                                  reinterpret_cast<const float4 *>(P.fb_w + P.fb_off[m]), nq),
+                                    P.log_floor, P.log_clamped);
+                if (kAffine) v = __fdiv_rn(__fsub_rn(v, G.log_mean), G.log_std);
                 if (P.layout == 0) P.out[u.out_off + f * P.n_mels + m] = v;
                 else P.out[u.out_off + (long long)m * u.out_stride + f] = v;
             }
@@ -459,8 +474,128 @@ void build_filterbank(int n_fft, int n_mels, int sample_rate, std::vector<float>
     }
 }
 
+// Swift's min / max on Comparable: min(x, y) = y < x ? y : x, max(x, y) = y >= x ? y : x
+template <typename T> static T swift_min(T x, T y) { return y < x ? y : x; }
+template <typename T> static T swift_max(T x, T y) { return y >= x ? y : x; }
+
+// CoherePipeline.swift:90-97: symmetric Hann, and a length-1 window is [0] (build_window would divide by zero)
+void build_window_cohere(int length, std::vector<float> &w) {
+    if (length > 1) build_window(length, false, w);
+    else w.assign(length, 0.0f);
+}
+
+// CoherePipeline.swift:273-323 (slaneyMelFilter): Float32 throughout, f_min .. f_max, 1e-10 clamped denominators
+void build_filterbank_cohere(int n_fft, int n_mels, int sample_rate, float f_min, float f_max, std::vector<float> &fb) {
+    const int bins = n_fft / 2 + 1;
+    const float f_sp = 200.0f / 3.0f, min_log_hz = 1000.0f, min_log_mel = 15.0f, log_step = 0.06875177742f;
+    auto to_mel = [&](float hz) { return hz >= min_log_hz ? min_log_mel + logf(hz / min_log_hz) / log_step : hz / f_sp; };
+    auto to_hz = [&](float mel) {
+        return mel >= min_log_mel ? min_log_hz * expf(log_step * (mel - min_log_mel)) : f_sp * mel;
+    };
+    std::vector<float> freq(bins), hz(n_mels + 2);
+    for (int k = 0; k < bins; ++k) freq[k] = (float)sample_rate * (float)k / (float)n_fft;
+    const float mel_min = to_mel(f_min), mel_max = to_mel(f_max);
+    const float step = (mel_max - mel_min) / (float)(n_mels + 1);
+    for (int i = 0; i < n_mels + 2; ++i) hz[i] = to_hz(mel_min + (float)i * step);
+    fb.assign((size_t)n_mels * bins, 0.0f);
+    for (int m = 0; m < n_mels; ++m) {
+        const float lower = hz[m], center = hz[m + 1], upper = hz[m + 2];
+        const float left_den = swift_max(center - lower, 1e-10f), right_den = swift_max(upper - center, 1e-10f);
+        float *row = &fb[(size_t)m * bins];
+        for (int k = 0; k < bins; ++k) {
+            const float f = freq[k];
+            if (f < lower || f > upper) continue;
+            row[k] = f <= center ? (f - lower) / left_den : (upper - f) / right_den;
+        }
+        const float enorm = 2.0f / swift_max(upper - lower, 1e-10f);
+        for (int k = 0; k < bins; ++k) row[k] *= enorm;
+    }
+}
+
+// StyleTTS2MelExtractor.swift:160-221 (htkMelFilterbank): HTK scale in Float32 (log10f, powf), no norm, 0 .. sr/2, bin
+// frequencies k * (sr / nFFT) for the rate the table is built for (16 kHz for StyleTTS2's 24 kHz audio)
+void build_filterbank_htk_f32(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb) {
+    const int bins = n_fft / 2 + 1;
+    auto to_mel = [](float hz) { return 2595.0f * log10f(1.0f + hz / 700.0f); };
+    auto to_hz = [](float mel) { return 700.0f * (powf(10.0f, mel / 2595.0f) - 1.0f); };
+    std::vector<float> freq(bins), hz(n_mels + 2);
+    const float bin_step = (float)sample_rate / (float)n_fft;
+    for (int k = 0; k < bins; ++k) freq[k] = (float)k * bin_step;
+    const float mel_min = to_mel(0.0f), mel_max = to_mel((float)sample_rate / 2.0f);
+    for (int i = 0; i < n_mels + 2; ++i) {
+        const float frac = (float)i / (float)(n_mels + 1);
+        hz[i] = to_hz(mel_min + (mel_max - mel_min) * frac);
+    }
+    fb.assign((size_t)n_mels * bins, 0.0f);
+    for (int m = 0; m < n_mels; ++m) {
+        const float left = hz[m], center = hz[m + 1], right = hz[m + 2];
+        const float left_slope = center - left, right_slope = right - center;
+        for (int k = 0; k < bins; ++k) {
+            const float f = freq[k];
+            if (f < left || f > right) continue;
+            float val;
+            if (f <= center) val = left_slope > 0 ? (f - left) / left_slope : 0.0f;
+            else val = right_slope > 0 ? (right - f) / right_slope : 0.0f;
+            fb[(size_t)m * bins + k] = swift_max(val, 0.0f);
+        }
+    }
+}
+
+// LuxTtsMelExtractor.swift:158-187 (torchaudio melscale_fbanks, norm nil, HTK): Double throughout, bins on
+// linspace(0, sr/2, bins), Float(max(0, min(up, down)))
+void build_filterbank_htk_f64(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb) {
+    const int bins = n_fft / 2 + 1;
+    const double f_max = (double)sample_rate / 2.0;
+    auto to_mel = [](double hz) { return 2595.0 * log10(1.0 + hz / 700.0); };
+    auto to_hz = [](double mel) { return 700.0 * (pow(10.0, mel / 2595.0) - 1.0); };
+    const double mel_min = to_mel(0.0), mel_max = to_mel(f_max);
+    std::vector<double> pts(n_mels + 2), freq(bins);
+    for (int i = 0; i < n_mels + 2; ++i) pts[i] = to_hz(mel_min + (double)i * (mel_max - mel_min) / (double)(n_mels + 1));
+    for (int b = 0; b < bins; ++b) freq[b] = (double)b * f_max / (double)(bins - 1);
+    fb.assign((size_t)n_mels * bins, 0.0f);
+    for (int m = 0; m < n_mels; ++m)
+        for (int b = 0; b < bins; ++b) {
+            const double up = (freq[b] - pts[m]) / (pts[m + 1] - pts[m]);
+            const double down = (pts[m + 2] - freq[b]) / (pts[m + 2] - pts[m + 1]);
+            fb[(size_t)m * bins + b] = (float)swift_max(0.0, swift_min(up, down));
+        }
+}
+
+int check_ex_config(const MelConfig &c) {
+    auto bad = [](const char *what) {
+        fa::set_error("mel ex config: %s", what);
+        return FA_INVALID_ARGUMENT;
+    };
+    if (c.fb_kind < 0 || c.fb_kind > 3) return bad("filterbank must be one of FA_MEL_FB_* (0..3)");
+    if (c.filter_sample_rate < 0) return bad("filter_sample_rate must be 0 (the audio's rate) or positive");
+    if (c.center_edge != 0 && c.center_edge != 1) return bad("center_edge must be FA_MEL_EDGE_ZERO or FA_MEL_EDGE_REFLECT");
+    if (!std::isfinite(c.spectrum_power) || !(c.spectrum_power > 0.0f)) return bad("spectrum_power must be finite and > 0");
+    if (!std::isfinite(c.log_mean) || !std::isfinite(c.log_std) || c.log_std == 0.0f)
+        return bad("log_mean must be finite and log_std finite and non-zero");
+    if (!std::isfinite(c.f_min) || !std::isfinite(c.f_max)) return bad("f_min and f_max must be finite");
+    if (c.fb_kind != 1 && (c.f_min != 0.0f || (c.f_max > 0.0f && c.f_max != (float)c.filter_rate() / 2.0f)))
+        return bad("f_min / f_max apply to FA_MEL_FB_COHERE only (the other tables span 0 .. filter_sample_rate / 2)");
+    if (c.reflect() && c.preemph != 0.0f)
+        return bad("FA_MEL_EDGE_REFLECT needs preemph 0 (no reference frontend pre-emphasises a reflected signal)");
+    return FA_OK;
+}
+
 static constexpr int kWarpsPerCta = 8;
 static constexpr int kCtasPerSm = 2;
+
+// the any-nFFT kernel's variant for a launch (see mel_generic_kernel)
+typedef void (*GenericKernel)(const MelLaunch, const GenericParams);
+template <bool R, int S> static GenericKernel generic_variant(bool affine) {
+    return affine ? mel_generic_kernel<R, S, true> : mel_generic_kernel<R, S, false>;
+}
+template <bool R> static GenericKernel generic_variant(int spectrum, bool affine) {
+    return spectrum == kSpecPower ? generic_variant<R, kSpecPower>(affine)
+                                  : (spectrum == kSpecMagnitude ? generic_variant<R, kSpecMagnitude>(affine)
+                                                                : generic_variant<R, kSpecGeneral>(affine));
+}
+static GenericKernel generic_variant(bool reflect, int spectrum, bool affine) {
+    return reflect ? generic_variant<true>(spectrum, affine) : generic_variant<false>(spectrum, affine);
+}
 
 // Device copy of a host table (at least one element, so that an empty table still has an address).
 template <typename T, typename U> static int upload_table(DeviceBuffer<T> &b, const std::vector<U> &v) {
@@ -484,11 +619,23 @@ int MelPlan::init(const MelConfig &c) {
                       cfg.n_fft, cfg.hop_length, cfg.win_length, cfg.n_mels);
         return FA_UNSUPPORTED;
     }
-    // the specialised kernel covers every in-repo caller's shape; anything else takes mel_generic_kernel
-    generic = cfg.n_fft != kNfft || (cfg.hop_length & 1) || cfg.hop_length > 1024;
-    const int n_fft = cfg.n_fft, bins = n_fft / 2 + 1;
-    build_window(cfg.win_length, cfg.window_periodic != 0, window);
-    build_filterbank(cfg.n_fft, cfg.n_mels, cfg.sample_rate, filterbank);
+    int st = check_ex_config(cfg);
+    if (st != FA_OK) return st;
+    // the specialised kernel covers every in-repo caller's shape; anything else takes mel_generic_kernel, and so do
+    // reflect padding, a spectrum other than |X|^2 and the affine epilogue (mel512_kernel only ever sees another table)
+    const int spectrum = spectrum_kind(cfg.spectrum_power);
+    generic = cfg.n_fft != kNfft || (cfg.hop_length & 1) || cfg.hop_length > 1024 || cfg.reflect() ||
+              spectrum != kSpecPower || cfg.affine();
+    const int n_fft = cfg.n_fft, bins = n_fft / 2 + 1, fr = cfg.filter_rate();
+    if (cfg.fb_kind == 1 && !cfg.window_periodic) build_window_cohere(cfg.win_length, window);
+    else build_window(cfg.win_length, cfg.window_periodic != 0, window);
+    switch (cfg.fb_kind) {
+    case 1: build_filterbank_cohere(n_fft, cfg.n_mels, fr, cfg.f_min, cfg.f_max > 0.0f ? cfg.f_max : (float)fr / 2.0f,
+                                    filterbank); break;
+    case 2: build_filterbank_htk_f32(n_fft, cfg.n_mels, fr, filterbank); break;
+    case 3: build_filterbank_htk_f64(n_fft, cfg.n_mels, fr, filterbank); break;
+    default: build_filterbank(n_fft, cfg.n_mels, fr, filterbank);
+    }
 
     // banded filterbank: per mel the contiguous range of non-zero bins, widened with explicit zero weights to whole
     // bin quads.  Weights are stored times 1/4 because the kernel's power tile holds 4|X|^2 (mel_core.cuh).
@@ -549,7 +696,7 @@ int MelPlan::init(const MelConfig &c) {
     int dev = 0;
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
-    int st = sm90_device_props(dev, prop);
+    st = sm90_device_props(dev, prop);
     if (st != FA_OK) return st;
     num_sms = prop.multiProcessorCount;
 
@@ -570,13 +717,14 @@ int MelPlan::init(const MelConfig &c) {
         }
     }
     // weights packed in the order the kernel finds the bins in its power tile: mel512_kernel swizzles inside each bin quad
-    // (pow_pos, mel_core.cuh), the any-nFFT kernel keeps the natural order
+    // (pow_pos, mel_core.cuh), the any-nFFT kernel keeps the natural order.  Scaled by 1/4 where the tile holds 4|X|^2.
+    const float wscale = spectrum == kSpecPower ? 0.25f : 1.0f;
     std::vector<float> w;
     w.reserve(fb_nnz);
     for (int m = 0; m < cfg.n_mels; ++m)
         for (int k = lo[m]; k < hi[m]; ++k) {
             const int src = generic ? k : ((k & ~3) | ((k & 3) ^ ((k >> 4) & 3)));   // position k holds bin src: pow_pos is an involution
-            w.push_back(src < bins ? 0.25f * filterbank[(size_t)m * bins + src] : 0.0f);
+            w.push_back(src < bins ? wscale * filterbank[(size_t)m * bins + src] : 0.0f);
         }
 
     std::vector<float> win_tab(n_fft, 0.0f);
@@ -630,7 +778,10 @@ int MelPlan::init(const MelConfig &c) {
             return FA_UNSUPPORTED;
         }
         smem_bytes = fixed + per_warp * generic_warps;
-        FA_CUDA_TRY(cudaFuncSetAttribute(mel_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+        // the variants this handle launches: .center (reflected or not) and the other modes, which never reflect
+        for (const bool r : {false, cfg.reflect()})
+            FA_CUDA_TRY(cudaFuncSetAttribute(generic_variant(r, spectrum, cfg.affine()),
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
         return FA_OK;
     }
     FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, double, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
@@ -712,9 +863,12 @@ int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inli
     P.inv_n_mels = (unsigned)((0x100000000ull + (unsigned)cfg.n_mels - 1) / (unsigned)cfg.n_mels);
     if (generic) {
         GenericParams G{cfg.n_fft, generic_log2n, cfg.n_fft / 2 + 1, generic_prow,
-                        static_cast<const cpxd *>(d_generic_tw.data()), generic_warps};
+                        static_cast<const cpxd *>(d_generic_tw.data()), generic_warps, cfg.spectrum_power, cfg.log_mean,
+                        cfg.log_std};
         const int ggrid = std::min(total_tiles, num_sms * std::max(1, 16 / generic_warps));
-        FA_CUDA_TRY(fa::launch(mel_generic_kernel, ggrid, generic_warps * 32, smem_bytes, stream, P, G));
+        const GenericKernel kernel = generic_variant(mode == 0 && cfg.reflect(), spectrum_kind(cfg.spectrum_power),
+                                                     cfg.affine());
+        FA_CUDA_TRY(fa::launch(kernel, ggrid, generic_warps * 32, smem_bytes, stream, P, G));
         return FA_OK;
     }
     const int grid = std::min(total_tiles, num_sms * kCtasPerSm);
@@ -773,6 +927,18 @@ int MelPlan::compute_device(const float *d_in, long long n, float last, int mode
     if (st != FA_OK) return st;
     const bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
     return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, tiles_of(T), mode, layout, stream,
+                  aligned);
+}
+
+int MelPlan::launch_clip(const float *d_in, long long n, long long T, int layout, float *d_out_buf, cudaStream_t stream) {
+    if (T <= 0) return FA_OK;
+    int st = units.reserve(unit_bytes(1));
+    if (st != FA_OK) return st;
+    units.host.data()[0] = MelUnit{0, n, 0, T, 0, T, 0.0f, 0};
+    st = units.upload(sizeof(MelUnit), stream);
+    if (st != FA_OK) return st;
+    const bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
+    return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, tiles_of(T), 0, layout, stream,
                   aligned);
 }
 
@@ -962,7 +1128,10 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
     for (int c = 0; c < chunks; ++c) {
         const bool tail = c == chunks - 1;
         // model-rate samples needed so far, and the input frames those samples depend on
-        const long long s_end = tail ? n : std::min(n, (bounds[c + 1] - 1) * cfg.hop_length + cfg.n_fft - pad);
+        long long s_end = tail ? n : std::min(n, (bounds[c + 1] - 1) * cfg.hop_length + cfg.n_fft - pad);
+        // Reflected .center frames read the clip's end only when they cross it (then s_end = n already), and a frame
+        // crossing the start reads up to x[pad] (reflect_index): every unit's range must hold that sample.
+        if (mode == 0 && cfg.reflect()) s_end = std::min(n, std::max(s_end, pad + 1));
         long long in_need = frames;
         if (!tail) {
             if (f.in_rate == f.out_rate) in_need = s_end;

@@ -23,7 +23,28 @@ struct MelConfig {
     float log_floor;
     int32_t log_floor_mode;    // 0 additive log(x + floor), 1 clamped log(max(x, floor))
     int32_t window_periodic;
+    // fa_mel_ex_config (fa_mel_create_ex); the defaults are fa_mel_create's behaviour
+    int32_t fb_kind = 0;              // FA_MEL_FB_*
+    int32_t filter_sample_rate = 0;   // 0 = sample_rate
+    float f_min = 0.0f, f_max = 0.0f;
+    int32_t center_edge = 0;          // FA_MEL_EDGE_*
+    float spectrum_power = 2.0f;
+    float log_mean = 0.0f, log_std = 1.0f;
+
+    int filter_rate() const { return filter_sample_rate > 0 ? filter_sample_rate : sample_rate; }
+    bool reflect() const { return center_edge == 1; }
+    bool affine() const { return log_mean != 0.0f || log_std != 1.0f; }
+    // every ex field as fa_mel_create leaves it: the streams and the NeMo adapters accept only such handles
+    bool neutral() const {
+        return fb_kind == 0 && filter_rate() == sample_rate && f_min == 0.0f && f_max <= 0.0f && center_edge == 0 &&
+               spectrum_power == 2.0f && !affine();
+    }
 };
+
+// Spectrum the any-nFFT kernel feeds its filterbank: |X|^2 (the power tile holds 4|X|^2, the weights carry 1/4),
+// |X| or |X|^p (the tile holds the value itself, the weights are unscaled).
+enum { kSpecPower = 0, kSpecMagnitude = 1, kSpecGeneral = 2 };
+inline int spectrum_kind(float p) { return p == 2.0f ? kSpecPower : (p == 1.0f ? kSpecMagnitude : kSpecGeneral); }
 
 // One unit of work = a run of frames of one clip.  A long clip is cut into several units so that H2D copies,
 // kernels and D2H copies of successive units overlap; a batch of clips is simply many units in one launch.
@@ -136,6 +157,9 @@ struct MelPlan {
     int compute_batch_device(const float *d_in, const long long *offsets, int count, const float *last, int mode,
                              int layout, float *d_out_buf, const long long *out_offsets, long long *mel_lengths,
                              long long *num_frames, cudaStream_t stream);
+    // One .center launch of exactly T frames of one n-sample clip at d_in, whatever n (an empty clip reads zeros): the
+    // torch-style frontends count their frames by their own rules (mel_adapters.cu).  last = 0.
+    int launch_clip(const float *d_in, long long n, long long T, int layout, float *d_out_buf, cudaStream_t stream);
 };
 
 // mel_stream.cu: live streams on one plan, SortformerDiarizer's incremental mel stream (SortformerDiarizer.swift:204-217,
@@ -175,9 +199,22 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
                      long long *total_frames, int *valid_frames);
 int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean, long long *cmn_count, float *out,
                     long long out_len, long long *frames);
+// the torch-style frontends (CoherePipeline.swift, StyleTTS2MelExtractor.swift, LuxTtsMelExtractor.swift)
+int cohere_features(MelPlan &p, const float *audio, long long n, long long fixed_frames, float *out, long long out_len,
+                    long long *frames, long long *valid_frames);
+int styletts2_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames);
+int luxtts_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames);
 
 void build_window(int length, bool periodic, std::vector<float> &w);
 void build_filterbank(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb);
+// fa_mel_create_ex's tables, each restating its Swift in that Swift's arithmetic (mel_kernels.cu)
+void build_window_cohere(int length, std::vector<float> &w);
+void build_filterbank_cohere(int n_fft, int n_mels, int sample_rate, float f_min, float f_max, std::vector<float> &fb);
+void build_filterbank_htk_f32(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb);
+void build_filterbank_htk_f64(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb);
+// every fa_mel_ex_config field the kernels cannot honour, as fa_last_error text (FA_INVALID_ARGUMENT), before any
+// allocation
+int check_ex_config(const MelConfig &c);
 
 } // namespace mel
 } // namespace fa

@@ -96,6 +96,10 @@ static void push_frames(const MelConfig &c, long long received, long long emitte
 }
 
 int MelStreamSet::check_config(const MelConfig &c) {
+    if (!c.neutral()) {
+        fa::set_error("mel stream: live streams run AudioMelSpectrogram only, not a handle with fa_mel_ex_config fields set");
+        return FA_INVALID_ARGUMENT;
+    }
     if (c.pad_to > 1) {
         fa::set_error("mel stream: pad_to must be 0 or 1 (an emit returns exactly its frames), got %d", c.pad_to);
         return FA_INVALID_ARGUMENT;

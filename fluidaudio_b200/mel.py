@@ -8,6 +8,8 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
+from dataclasses import dataclass
+from typing import NamedTuple
 
 import numpy as np
 
@@ -29,7 +31,34 @@ class Precision(enum.IntEnum):
     f32 = 1           # FA_MEL_PRECISION_F32: float32 transform like vDSP_DFT, two frames per warp
 
 
+class MelFilterbank(enum.IntEnum):   # FA_MEL_FB_*: whose table construction a handle restates
+    audio_mel = 0
+    cohere = 1
+    styletts2 = 2
+    luxtts = 3
+
+
+class CenterEdge(enum.IntEnum):      # FA_MEL_EDGE_*: what .center pads with
+    zero = 0
+    reflect = 1
+
+
 _TIME_MAJOR, _MEL_MAJOR = 0, 1
+_EX_FIELDS = {name for name, _ in _lib.MelExConfig._fields_} - {"base"}
+
+
+def ex_config(preset: str | None = None, **fields) -> "_lib.MelExConfig":
+    """An ``fa_mel_ex_config``: neutral (``fa_mel_ex_default_config``) or one of the presets ``"cohere"``,
+    ``"styletts2"``, ``"luxtts"``, then ``fields`` set by name (base fields such as ``n_mels`` or ex fields such as
+    ``spectrum_power``)."""
+    L = _lib.load()
+    cfg = _lib.MelExConfig()
+    init = {None: L.fa_mel_ex_default_config, "cohere": L.fa_mel_preset_cohere, "styletts2": L.fa_mel_preset_styletts2,
+            "luxtts": L.fa_mel_preset_luxtts}[preset]
+    init(C.byref(cfg))
+    for k, v in fields.items():
+        setattr(cfg if k in _EX_FIELDS else cfg.base, k, v)
+    return cfg
 _LEGACY = 2
 
 
@@ -50,6 +79,23 @@ class AudioMelSpectrogram:
         self.precision = Precision(precision)
         if self.precision != Precision.f64:
             self.set_precision(self.precision)
+
+    @classmethod
+    def from_ex_config(cls, cfg: "_lib.MelExConfig", precision: Precision = Precision.f64) -> "AudioMelSpectrogram":
+        """A handle made by ``fa_mel_create_ex``: every method of this class works on it unchanged."""
+        self = cls.__new__(cls)
+        b = cfg.base
+        self.sample_rate, self.n_mels, self.n_fft = b.sample_rate, b.n_mels, b.n_fft
+        self.hop_length, self.win_length, self.preemph = b.hop_length, b.win_length, b.preemph
+        self.pad_to = max(1, b.pad_to)
+        self._L = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._L.fa_mel_create_ex(C.byref(cfg), C.byref(h)), "fa_mel_create_ex")
+        self._h = h
+        self.precision = Precision.f64
+        if Precision(precision) != Precision.f64:
+            self.set_precision(precision)
+        return self
 
     def set_precision(self, precision: Precision):
         """Not part of the Swift class: selects the transform arithmetic (see include/fluidaudio_b200.h)."""
@@ -343,3 +389,124 @@ class LSEENDMelFrontend:
                                                        out.size, C.byref(frames)), "fa_mel_lseend_features")
         self.cmn_count = cnt.value
         return out[: frames.value]
+
+
+# ================================================================================================ torch-style frontends
+class CohereMelSpectrogram:
+    """ASR/Cohere/CoherePipeline.swift:41-324: NeMo FilterbankFeatures-compatible log-mel (Slaney table over
+    ``f_min`` .. ``f_max``, ``|X|^magPower``, additive log guard), per-feature CMVN over the valid frames and
+    ``padOrTruncate``.  The STFT, the table product and the log run in the mel kernel, the CMVN and the packing in one
+    epilogue kernel behind it (``fa_mel_cohere_features``).  Pre-emphasis is one fused multiply-add per sample where the
+    Swift rounds twice (DESIGN §4.1b)."""
+
+    @dataclass(frozen=True)
+    class Config:
+        sample_rate: int = 16_000
+        win_length: int = 400
+        hop_length: int = 160
+        n_mels: int = 128
+        f_min: float = 0.0
+        f_max: float = 8_000.0
+        preemph: float = 0.97
+        mag_power: float = 2.0
+        log_zero_guard: float = 5.9604645e-08   # 2^-24
+        cmvn_epsilon: float = 1.0e-5
+
+    class Output(NamedTuple):
+        mel: np.ndarray          # [nMels x nFrames]
+        valid_frames: int
+
+    def __init__(self, config: "CohereMelSpectrogram.Config | None" = None,
+                 precision: Precision = Precision.f64):
+        self.config = c = config or CohereMelSpectrogram.Config()
+        if c.cmvn_epsilon != 1.0e-5:
+            raise ValueError("the CMVN epsilon of the device epilogue is CohereMelSpectrogram.Config's 1e-5")
+        self.n_fft = 1 << max(0, (c.win_length - 1).bit_length())   # nextPowerOfTwo(atLeast: winLength)
+        cfg = ex_config("cohere", sample_rate=c.sample_rate, win_length=c.win_length, hop_length=c.hop_length,
+                        n_mels=c.n_mels, n_fft=self.n_fft, f_min=c.f_min, f_max=c.f_max, preemph=c.preemph,
+                        spectrum_power=c.mag_power, log_floor=c.log_zero_guard)
+        self.mel = AudioMelSpectrogram.from_ex_config(cfg, precision)
+
+    def valid_frame_count(self, n: int) -> int:
+        return max(0, n) // self.config.hop_length
+
+    def features(self, audio, fixed_frames: int = 3_500) -> tuple[np.ndarray, int]:
+        """``compute`` followed by ``padOrTruncate(fixedFrames:)`` in one call: ([nMels x fixedFrames], featureLength).
+        ``fixed_frames < 0`` skips the padOrTruncate (then this is ``compute``)."""
+        audio = np.ascontiguousarray(audio, np.float32).reshape(-1)
+        n = audio.size
+        W = 1 + n // self.config.hop_length if fixed_frames < 0 else int(fixed_frames)
+        out = np.zeros((self.config.n_mels, W), np.float32)
+        frames, valid = C.c_int64(), C.c_int64()
+        _lib.check(self.mel._L.fa_mel_cohere_features(self.mel._h, _lib.ptr(audio) if n else None, n, int(fixed_frames),
+                                                      out.ctypes.data, out.size, C.byref(frames), C.byref(valid)),
+                   "fa_mel_cohere_features")
+        return out, int(valid.value)
+
+    def compute(self, audio) -> "CohereMelSpectrogram.Output":
+        mel, valid = self.features(audio, -1)
+        return CohereMelSpectrogram.Output(mel, valid)
+
+    @staticmethod
+    def pad_or_truncate(mel: np.ndarray, valid_frames: int, fixed_frames: int = 3_500) -> tuple[np.ndarray, int]:
+        """``padOrTruncate`` (:250-263) on a [nMels x T] array."""
+        mel = np.asarray(mel, np.float32)
+        if mel.shape[0] == 0:
+            return mel, 0
+        cur = mel.shape[1]
+        if cur >= fixed_frames:
+            return mel[:, :fixed_frames].copy(), min(valid_frames, fixed_frames)
+        pad = np.zeros((mel.shape[0], fixed_frames - cur), np.float32)
+        return np.concatenate([mel, pad], axis=1), min(valid_frames, fixed_frames)
+
+
+class StyleTTS2MelExtractor:
+    """TTS/StyleTTS2/Pipeline/Preprocess/StyleTTS2MelExtractor.swift: torchaudio MelSpectrogram(n_mels 80, n_fft 2048,
+    win 1200, hop 300) on 24 kHz audio with the HTK table built for 16 kHz bins, reflect padding, and
+    ``(log(mel + 1e-5) - (-4)) / 4`` (``fa_mel_styletts2_features``: one kernel launch)."""
+
+    def __init__(self, n_fft: int = 2048, win_length: int = 1200, hop_length: int = 300, n_mels: int = 80,
+                 filter_sample_rate: int = 16_000, mean: float = -4.0, std: float = 4.0, log_epsilon: float = 1e-5,
+                 sample_rate: int = 24_000):
+        self.n_mels, self.hop_length = n_mels, hop_length
+        cfg = ex_config("styletts2", n_fft=n_fft, win_length=win_length, hop_length=hop_length, n_mels=n_mels,
+                        filter_sample_rate=filter_sample_rate, log_mean=mean, log_std=std, log_floor=log_epsilon,
+                        sample_rate=sample_rate)
+        self.mel = AudioMelSpectrogram.from_ex_config(cfg)
+
+    def compute(self, audio) -> tuple[np.ndarray, int]:
+        """(mel [nMels x frames] row-major, frames), frames = 1 + n / hop."""
+        audio = np.ascontiguousarray(audio, np.float32).reshape(-1)
+        n = audio.size
+        T = 1 + n // self.hop_length
+        out = np.empty((self.n_mels, T), np.float32)
+        frames = C.c_int64()
+        _lib.check(self.mel._L.fa_mel_styletts2_features(self.mel._h, _lib.ptr(audio) if n else None, n, out.ctypes.data,
+                                                         out.size, C.byref(frames)), "fa_mel_styletts2_features")
+        return out, int(frames.value)
+
+
+class LuxTtsMelExtractor:
+    """TTS/LuxTts/LuxTtsMelExtractor.swift: torchaudio MelSpectrogram(24000, n_fft 1024, hop 256, 100 mels, power 1,
+    reflect padding) with the float64 HTK table, ``log(max(mel, 1e-7))`` and lhotse's frame count
+    (``fa_mel_luxtts_features``: one kernel launch)."""
+
+    def __init__(self):
+        self.n_mels, self.hop_length = 100, 256
+        self.mel = AudioMelSpectrogram.from_ex_config(ex_config("luxtts"))
+
+    def frame_count(self, sample_count: int) -> int:
+        """lhotse ``compute_num_frames``: (n + hop/2) / hop."""
+        return (sample_count + self.hop_length // 2) // self.hop_length
+
+    def extract(self, audio) -> np.ndarray:
+        """[T x nMels] log-mel frames, T = frame_count(n) (none for an empty clip)."""
+        audio = np.ascontiguousarray(audio, np.float32).reshape(-1)
+        n = audio.size
+        T = self.frame_count(n) if n else 0
+        out = np.empty((T, self.n_mels), np.float32)
+        frames = C.c_int64()
+        _lib.check(self.mel._L.fa_mel_luxtts_features(self.mel._h, _lib.ptr(audio) if n else None, n,
+                                                      out.ctypes.data if T else None, out.size, C.byref(frames)),
+                   "fa_mel_luxtts_features")
+        return out

@@ -99,6 +99,53 @@ typedef struct fa_mel fa_mel;   /* one handle per stream of calls: like the Swif
 
 void fa_mel_default_config(fa_mel_config *cfg);
 fa_status fa_mel_create(const fa_mel_config *cfg, fa_mel **out);
+
+/* The other STFT -> mel -> log frontends of the reference, as a superset of fa_mel_config.  A handle made by
+ * fa_mel_create_ex is an ordinary fa_mel: every fa_mel_compute* call, fa_audio_to_mel, the timers and the getters work
+ * on it.  Reflect padding, spectrum_power != 2 and the affine epilogue run on the any-nFFT kernel; fa_mel_stream_*,
+ * fa_mel_unified_features and fa_mel_lseend_features refuse a handle whose ex fields are not neutral
+ * (FA_STATUS_INVALID_ARGUMENT).  A handle from fa_mel_ex_default_config equals fa_mel_create on the same base.
+ *   FA_MEL_FB_AUDIO_MEL  AudioMelSpectrogram's Slaney table (Shared/AudioMelSpectrogram.swift:564-642)
+ *   FA_MEL_FB_COHERE     CohereMelSpectrogram.slaneyMelFilter, f_min .. f_max (ASR/Cohere/CoherePipeline.swift:273-303);
+ *                        also its window: symmetric Hann with a length-1 window [0] (:90-97)
+ *   FA_MEL_FB_STYLETTS2  StyleTTS2MelExtractor.htkMelFilterbank, float32, bins k * filter_sample_rate / nFFT
+ *                        (TTS/StyleTTS2/Pipeline/Preprocess/StyleTTS2MelExtractor.swift:174-221)
+ *   FA_MEL_FB_LUXTTS     LuxTtsMelExtractor.htkMelFilterbank, float64 (TTS/LuxTts/LuxTtsMelExtractor.swift:160-187)
+ * FA_MEL_EDGE_REFLECT changes what FA_MEL_PAD_CENTER pads with: audio index i < 0 reads x[min(-i, n-1)], i >= n reads
+ * x[max(2n-2-i, 0)] (the reference's reflectPad clamps, :226-250), an empty clip reads zeros.  It needs preemph 0. */
+enum { FA_MEL_FB_AUDIO_MEL = 0, FA_MEL_FB_COHERE = 1, FA_MEL_FB_STYLETTS2 = 2, FA_MEL_FB_LUXTTS = 3 };
+enum { FA_MEL_EDGE_ZERO = 0, FA_MEL_EDGE_REFLECT = 1 };
+typedef struct {
+    fa_mel_config base;          /* sample_rate = the audio's rate (and the converter stage's target rate) */
+    int32_t filterbank;          /* FA_MEL_FB_*: whose table construction, restated exactly */
+    int32_t filter_sample_rate;  /* rate the bin frequencies are computed for; 0 = base.sample_rate (StyleTTS2: 16000) */
+    float f_min, f_max;          /* Hz; f_max <= 0 means filter_sample_rate / 2 (Cohere only; the others fix 0 .. sr/2) */
+    int32_t center_edge;         /* what .center pads with: zeros (default) or reflection */
+    float spectrum_power;        /* 2 = |X|^2 (default), 1 = |X|, any other p > 0 = |X|^p */
+    float log_mean, log_std;     /* out = (log(..) - log_mean) / log_std; 0 / 1 (default) skips it */
+} fa_mel_ex_config;
+void fa_mel_ex_default_config(fa_mel_ex_config *cfg);   /* base = fa_mel_default_config, everything else neutral */
+void fa_mel_preset_cohere(fa_mel_ex_config *cfg);       /* CohereMelSpectrogram.Config() + CohereAsrConfig */
+void fa_mel_preset_styletts2(fa_mel_ex_config *cfg);    /* StyleTTS2Constants */
+void fa_mel_preset_luxtts(fa_mel_ex_config *cfg);       /* LuxTtsConstants */
+/* Anything the kernels cannot honour is refused before any allocation, with fa_last_error text. */
+fa_status fa_mel_create_ex(const fa_mel_ex_config *cfg, fa_mel **out);
+
+/* The reference classes' own calls, one mel launch each (plus the CMVN epilogue for Cohere).  Each needs a handle of its
+ * class (filterbank kind, edge, spectrum and log mode; pad_to 0 or 1), else FA_STATUS_INVALID_ARGUMENT; a too small
+ * out_len gives FA_STATUS_OUTPUT_TOO_SMALL.  Both are returned before any copy or launch, with out untouched.
+ * fa_mel_cohere_features = CohereMelSpectrogram.compute + padOrTruncate (CoherePipeline.swift:127-263): T = 1 + n / hop
+ *   frames, valid = n / hop, per-mel CMVN (ddof 1, epsilon 1e-5) over all valid frames when valid > 1, frames >= valid
+ *   zeroed, out = [n_mels x W] with W = fixed_frames (truncated or zero-padded), or W = T when fixed_frames < 0;
+ *   *frames = W, *valid_frames = min(valid, W).  Pre-emphasis runs as one fused multiply-add per sample where the
+ *   reference rounds twice (see DESIGN §4.1b).
+ * fa_mel_styletts2_features = StyleTTS2MelExtractor.compute: [n_mels x frames], frames = 1 + n / hop (1 for n = 0).
+ * fa_mel_luxtts_features = LuxTtsMelExtractor.extract: [frames x n_mels], frames = (n + hop/2) / hop (0 when n == 0). */
+fa_status fa_mel_cohere_features(fa_mel *mel, const float *audio, size_t n, int64_t fixed_frames, float *out,
+                                 size_t out_len, int64_t *frames, int64_t *valid_frames);
+fa_status fa_mel_styletts2_features(fa_mel *mel, const float *audio, size_t n, float *out, size_t out_len,
+                                    int64_t *frames);
+fa_status fa_mel_luxtts_features(fa_mel *mel, const float *audio, size_t n, float *out, size_t out_len, int64_t *frames);
 void fa_mel_destroy(fa_mel *mel);
 fa_status fa_mel_get_window(const fa_mel *mel, float *out, size_t len);       /* getHannWindow(): win_length floats */
 fa_status fa_mel_get_filterbank(const fa_mel *mel, float *out, size_t len);   /* getFilterbank(): n_mels x (n_fft/2+1) */

@@ -98,4 +98,18 @@ cl.OfflineClusterer().cluster(wide, rng.standard_normal((40, 16)))
 emb, _ = synth.speaker_embeddings(900, 256, 4, seed=12)
 rho, psi = synth.synthetic_plda(emb)
 cl.OfflineClusterer(psi=psi).cluster_batch(emb, rho, np.array([0, 0, 300, 300, 600, 900, 900], np.int64))
+# torch-style frontends: the any-nFFT kernel's reflect / magnitude / affine variants on clips shorter than the pad, the
+# Cohere table on mel512_kernel with its CMVN epilogue (padOrTruncate both ways), and a general spectrum power
+from fluidaudio_b200.mel import CohereMelSpectrogram, LuxTtsMelExtractor, StyleTTS2MelExtractor
+b = synth.tone_noise_audio(24000 * 2 + 5)
+sty, lux = StyleTTS2MelExtractor(), LuxTtsMelExtractor()
+for n in (0, 1, 700, 24000 * 2 + 5):
+    sty.compute(b[:n])
+    lux.extract(b[:n])
+coh = CohereMelSpectrogram()
+coh.features(a[:16000 * 3], 100)
+coh.features(a[:1000], 3500)
+coh.compute(a[:1])
+CohereMelSpectrogram(CohereMelSpectrogram.Config(mag_power=1.5)).compute(a[:5000])
+sty.mel.compute_batch([b[:3], b[:30000]])
 print("sanitize target done")
