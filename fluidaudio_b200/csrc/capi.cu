@@ -668,8 +668,10 @@ FA_API fa_status fa_mel_create_ex(const fa_mel_ex_config *cfg, fa_mel **out) {
     c.spectrum_power = cfg->spectrum_power;
     c.log_mean = cfg->log_mean;
     c.log_std = cfg->log_std;
-    const int st = mel::check_ex_config(c);   // before the device is touched
-    if (st != FA_OK) return (fa_status)st;
+    if (const char *why = mel::check_ex_config(c)) {   // before the device is touched
+        fa::set_error("mel ex config: %s", why);
+        return FA_STATUS_INVALID_ARGUMENT;
+    }
     return create_mel(c, out);
 }
 
@@ -719,7 +721,7 @@ FA_API int32_t fa_mel_get_precision(const fa_mel *mel) {
 }
 
 static bool mel_args_ok(int32_t mode, int32_t layout) {
-    if (mode < 0 || mode > 2 || layout < 0 || layout > 1) {
+    if (mode < FA_MEL_PAD_CENTER || mode > FA_MEL_LEGACY_COMPUTE || layout < FA_MEL_TIME_MAJOR || layout > FA_MEL_MEL_MAJOR) {
         fa::set_error("padding_mode must be 0..2 and layout 0..1");
         return false;
     }

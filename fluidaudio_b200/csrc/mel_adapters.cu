@@ -137,7 +137,7 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
     float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
     if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), window, sizeof(float) * n, cudaMemcpyHostToDevice, s));
     long long ml = 0, nf = 0;
-    st = p.compute_device(p.d_audio.data(), n, 0.0f, 0, T, 0, d_flat, T * M, &ml, &nf, s);
+    st = p.compute_device(p.d_audio.data(), n, 0.0f, FA_MEL_PAD_CENTER, T, FA_MEL_TIME_MAJOR, d_flat, T * M, &ml, &nf, s);
     if (st != FA_OK) return st;
     if (valid <= 0) {
         FA_CUDA_TRY(cudaMemsetAsync(d_pack, 0, sizeof(float) * T * M, s));
@@ -155,7 +155,7 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
     int st = check_adapter_config(p, "LS-EEND features");
     if (st != FA_OK) return st;
     const int M = p.cfg.n_mels;
-    const long long T = p.frame_count(n, 1, -1);
+    const long long T = p.frame_count(n, FA_MEL_PAD_PREPADDED, -1);
     if (frames) *frames = T;
     if (T <= 0) return FA_OK;
     if (out_len < T * M) {
@@ -169,7 +169,8 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
     FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), chunk, sizeof(float) * n, cudaMemcpyHostToDevice, s));
     FA_CUDA_TRY(cudaMemcpyAsync(d_mean, cmn_mean, sizeof(float) * M, cudaMemcpyHostToDevice, s));
     long long ml = 0, nf = 0;
-    st = p.compute_device(p.d_audio.data(), n, 0.0f, 1, -1, 0, d_flat, T * M, &ml, &nf, s);
+    st = p.compute_device(p.d_audio.data(), n, 0.0f, FA_MEL_PAD_PREPADDED, -1, FA_MEL_TIME_MAJOR, d_flat, T * M, &ml, &nf,
+                          s);
     if (st != FA_OK) return st;
     const float scale = 1.0f / logf(10.0f);   // LSEENDPreprocessor.swift:36, Float arithmetic
     FA_CUDA_TRY(fa::launch(lseend_scale_cmn_kernel, (M + 127) / 128, 128, 0, s, d_flat, T, M, d_mean, *cmn_count, scale));
@@ -227,7 +228,7 @@ static int check_class(const MelPlan &p, const char *what, int fb_kind, int edge
     const MelConfig &c = p.cfg;
     const bool any_power = power < 0.0f;   // CohereMelSpectrogram.Config.magPower is a parameter
     if (c.fb_kind != fb_kind || c.center_edge != edge || (!any_power && c.spectrum_power != power) ||
-        c.log_floor_mode != log_mode || c.pad_to > 1 || (fb_kind == 1 && c.affine())) {
+        c.log_floor_mode != log_mode || c.pad_to > 1 || (fb_kind == FA_MEL_FB_COHERE && c.affine())) {
         fa::set_error("%s: the handle is not configured as its reference class (see its fa_mel_preset_*)", what);
         return FA_INVALID_ARGUMENT;
     }
@@ -245,7 +246,7 @@ static int check_out(const char *what, long long need, long long out_len) {
 int cohere_features(MelPlan &p, const float *audio, long long n, long long fixed_frames, float *out, long long out_len,
                     long long *frames, long long *valid_frames) {
     const char *what = "Cohere mel features";
-    int st = check_class(p, what, 1, 0, -1.0f, 0);
+    int st = check_class(p, what, FA_MEL_FB_COHERE, FA_MEL_EDGE_ZERO, -1.0f, 0);
     if (st != FA_OK) return st;
     const int M = p.cfg.n_mels, hop = p.cfg.hop_length;
     const long long T = 1 + n / hop, valid = n / hop;   // padded.count = n + nFFT: 1 + n / hop frames (:146), :120
@@ -259,7 +260,7 @@ int cohere_features(MelPlan &p, const float *audio, long long n, long long fixed
     cudaStream_t s = p.streams[1];
     float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
     if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    st = p.launch_clip(p.d_audio.data(), n, T, 0, d_flat, s);
+    st = p.launch_clip(p.d_audio.data(), n, T, FA_MEL_TIME_MAJOR, d_flat, s);
     if (st != FA_OK) return st;
     FA_CUDA_TRY(fa::launch(cohere_cmvn_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, s, d_flat, M, valid, W,
                            1.0e-5f, d_pack));   // Config.cmvnEpsilon
@@ -284,17 +285,17 @@ static int run_clip(MelPlan &p, const float *audio, long long n, long long T, in
 
 int styletts2_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames) {
     const char *what = "StyleTTS2 mel features";
-    int st = check_class(p, what, 2, 1, 2.0f, 0);
+    int st = check_class(p, what, FA_MEL_FB_STYLETTS2, FA_MEL_EDGE_REFLECT, 2.0f, 0);
     if (st != FA_OK) return st;
     const long long T = 1 + n / p.cfg.hop_length;   // reflectPad keeps n + nFFT samples, an empty clip nFFT zeros (:78-87)
     if (frames) *frames = T;
     st = check_out(what, T * p.cfg.n_mels, out_len);
-    return st != FA_OK ? st : run_clip(p, audio, n, T, 1, out);
+    return st != FA_OK ? st : run_clip(p, audio, n, T, FA_MEL_MEL_MAJOR, out);
 }
 
 int luxtts_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames) {
     const char *what = "LuxTTS mel features";
-    int st = check_class(p, what, 3, 1, 1.0f, 1);
+    int st = check_class(p, what, FA_MEL_FB_LUXTTS, FA_MEL_EDGE_REFLECT, 1.0f, 1);
     if (st != FA_OK) return st;
     // lhotse's count (:44-47).  It never exceeds the STFT's 1 + n / hop (:67), so the reference's replicate-last-frame
     // branch (:126-130) is never taken and the frames are the first T STFT frames.
@@ -302,7 +303,7 @@ int luxtts_features(MelPlan &p, const float *audio, long long n, float *out, lon
     if (frames) *frames = T;
     if (T == 0) return FA_OK;
     st = check_out(what, T * p.cfg.n_mels, out_len);
-    return st != FA_OK ? st : run_clip(p, audio, n, T, 0, out);
+    return st != FA_OK ? st : run_clip(p, audio, n, T, FA_MEL_TIME_MAJOR, out);
 }
 
 } // namespace mel

@@ -57,6 +57,7 @@ constexpr int kHalf = 256;
 constexpr int kBins = 257;
 constexpr int kFftPad = 304;      // complex values per warp buffer (max layout extent 296 + Z[0] mirror at 288)
 constexpr int kTileFrames = 16;   // frames per CTA tile; the mel stage maps 32 / kTileFrames mel bins onto one warp
+constexpr int kWarpsPerCta = 8;   // warps of a mel512_kernel CTA, for which the plan deals out the filterbank schedule
 // Power tile: one row per frame PAIR, the two frames' values of a bin side by side: row[2 * bin + slot], slot = frame & 1.
 // The float32-pair transform stores both frames of a bin with ONE 64-bit store, and the filterbank stage runs two frames
 // per lane, both multiplied by the same weight.  Row stride 524 floats = 2 x 260 bins + 4: 16-byte

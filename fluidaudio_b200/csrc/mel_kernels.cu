@@ -25,10 +25,6 @@
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <limits>
 #include <vector>
 
 namespace fa {
@@ -430,158 +426,17 @@ __global__ void __launch_bounds__(256) mel_generic_kernel(const MelLaunch P, con
 }
 
 // ------------------------------------------------------------------------------------------------ host plan
-static float swift_float_pi() {
-    const uint32_t bits = 0x40490FDAu;   // Swift's Float.pi is rounded toward zero
-    float f;
-    std::memcpy(&f, &bits, 4);
-    return f;
-}
-
-// AudioMelSpectrogram.swift:553-562
-void build_window(int length, bool periodic, std::vector<float> &w) {
-    w.resize(length);
-    const float divisor = periodic ? (float)length : (float)(length - 1);
-    const float pi = swift_float_pi();
-    for (int i = 0; i < length; ++i) {
-        const float phase = 2.0f * pi * (float)i / divisor;
-        w[i] = 0.5f * (1.0f - cosf(phase));
-    }
-}
-
-// AudioMelSpectrogram.swift:564-642 (Slaney mel scale, Slaney area normalisation, Float32 arithmetic)
-void build_filterbank(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb) {
-    const int bins = n_fft / 2 + 1;
-    const float f_sp = 200.0f / 3.0f, min_log_hz = 1000.0f;
-    const float min_log_mel = min_log_hz / f_sp;
-    const float log_step = logf(6.4f) / 27.0f;
-    auto to_mel = [&](float hz) { return hz >= min_log_hz ? min_log_mel + logf(hz / min_log_hz) / log_step : hz / f_sp; };
-    auto to_hz = [&](float mel) {
-        return mel >= min_log_mel ? min_log_hz * expf(log_step * (mel - min_log_mel)) : f_sp * mel;
-    };
-    const float mel_lo = to_mel(0.0f), mel_hi = to_mel((float)sample_rate / 2.0f);
-    std::vector<float> edge(n_mels + 2), freq(bins);
-    for (int i = 0; i < n_mels + 2; ++i) edge[i] = to_hz(mel_lo + (float)i * (mel_hi - mel_lo) / (float)(n_mels + 1));
-    for (int i = 0; i < bins; ++i) freq[i] = (float)i * (float)sample_rate / (float)n_fft;
-    fb.assign((size_t)n_mels * bins, 0.0f);
-    for (int m = 0; m < n_mels; ++m) {
-        const float l = edge[m], c = edge[m + 1], r = edge[m + 2];
-        const float norm = 2.0f / (r - l);
-        for (int b = 0; b < bins; ++b) {
-            const float f = freq[b];
-            if (f >= l && f < c) fb[(size_t)m * bins + b] = norm * (f - l) / (c - l);
-            else if (f >= c && f <= r) fb[(size_t)m * bins + b] = norm * (r - f) / (r - c);
-        }
-    }
-}
-
-// Swift's min / max on Comparable: min(x, y) = y < x ? y : x, max(x, y) = y >= x ? y : x
-template <typename T> static T swift_min(T x, T y) { return y < x ? y : x; }
-template <typename T> static T swift_max(T x, T y) { return y >= x ? y : x; }
-
-// CoherePipeline.swift:90-97: symmetric Hann, and a length-1 window is [0] (build_window would divide by zero)
-void build_window_cohere(int length, std::vector<float> &w) {
-    if (length > 1) build_window(length, false, w);
-    else w.assign(length, 0.0f);
-}
-
-// CoherePipeline.swift:273-323 (slaneyMelFilter): Float32 throughout, f_min .. f_max, 1e-10 clamped denominators
-void build_filterbank_cohere(int n_fft, int n_mels, int sample_rate, float f_min, float f_max, std::vector<float> &fb) {
-    const int bins = n_fft / 2 + 1;
-    const float f_sp = 200.0f / 3.0f, min_log_hz = 1000.0f, min_log_mel = 15.0f, log_step = 0.06875177742f;
-    auto to_mel = [&](float hz) { return hz >= min_log_hz ? min_log_mel + logf(hz / min_log_hz) / log_step : hz / f_sp; };
-    auto to_hz = [&](float mel) {
-        return mel >= min_log_mel ? min_log_hz * expf(log_step * (mel - min_log_mel)) : f_sp * mel;
-    };
-    std::vector<float> freq(bins), hz(n_mels + 2);
-    for (int k = 0; k < bins; ++k) freq[k] = (float)sample_rate * (float)k / (float)n_fft;
-    const float mel_min = to_mel(f_min), mel_max = to_mel(f_max);
-    const float step = (mel_max - mel_min) / (float)(n_mels + 1);
-    for (int i = 0; i < n_mels + 2; ++i) hz[i] = to_hz(mel_min + (float)i * step);
-    fb.assign((size_t)n_mels * bins, 0.0f);
-    for (int m = 0; m < n_mels; ++m) {
-        const float lower = hz[m], center = hz[m + 1], upper = hz[m + 2];
-        const float left_den = swift_max(center - lower, 1e-10f), right_den = swift_max(upper - center, 1e-10f);
-        float *row = &fb[(size_t)m * bins];
-        for (int k = 0; k < bins; ++k) {
-            const float f = freq[k];
-            if (f < lower || f > upper) continue;
-            row[k] = f <= center ? (f - lower) / left_den : (upper - f) / right_den;
-        }
-        const float enorm = 2.0f / swift_max(upper - lower, 1e-10f);
-        for (int k = 0; k < bins; ++k) row[k] *= enorm;
-    }
-}
-
-// StyleTTS2MelExtractor.swift:160-221 (htkMelFilterbank): HTK scale in Float32 (log10f, powf), no norm, 0 .. sr/2, bin
-// frequencies k * (sr / nFFT) for the rate the table is built for (16 kHz for StyleTTS2's 24 kHz audio)
-void build_filterbank_htk_f32(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb) {
-    const int bins = n_fft / 2 + 1;
-    auto to_mel = [](float hz) { return 2595.0f * log10f(1.0f + hz / 700.0f); };
-    auto to_hz = [](float mel) { return 700.0f * (powf(10.0f, mel / 2595.0f) - 1.0f); };
-    std::vector<float> freq(bins), hz(n_mels + 2);
-    const float bin_step = (float)sample_rate / (float)n_fft;
-    for (int k = 0; k < bins; ++k) freq[k] = (float)k * bin_step;
-    const float mel_min = to_mel(0.0f), mel_max = to_mel((float)sample_rate / 2.0f);
-    for (int i = 0; i < n_mels + 2; ++i) {
-        const float frac = (float)i / (float)(n_mels + 1);
-        hz[i] = to_hz(mel_min + (mel_max - mel_min) * frac);
-    }
-    fb.assign((size_t)n_mels * bins, 0.0f);
-    for (int m = 0; m < n_mels; ++m) {
-        const float left = hz[m], center = hz[m + 1], right = hz[m + 2];
-        const float left_slope = center - left, right_slope = right - center;
-        for (int k = 0; k < bins; ++k) {
-            const float f = freq[k];
-            if (f < left || f > right) continue;
-            float val;
-            if (f <= center) val = left_slope > 0 ? (f - left) / left_slope : 0.0f;
-            else val = right_slope > 0 ? (right - f) / right_slope : 0.0f;
-            fb[(size_t)m * bins + k] = swift_max(val, 0.0f);
-        }
-    }
-}
-
-// LuxTtsMelExtractor.swift:158-187 (torchaudio melscale_fbanks, norm nil, HTK): Double throughout, bins on
-// linspace(0, sr/2, bins), Float(max(0, min(up, down)))
-void build_filterbank_htk_f64(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb) {
-    const int bins = n_fft / 2 + 1;
-    const double f_max = (double)sample_rate / 2.0;
-    auto to_mel = [](double hz) { return 2595.0 * log10(1.0 + hz / 700.0); };
-    auto to_hz = [](double mel) { return 700.0 * (pow(10.0, mel / 2595.0) - 1.0); };
-    const double mel_min = to_mel(0.0), mel_max = to_mel(f_max);
-    std::vector<double> pts(n_mels + 2), freq(bins);
-    for (int i = 0; i < n_mels + 2; ++i) pts[i] = to_hz(mel_min + (double)i * (mel_max - mel_min) / (double)(n_mels + 1));
-    for (int b = 0; b < bins; ++b) freq[b] = (double)b * f_max / (double)(bins - 1);
-    fb.assign((size_t)n_mels * bins, 0.0f);
-    for (int m = 0; m < n_mels; ++m)
-        for (int b = 0; b < bins; ++b) {
-            const double up = (freq[b] - pts[m]) / (pts[m + 1] - pts[m]);
-            const double down = (pts[m + 2] - freq[b]) / (pts[m + 2] - pts[m + 1]);
-            fb[(size_t)m * bins + b] = (float)swift_max(0.0, swift_min(up, down));
-        }
-}
-
-int check_ex_config(const MelConfig &c) {
-    auto bad = [](const char *what) {
-        fa::set_error("mel ex config: %s", what);
-        return FA_INVALID_ARGUMENT;
-    };
-    if (c.fb_kind < 0 || c.fb_kind > 3) return bad("filterbank must be one of FA_MEL_FB_* (0..3)");
-    if (c.filter_sample_rate < 0) return bad("filter_sample_rate must be 0 (the audio's rate) or positive");
-    if (c.center_edge != 0 && c.center_edge != 1) return bad("center_edge must be FA_MEL_EDGE_ZERO or FA_MEL_EDGE_REFLECT");
-    if (!std::isfinite(c.spectrum_power) || !(c.spectrum_power > 0.0f)) return bad("spectrum_power must be finite and > 0");
-    if (!std::isfinite(c.log_mean) || !std::isfinite(c.log_std) || c.log_std == 0.0f)
-        return bad("log_mean must be finite and log_std finite and non-zero");
-    if (!std::isfinite(c.f_min) || !std::isfinite(c.f_max)) return bad("f_min and f_max must be finite");
-    if (c.fb_kind != 1 && (c.f_min != 0.0f || (c.f_max > 0.0f && c.f_max != (float)c.filter_rate() / 2.0f)))
-        return bad("f_min / f_max apply to FA_MEL_FB_COHERE only (the other tables span 0 .. filter_sample_rate / 2)");
-    if (c.reflect() && c.preemph != 0.0f)
-        return bad("FA_MEL_EDGE_REFLECT needs preemph 0 (no reference frontend pre-emphasises a reflected signal)");
-    return FA_OK;
-}
-
-static constexpr int kWarpsPerCta = 8;
 static constexpr int kCtasPerSm = 2;
+
+// the specialised kernel's variant for a precision and a layout
+typedef void (*Mel512Kernel)(const MelLaunch);
+template <typename V> static Mel512Kernel mel512_variant(int layout) {
+    return layout == FA_MEL_TIME_MAJOR ? mel512_kernel<kWarpsPerCta, V, FA_MEL_TIME_MAJOR>
+                                       : mel512_kernel<kWarpsPerCta, V, FA_MEL_MEL_MAJOR>;
+}
+static Mel512Kernel mel512_variant(int precision, int layout) {
+    return precision == FA_MEL_PRECISION_F64 ? mel512_variant<double>(layout) : mel512_variant<f32x2>(layout);
+}
 
 // the any-nFFT kernel's variant for a launch (see mel_generic_kernel)
 typedef void (*GenericKernel)(const MelLaunch, const GenericParams);
@@ -596,6 +451,13 @@ template <bool R> static GenericKernel generic_variant(int spectrum, bool affine
 static GenericKernel generic_variant(bool reflect, int spectrum, bool affine) {
     return reflect ? generic_variant<true>(spectrum, affine) : generic_variant<false>(spectrum, affine);
 }
+
+// Window placement of a mode (index of d_win_tab_mode / d_in_tab_mode / d_lane_tab): 0 centred at (nFFT - win) / 2,
+// 1 at offset 0 for the legacy compute()
+static int placement_of(int mode) { return mode == FA_MEL_LEGACY_COMPUTE ? 1 : 0; }
+static int window_offset(const MelConfig &c, int placement) { return placement == 1 ? 0 : (c.n_fft - c.win_length) / 2; }
+
+static_assert(sizeof(MelSlot) == sizeof(int4) && offsetof(MelSlot, mel) == offsetof(int4, w), "MelSlot is an int4");
 
 // Device copy of a host table (at least one element, so that an empty table still has an address).
 template <typename T, typename U> static int upload_table(DeviceBuffer<T> &b, const std::vector<U> &v) {
@@ -619,84 +481,25 @@ int MelPlan::init(const MelConfig &c) {
                       cfg.n_fft, cfg.hop_length, cfg.win_length, cfg.n_mels);
         return FA_UNSUPPORTED;
     }
-    int st = check_ex_config(cfg);
-    if (st != FA_OK) return st;
+    if (const char *why = check_ex_config(cfg)) {
+        fa::set_error("mel ex config: %s", why);
+        return FA_INVALID_ARGUMENT;
+    }
     // the specialised kernel covers every in-repo caller's shape; anything else takes mel_generic_kernel, and so do
     // reflect padding, a spectrum other than |X|^2 and the affine epilogue (mel512_kernel only ever sees another table)
     const int spectrum = spectrum_kind(cfg.spectrum_power);
     generic = cfg.n_fft != kNfft || (cfg.hop_length & 1) || cfg.hop_length > 1024 || cfg.reflect() ||
               spectrum != kSpecPower || cfg.affine();
-    const int n_fft = cfg.n_fft, bins = n_fft / 2 + 1, fr = cfg.filter_rate();
-    if (cfg.fb_kind == 1 && !cfg.window_periodic) build_window_cohere(cfg.win_length, window);
-    else build_window(cfg.win_length, cfg.window_periodic != 0, window);
-    switch (cfg.fb_kind) {
-    case 1: build_filterbank_cohere(n_fft, cfg.n_mels, fr, cfg.f_min, cfg.f_max > 0.0f ? cfg.f_max : (float)fr / 2.0f,
-                                    filterbank); break;
-    case 2: build_filterbank_htk_f32(n_fft, cfg.n_mels, fr, filterbank); break;
-    case 3: build_filterbank_htk_f64(n_fft, cfg.n_mels, fr, filterbank); break;
-    default: build_filterbank(n_fft, cfg.n_mels, fr, filterbank);
-    }
-
-    // banded filterbank: per mel the contiguous range of non-zero bins, widened with explicit zero weights to whole
-    // bin quads.  Weights are stored times 1/4 because the kernel's power tile holds 4|X|^2 (mel_core.cuh).
-    std::vector<int> lo(cfg.n_mels), hi(cfg.n_mels), off(cfg.n_mels);
-    fb_nnz = 0;
-    for (int m = 0; m < cfg.n_mels; ++m) {
-        int a = bins, b = 0;
-        for (int k = 0; k < bins; ++k)
-            if (filterbank[(size_t)m * bins + k] != 0.0f) {
-                a = std::min(a, k);
-                b = k + 1;
-            }
-        if (b == 0) a = 0;
-        a &= ~3;                       // whole bin quads: 16-byte aligned reads of the power row (pair rows, kPairStride)
-        b = (b + 3) & ~3;              // may reach 260 > 257: the tile's pad columns are zero, so are these weights
-        lo[m] = a;
-        hi[m] = b;
-        off[m] = fb_nnz;               // a multiple of four: 16-byte aligned weight quads
-        fb_nnz += b - a;
-    }
-    // filterbank-stage schedule of mel512_kernel: groups of four consecutive filters, dealt to the 8 warps longest first
-    // (cost = widest band of the group, in quads); slot = (iteration * 8 + warp) * 4 + member
-    std::vector<int4> slots;
-    {
-        const int groups = (cfg.n_mels + 3) / 4;
-        std::vector<int> cost(groups, 0), order(groups);
-        for (int g = 0; g < groups; ++g) {
-            for (int m = 4 * g; m < std::min(cfg.n_mels, 4 * g + 4); ++m) cost[g] = std::max(cost[g], (hi[m] - lo[m]) >> 2);
-            order[g] = g;
-        }
-        std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return cost[a] > cost[b]; });
-        std::vector<std::vector<int>> mine(kWarpsPerCta);
-        std::vector<long long> load(kWarpsPerCta, 0);
-        // warp 0's lane 0 also computes the next tile's geometry and issues its bulk copy in this phase: measured, that is
-        // worth more than a full share of the filterbank work (handicap 0 / 6 / 12 / 24 quads: 0.3109 / 0.3049 / 0.2996 /
-        // 0.2982 ms per audio-hour, identical output; profiles/r02_mel.md), so warp 0 only takes a group when the others
-        // are this far ahead
-        load[0] = 24;
-        for (int g : order) {
-            int best = 0;
-            for (int wv = 1; wv < kWarpsPerCta; ++wv)
-                if (load[wv] + 2 * (long long)mine[wv].size() < load[best] + 2 * (long long)mine[best].size()) best = wv;
-            mine[best].push_back(g);
-            load[best] += cost[g] + 4;   // + per-iteration control
-        }
-        size_t iters = 0;
-        for (auto &v : mine) iters = std::max(iters, v.size());
-        slots.assign(iters * kWarpsPerCta * 4, make_int4(0, 0, 0, -1));
-        for (int wv = 0; wv < kWarpsPerCta; ++wv)
-            for (size_t it = 0; it < mine[wv].size(); ++it)
-                for (int q = 0; q < 4; ++q) {
-                    const int m = 4 * mine[wv][it] + q;
-                    if (m < cfg.n_mels) slots[(it * kWarpsPerCta + wv) * 4 + q] = make_int4(lo[m], (hi[m] - lo[m]) >> 2, off[m], m);
-                }
-    }
-    n_slots = (int)slots.size();
+    const int n_fft = cfg.n_fft, bins = n_fft / 2 + 1;
+    build_tables(cfg, window, filterbank);
+    const MelBands bands = pack_bands(filterbank, cfg.n_mels, bins);
+    fb_nnz = bands.nnz;
+    n_slots = (int)bands.slots.size();
 
     int dev = 0;
     FA_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp prop;
-    st = sm90_device_props(dev, prop);
+    int st = sm90_device_props(dev, prop);
     if (st != FA_OK) return st;
     num_sms = prop.multiProcessorCount;
 
@@ -716,29 +519,13 @@ int MelPlan::init(const MelConfig &c) {
             pt_len = pt_cap = raw_cap = fb_cap = 0;
         }
     }
-    // weights packed in the order the kernel finds the bins in its power tile: mel512_kernel swizzles inside each bin quad
-    // (pow_pos, mel_core.cuh), the any-nFFT kernel keeps the natural order.  Scaled by 1/4 where the tile holds 4|X|^2.
-    const float wscale = spectrum == kSpecPower ? 0.25f : 1.0f;
-    std::vector<float> w;
-    w.reserve(fb_nnz);
-    for (int m = 0; m < cfg.n_mels; ++m)
-        for (int k = lo[m]; k < hi[m]; ++k) {
-            const int src = generic ? k : ((k & ~3) | ((k & 3) ^ ((k >> 4) & 3)));   // position k holds bin src: pow_pos is an involution
-            w.push_back(src < bins ? wscale * filterbank[(size_t)m * bins + src] : 0.0f);
-        }
 
-    std::vector<float> win_tab(n_fft, 0.0f);
-    std::vector<uint8_t> in_tab(n_fft, 0);
-    for (int mode = 0; mode < 2; ++mode) {   // 0: centred window (offset (nFFT-win)/2); 1: legacy compute(), offset 0
-        const int off_w = mode == 0 ? (cfg.n_fft - cfg.win_length) / 2 : 0;
-        std::fill(win_tab.begin(), win_tab.end(), 0.0f);
-        std::fill(in_tab.begin(), in_tab.end(), 0);
-        for (int j = 0; j < cfg.win_length; ++j) {
-            win_tab[off_w + j] = window[j];
-            in_tab[off_w + j] = 1;
-        }
-        st = upload_table(d_win_tab_mode[mode], win_tab);
-        if (st == FA_OK) st = upload_table(d_in_tab_mode[mode], in_tab);
+    std::vector<float> win_tab;
+    std::vector<uint8_t> in_tab;
+    for (int pl = 0; pl < 2; ++pl) {
+        place_window(window, n_fft, window_offset(cfg, pl), win_tab, in_tab);
+        st = upload_table(d_win_tab_mode[pl], win_tab);
+        if (st == FA_OK) st = upload_table(d_in_tab_mode[pl], in_tab);
         if (st != FA_OK) return st;
         if (!generic) {
             std::vector<LaneTables<double>> t64(32);
@@ -747,16 +534,18 @@ int MelPlan::init(const MelConfig &c) {
                 load_lane_tables(l, win_tab.data(), in_tab.data(), t64[l]);
                 load_lane_tables(l, win_tab.data(), in_tab.data(), t32[l]);
             }
-            st = upload_table(d_lane_tab[mode][0], t64);
-            if (st == FA_OK) st = upload_table(d_lane_tab[mode][1], t32);
+            st = upload_table(d_lane_tab[pl][FA_MEL_PRECISION_F64], t64);
+            if (st == FA_OK) st = upload_table(d_lane_tab[pl][FA_MEL_PRECISION_F32], t32);
             if (st != FA_OK) return st;
         }
     }
-    st = upload_table(d_fb_w, w);
-    if (st == FA_OK) st = upload_table(d_fb_slots, slots);
-    if (st == FA_OK) st = upload_table(d_fb_lo, lo);
-    if (st == FA_OK) st = upload_table(d_fb_hi, hi);
-    if (st == FA_OK) st = upload_table(d_fb_off, off);
+    // mel512_kernel finds the bins of a quad swizzled in its power tile, the any-nFFT kernel in natural order; the
+    // weights carry 1/4 where the tile holds 4|X|^2
+    st = upload_table(d_fb_w, pack_weights(filterbank, bands, bins, !generic, spectrum == kSpecPower ? 0.25f : 1.0f));
+    if (st == FA_OK) st = upload_table(d_fb_slots, bands.slots);
+    if (st == FA_OK) st = upload_table(d_fb_lo, bands.lo);
+    if (st == FA_OK) st = upload_table(d_fb_hi, bands.hi);
+    if (st == FA_OK) st = upload_table(d_fb_off, bands.off);
     for (auto &s : streams)
         if (st == FA_OK) st = s.create();
     if (st != FA_OK) return st;
@@ -784,23 +573,20 @@ int MelPlan::init(const MelConfig &c) {
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
         return FA_OK;
     }
-    FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, double, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, double, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, f32x2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    FA_CUDA_TRY(cudaFuncSetAttribute(mel512_kernel<kWarpsPerCta, f32x2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    for (const int precision : {FA_MEL_PRECISION_F64, FA_MEL_PRECISION_F32})
+        for (const int layout : {FA_MEL_TIME_MAJOR, FA_MEL_MEL_MAJOR})
+            FA_CUDA_TRY(cudaFuncSetAttribute(mel512_variant(precision, layout), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)smem_bytes));
     return FA_OK;
 }
 
 long long MelPlan::frame_count(long long n, int mode, long long expected) const {
     long long computed;   // C++ integer division truncates toward zero exactly like Swift's Int '/'
-    if (mode == 0) computed = 1 + (n + 2 * (long long)(cfg.n_fft / 2) - cfg.win_length) / cfg.hop_length;
-    else if (mode == 1) computed = std::max<long long>(0, (n - cfg.n_fft) / cfg.hop_length + 1);
+    if (mode == FA_MEL_PAD_CENTER) computed = 1 + (n + 2 * (long long)(cfg.n_fft / 2) - cfg.win_length) / cfg.hop_length;
+    else if (mode == FA_MEL_PAD_PREPADDED) computed = std::max<long long>(0, (n - cfg.n_fft) / cfg.hop_length + 1);
     else computed = 1 + (n - cfg.win_length) / cfg.hop_length;
     return expected >= 0 ? expected : computed;
 }
-
-// bytes of the unit descriptors of a call with `count` units
-static size_t unit_bytes(int count) { return (size_t)std::max(count, 64) * sizeof(MelUnit); }
 
 int MelPlan::ensure_staging(size_t audio_floats, size_t out_floats) {
     const int st = d_audio.grow(audio_floats * sizeof(float));
@@ -817,8 +603,20 @@ int MelPlan::ensure_events(size_t count) {
     return FA_OK;
 }
 
+static int tiles_of(long long frames) { return (int)((frames + kTileFrames - 1) / kTileFrames); }
+
+int number_tiles(MelUnit *u, int count) {
+    int tiles = 0;
+    for (int i = 0; i < count; ++i) {
+        u[i].tile_begin = tiles;
+        tiles += tiles_of(u[i].frame_count);
+    }
+    return tiles;
+}
+
 int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inline_unit, const float *d_audio_base,
-                    float *d_out_base, int total_tiles, int mode, int layout, cudaStream_t stream, bool aligned16) {
+                    float *d_out_base, int mode, int layout, cudaStream_t stream) {
+    const int total_tiles = count > 0 ? h_u[count - 1].tile_begin + tiles_of(h_u[count - 1].frame_count) : 0;
     if (total_tiles <= 0) return FA_OK;
     MelLaunch P{};
     P.audio = d_audio_base;
@@ -829,8 +627,8 @@ int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inli
     if (P.inline_unit) P.unit0 = h_u[0];
     P.total_tiles = total_tiles;
     P.hop = cfg.hop_length;
-    P.pad = mode == 0 ? cfg.n_fft / 2 : 0;
-    P.preemph = mode == 2 ? 0.0f : cfg.preemph;
+    P.pad = mode == FA_MEL_PAD_CENTER ? cfg.n_fft / 2 : 0;
+    P.preemph = mode == FA_MEL_LEGACY_COMPUTE ? 0.0f : cfg.preemph;
     P.n_mels = cfg.n_mels;
     P.log_floor = cfg.log_floor;
     P.log_clamped = cfg.log_floor_mode;
@@ -841,9 +639,10 @@ int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inli
     for (int i = 0; i < count && P.out_vec4; ++i) P.out_vec4 = (h_u[i].out_off & 3) == 0;
     P.log_normal = cfg.log_floor >= 1e-37f ? 1 : 0;   // mel energies are >= 0: log's argument is then never a denormal
     P.layout = layout;
-    P.lane_tab = d_lane_tab[mode == 2 ? 1 : 0][precision == 1 ? 1 : 0].data();
-    P.win_tab = d_win_tab_mode[mode == 2 ? 1 : 0].data();
-    P.in_tab = d_in_tab_mode[mode == 2 ? 1 : 0].data();
+    const int pl = placement_of(mode);
+    P.lane_tab = d_lane_tab[pl][precision == FA_MEL_PRECISION_F32 ? 1 : 0].data();
+    P.win_tab = d_win_tab_mode[pl].data();
+    P.in_tab = d_in_tab_mode[pl].data();
     P.fb_w = d_fb_w.data();
     P.fb_slots = d_fb_slots.data();
     P.n_slots = n_slots;
@@ -855,9 +654,12 @@ int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inli
     P.pt_len = pt_len;
     P.pt_cap = pt_cap;
     P.raw_cap = raw_cap;
-    P.use_tma = aligned16 ? 1 : 0;
+    // the bulk copy moves whole 16-byte runs of a unit's samples (tile_geom): the audio base must be 16-byte aligned and
+    // every unit must start at a multiple of four floats, or every sample takes the read-only path
+    P.use_tma = (reinterpret_cast<uintptr_t>(d_audio_base) & 15) == 0;
+    for (int i = 0; i < count && P.use_tma; ++i) P.use_tma = (h_u[i].audio_off & 3) == 0;
     {
-        const int off_w = mode == 2 ? 0 : (cfg.n_fft - cfg.win_length) / 2;
+        const int off_w = window_offset(cfg, pl);
         P.mid_full = (off_w <= 64 && off_w + cfg.win_length >= 448) ? 1 : 0;
     }
     P.inv_n_mels = (unsigned)((0x100000000ull + (unsigned)cfg.n_mels - 1) / (unsigned)cfg.n_mels);
@@ -866,38 +668,31 @@ int MelPlan::launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inli
                         static_cast<const cpxd *>(d_generic_tw.data()), generic_warps, cfg.spectrum_power, cfg.log_mean,
                         cfg.log_std};
         const int ggrid = std::min(total_tiles, num_sms * std::max(1, 16 / generic_warps));
-        const GenericKernel kernel = generic_variant(mode == 0 && cfg.reflect(), spectrum_kind(cfg.spectrum_power),
-                                                     cfg.affine());
+        const GenericKernel kernel = generic_variant(mode == FA_MEL_PAD_CENTER && cfg.reflect(),
+                                                     spectrum_kind(cfg.spectrum_power), cfg.affine());
         FA_CUDA_TRY(fa::launch(kernel, ggrid, generic_warps * 32, smem_bytes, stream, P, G));
         return FA_OK;
     }
     const int grid = std::min(total_tiles, num_sms * kCtasPerSm);
     const dim3 blk(kWarpsPerCta * 32);
-    auto kernel = precision == 1 ? (layout == 0 ? mel512_kernel<kWarpsPerCta, f32x2, 0> : mel512_kernel<kWarpsPerCta, f32x2, 1>)
-                                 : (layout == 0 ? mel512_kernel<kWarpsPerCta, double, 0> : mel512_kernel<kWarpsPerCta, double, 1>);
-    FA_CUDA_TRY(fa::launch(kernel, grid, blk, smem_bytes, stream, P));
+    FA_CUDA_TRY(fa::launch(mel512_variant(precision, layout), grid, blk, smem_bytes, stream, P));
     return FA_OK;
 }
-
-static inline long long ceil_to(long long v, long long m) { return ((v + m - 1) / m) * m; }
-static inline int tiles_of(long long frames) { return (int)((frames + kTileFrames - 1) / kTileFrames); }
 
 // Shape rules shared by every entry point.  Returns false for the reference's "empty" guard
 // (AudioMelSpectrogram.swift:135-137, :199-201, :349-351).
 static bool shape_of(const MelPlan &p, long long n, int mode, long long expected, long long &T, long long &Tp) {
-    T = p.frame_count(n, mode, mode == 0 || mode == 1 ? expected : -1);
+    T = p.frame_count(n, mode, mode == FA_MEL_PAD_CENTER || mode == FA_MEL_PAD_PREPADDED ? expected : -1);
     if (T <= 0 || n <= 0) return false;
-    Tp = mode == 2 ? T : ceil_to(T, p.cfg.pad_to);
+    Tp = mode == FA_MEL_LEGACY_COMPUTE ? T : ceil_to(T, p.cfg.pad_to);
     return true;
 }
 
-// Output shape of one clip, reported through mel_length / num_frames: T frames computed, Tp rows returned.  Empty input
-// gives T = 0 and one pad row (none in mode 2), which the caller zeroes.  Fails when out_len floats cannot hold Tp rows.
-static int clip_shape(const MelPlan &p, long long n, int mode, long long expected, long long out_len, long long &T,
-                      long long &Tp, long long *mel_length, long long *num_frames) {
+int clip_shape(const MelPlan &p, long long n, int mode, long long expected, long long out_len, long long &T,
+               long long &Tp, long long *mel_length, long long *num_frames) {
     if (!shape_of(p, n, mode, expected, T, Tp)) {
         T = 0;
-        Tp = mode == 2 ? 0 : 1;
+        Tp = mode == FA_MEL_LEGACY_COMPUTE ? 0 : 1;
     }
     if (mel_length) *mel_length = T;
     if (num_frames) *num_frames = Tp;
@@ -907,7 +702,6 @@ static int clip_shape(const MelPlan &p, long long n, int mode, long long expecte
     }
     return FA_OK;
 }
-static constexpr long long kUnchecked = std::numeric_limits<long long>::max();   // batch calls take no output lengths
 
 int MelPlan::compute_device(const float *d_in, long long n, float last, int mode, long long expected, int layout,
                             float *d_out_buf, long long out_len, long long *mel_length, long long *num_frames,
@@ -925,9 +719,7 @@ int MelPlan::compute_device(const float *d_in, long long n, float last, int mode
     units.host.data()[0] = MelUnit{0, n, 0, Tp, 0, T, last, 0};
     st = units.upload(sizeof(MelUnit), stream);
     if (st != FA_OK) return st;
-    const bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
-    return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, tiles_of(T), mode, layout, stream,
-                  aligned);
+    return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, mode, layout, stream);
 }
 
 int MelPlan::launch_clip(const float *d_in, long long n, long long T, int layout, float *d_out_buf, cudaStream_t stream) {
@@ -937,9 +729,7 @@ int MelPlan::launch_clip(const float *d_in, long long n, long long T, int layout
     units.host.data()[0] = MelUnit{0, n, 0, T, 0, T, 0.0f, 0};
     st = units.upload(sizeof(MelUnit), stream);
     if (st != FA_OK) return st;
-    const bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
-    return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, tiles_of(T), 0, layout, stream,
-                  aligned);
+    return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, FA_MEL_PAD_CENTER, layout, stream);
 }
 
 int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, int count, const float *last, int mode,
@@ -948,8 +738,7 @@ int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, i
     int st = units.reserve(unit_bytes(count));
     if (st != FA_OK) return st;
     MelUnit *h_units = units.host.data();
-    int tiles = 0, used = 0;
-    bool aligned = (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;
+    int used = 0;
     for (int i = 0; i < count; ++i) {
         const long long n = offsets[i + 1] - offsets[i];
         long long T, Tp;
@@ -960,332 +749,13 @@ int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, i
             continue;
         }
         if (Tp > T) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf + out_offsets[i], 0, Tp * cfg.n_mels * sizeof(float), stream));
-        if (offsets[i] & 3) aligned = false;
-        h_units[used] = MelUnit{offsets[i], n, out_offsets[i], Tp, 0, T, last ? last[i] : 0.0f, tiles};
-        tiles += tiles_of(T);
-        ++used;
+        h_units[used++] = MelUnit{offsets[i], n, out_offsets[i], Tp, 0, T, last ? last[i] : 0.0f, 0};
     }
     if (!used) return FA_OK;
+    number_tiles(h_units, used);
     st = units.upload(used * sizeof(MelUnit), stream);
     if (st != FA_OK) return st;
-    return launch(units.device.data(), h_units, used, false, d_in, d_out_buf, tiles, mode, layout, stream, aligned);
-}
-
-// A pinned (page-locked, mapped) host buffer has a device alias under UVA: the kernel can then store its output rows
-// straight into host memory (coalesced 16-byte stores become posted PCIe writes), which removes the D2H copy stage and its
-// cross-stream hand-offs from the pipeline.  Pageable memory returns nullptr and takes the staged copy.
-static float *device_alias_if_pinned(float *host) {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, host) != cudaSuccess) {
-        cudaGetLastError();
-        return nullptr;
-    }
-    return (a.type == cudaMemoryTypeHost && a.devicePointer) ? static_cast<float *>(a.devicePointer) : nullptr;
-}
-
-// FA_MEL_TRACE_PIPELINE=1: device timestamps (timing events) at the end of every unit's H2D, kernels and D2H of the
-// host-buffer pipeline (MelPlan::compute_host), printed to stderr after the call.  Off: no events, no cost.
-struct PipelineTrace {
-    bool on = false;
-    Event t0;
-    std::vector<Event> ev;
-    std::vector<int> tag;   // unit * 4 + stage (0 H2D done, 1 kernels done, 2 D2H done)
-    PipelineTrace() {
-        static const bool want = [] { const char *e = std::getenv("FA_MEL_TRACE_PIPELINE"); return e && *e && *e != '0'; }();
-        on = want;
-    }
-    void start(cudaStream_t s) {
-        if (!on) return;
-        t0.create();
-        cudaEventRecord(t0, s);
-    }
-    void mark(cudaStream_t s, int unit, int stage) {
-        if (!on) return;
-        ev.emplace_back();
-        ev.back().create();
-        cudaEventRecord(ev.back(), s);
-        tag.push_back(unit * 4 + stage);
-    }
-    void dump(const char *what) {
-        if (!on) return;
-        static const char *names[3] = {"h2d", "kern", "d2h"};
-        std::fprintf(stderr, "[pipeline %s]", what);
-        for (size_t i = 0; i < ev.size(); ++i) {
-            float ms = 0.0f;
-            cudaEventElapsedTime(&ms, t0, ev[i]);
-            std::fprintf(stderr, " u%d.%s=%.3f", tag[i] / 4, names[tag[i] & 3], ms);
-        }
-        std::fprintf(stderr, "\n");
-    }
-};
-
-// Frame ranges of the pipeline's units.  The pipeline's fixed cost is its ramp: nothing can be computed before the first
-// unit's samples have landed, and the last unit's kernel + D2H run after the last byte of input.  So the units at both ends
-// are small (1 : 2 : 4 ... 4 : 2 : 1) and the ones in between large enough to amortise the per-transfer cost.  Bounds are
-// multiples of the tile height; no unit is shorter than min_unit frames (fewer units otherwise).
-static std::vector<long long> unit_bounds(long long T, long long max_units, long long min_unit) {
-    std::vector<long long> b{0};
-    long long K = std::max<long long>(1, std::min(max_units, T / std::max<long long>(1, min_unit)));
-    auto weight = [&](long long c, long long k) -> long long {
-        if (k < 6) return 4;
-        const long long e = std::min(c, k - 1 - c);
-        return e == 0 ? 1 : (e == 1 ? 2 : 4);
-    };
-    for (; K > 1; --K) {   // the smallest unit must still hold min_unit frames
-        long long sum = 0;
-        for (long long c = 0; c < K; ++c) sum += weight(c, K);
-        if (T * weight(0, K) / sum >= min_unit) break;
-    }
-    long long sum = 0, acc = 0;
-    for (long long c = 0; c < K; ++c) sum += weight(c, K);
-    for (long long c = 0; c + 1 < K; ++c) {
-        acc += weight(c, K);
-        const long long e = std::min(T, ceil_to((long long)((double)T * (double)acc / (double)sum), kTileFrames));
-        if (e > b.back() && e < T) b.push_back(e);
-    }
-    b.push_back(T);
-    return b;
-}
-
-int MelPlan::ensure_resampler(double in_rate, double out_rate) {
-    if (in_rate == out_rate || (in_rate == rs_in && out_rate == rs_out && d_rs_tab.data())) return FA_OK;
-    resample::Design d;
-    int st = resample::make_design(in_rate, out_rate, d);
-    if (st != FA_OK) return st;
-    rs_in = rs_out = 0.0;   // the table is being replaced
-    st = d_rs_tab.grow(d.table.size() * sizeof(float));
-    if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpy(d_rs_tab.data(), d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice));
-    rs_design = std::move(d);
-    rs_in = in_rate;
-    rs_out = out_rate;
-    return FA_OK;
-}
-
-// Host buffers in, host buffers out: AudioConverter.resample + computeFlatTransposed as one device pipeline.  A long
-// clip is cut into units.  The PCM is copied in chunks; as soon as a chunk has landed the compute stream converts the
-// samples it completes (mixdown + polyphase / linear, see resample_kernels.cu) into the float buffer the mel kernel
-// reads, runs the frames those samples complete, and the D2H stream returns their rows — H2D of unit c+1, kernels of
-// unit c and D2H of unit c-1 overlap.  Identity input (mono float32 at the model rate) is copied straight into the float
-// buffer and needs no conversion kernel.
-int MelPlan::compute_host(const void *pcm, long long frames, const resample::AudioFormat &f, float last, int mode,
-                          long long expected, int layout, float *out, long long out_len, long long *mel_length,
-                          long long *num_frames, long long *resampled) {
-    const long long n = resample::output_count(frames, f.in_rate, f.out_rate);
-    if (resampled) *resampled = n;
-    long long T, Tp;
-    int st = clip_shape(*this, n, mode, expected, out_len, T, Tp, mel_length, num_frames);
-    if (st != FA_OK) return st;
-    if (T == 0) {
-        if (Tp) std::fill(out, out + cfg.n_mels, 0.0f);   // padValue
-        return FA_OK;
-    }
-    const bool identity = resample::is_identity(f);
-    const long long need = Tp * cfg.n_mels;
-    st = ensure_resampler(f.in_rate, f.out_rate);
-    if (st != FA_OK) return st;
-    st = ensure_staging((size_t)n + 8, (size_t)need);
-    if (st != FA_OK) return st;
-    const size_t bps = f.format == resample::kPcmI16 ? 2 : 4;
-    const size_t pcm_bytes = (size_t)frames * f.channels * bps;
-    float *const d_f32 = d_audio.data(), *const d_rows = d_out.data();   // kernel input, staged output
-    char *d_in = reinterpret_cast<char *>(d_f32);   // where the input lands
-    if (!identity) {
-        st = d_pcm.grow(pcm_bytes + 16);
-        if (st != FA_OK) return st;
-        d_in = static_cast<char *>(d_pcm.data());
-    }
-    // Units: pipeline_chunks for identity input; converted input keeps ~10 MB of PCM per unit (the copy engines' fixed
-    // cost per transfer and the host's enqueue rate make finer units slower there: int16 hour 3.08 ms at 8-12 units,
-    // 3.44 at 24, 3.61 at 96).
-    const long long max_units =
-        identity ? pipeline_chunks : std::min<long long>(pipeline_chunks, (long long)(pcm_bytes / (10u << 20)) + 1);
-    const std::vector<long long> bounds = unit_bounds(T, max_units, 4096);
-    const int chunks = (int)bounds.size() - 1;
-    // A single unit is the streaming callers' shape (a few thousand samples, SortformerDiarizer.swift:857-905): nothing
-    // to overlap, so one stream, no events, the unit descriptor passed in the kernel parameters, one synchronisation.
-    const bool single = chunks == 1;
-    float *out_alias = (zero_copy_out && layout == 0 && !single) ? device_alias_if_pinned(out) : nullptr;
-    float *k_out = out_alias ? out_alias : d_rows;   // where the kernel writes
-    if (out_alias && Tp > T) std::memset(out + T * cfg.n_mels, 0, (size_t)(Tp - T) * cfg.n_mels * sizeof(float));
-    st = units.reserve(unit_bytes(chunks));
-    if (st != FA_OK) return st;
-    st = ensure_events(2 * (size_t)chunks);
-    if (st != FA_OK) return st;
-    cudaStream_t s_k = streams[1], s_in = single ? s_k : streams[0], s_out = single ? s_k : streams[2];
-    MelUnit *h_units = units.host.data();
-    for (int c = 0; c < chunks; ++c) h_units[c] = MelUnit{0, n, 0, Tp, bounds[c], bounds[c + 1] - bounds[c], last, 0};
-    if (!single) {
-        st = units.upload(chunks * sizeof(MelUnit), s_k);
-        if (st != FA_OK) return st;
-    }
-    const long long pad = mode == 0 ? cfg.n_fft / 2 : 0;
-    const resample::Design &D = rs_design;
-    const bool linear = f.in_rate != f.out_rate && resample::resolve_algorithm(f) == resample::kAlgoLinear;
-    long long in_copied = 0, converted = 0;
-    PipelineTrace trace;
-    trace.start(s_in);
-    for (int c = 0; c < chunks; ++c) {
-        const bool tail = c == chunks - 1;
-        // model-rate samples needed so far, and the input frames those samples depend on
-        long long s_end = tail ? n : std::min(n, (bounds[c + 1] - 1) * cfg.hop_length + cfg.n_fft - pad);
-        // Reflected .center frames read the clip's end only when they cross it (then s_end = n already), and a frame
-        // crossing the start reads up to x[pad] (reflect_index): every unit's range must hold that sample.
-        if (mode == 0 && cfg.reflect()) s_end = std::min(n, std::max(s_end, pad + 1));
-        long long in_need = frames;
-        if (!tail) {
-            if (f.in_rate == f.out_rate) in_need = s_end;
-            else if (linear) in_need = (long long)((double)(s_end + 1) * (f.in_rate / f.out_rate)) + 4;
-            else in_need = ((s_end + 2) * D.M) / D.L + D.half + 3;
-            in_need = std::min(frames, std::max(in_need, in_copied));
-        }
-        if (in_need > in_copied) {
-            const char *src = static_cast<const char *>(pcm);
-            if (f.interleaved || f.channels == 1) {
-                const size_t a = (size_t)in_copied * f.channels * bps, b = (size_t)in_need * f.channels * bps;
-                FA_CUDA_TRY(cudaMemcpyAsync(d_in + a, src + a, b - a, cudaMemcpyHostToDevice, s_in));
-            } else {
-                for (int ch = 0; ch < f.channels; ++ch) {
-                    const size_t a = ((size_t)ch * frames + in_copied) * bps, b = ((size_t)ch * frames + in_need) * bps;
-                    FA_CUDA_TRY(cudaMemcpyAsync(d_in + a, src + a, b - a, cudaMemcpyHostToDevice, s_in));
-                }
-            }
-            in_copied = in_need;
-        }
-        // zero the pad rows after the first input copy: a copy from pageable memory first waits for its stream's queue
-        if (c == 0 && Tp > T && !out_alias) FA_CUDA_TRY(cudaMemsetAsync(d_rows, 0, need * sizeof(float), s_k));
-        if (!single) {
-            FA_CUDA_TRY(cudaEventRecord(events[2 * c], s_in));
-            FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * c], 0));
-        }
-        trace.mark(s_in, c, 0);
-        if (!identity) {
-            const long long ready = resample::outputs_ready(f, D, frames, in_copied, n);
-            if (ready < s_end) {
-                fa::set_error("internal: resampler window accounting (%lld < %lld)", ready, s_end);
-                return FA_RUNTIME_ERROR;
-            }
-            st = resample::launch_convert(d_pcm.data(), frames, f, D, d_rs_tab.data(), d_f32, converted, s_end, s_k);
-            if (st != FA_OK) return st;
-            converted = std::max(converted, s_end);
-        }
-        st = launch(units.device.data() + c, h_units + c, 1, single, d_f32, k_out, tiles_of(bounds[c + 1] - bounds[c]),
-                    mode, layout, s_k, true);
-        if (st != FA_OK) return st;
-        trace.mark(s_k, c, 1);
-        if (out_alias) continue;   // the kernel stored its rows in the caller's pinned buffer: no D2H stage
-        if (!single) {
-            FA_CUDA_TRY(cudaEventRecord(events[2 * c + 1], s_k));
-            FA_CUDA_TRY(cudaStreamWaitEvent(s_out, events[2 * c + 1], 0));
-        }
-        const long long fb = bounds[c], rows = (tail ? Tp : bounds[c + 1]) - fb;   // the last unit also returns the pad rows
-        if (layout == 0 || single) {   // a single unit returns the whole buffer in either layout
-            FA_CUDA_TRY(cudaMemcpyAsync(out + fb * cfg.n_mels, d_rows + fb * cfg.n_mels, rows * cfg.n_mels * sizeof(float),
-                                        cudaMemcpyDeviceToHost, s_out));
-        } else {
-            FA_CUDA_TRY(cudaMemcpy2DAsync(out + fb, Tp * sizeof(float), d_rows + fb, Tp * sizeof(float),
-                                          rows * sizeof(float), cfg.n_mels, cudaMemcpyDeviceToHost, s_out));
-        }
-        trace.mark(s_out, c, 2);
-    }
-    FA_CUDA_TRY(cudaStreamSynchronize(s_out));
-    if (!single) FA_CUDA_TRY(cudaStreamSynchronize(s_k));
-    trace.dump(identity ? "f32" : "pcm");
-    return FA_OK;
-}
-
-// Batch of clips, host buffers: clips are grouped so that copies and kernels of successive groups overlap.
-int MelPlan::compute_batch_host(const float *audio, const long long *offsets, int count, const float *last, int mode,
-                                int layout, float *out, const long long *out_offsets, long long *mel_lengths,
-                                long long *num_frames) {
-    if (count <= 0) return FA_OK;
-    // device-side packing: clip i starts at a 4-float aligned offset so that every tile can use the TMA path
-    // When every clip already starts at a multiple of four floats in the caller's buffer, the device copy keeps the
-    // caller's layout and a whole group of clips travels in ONE transfer (a bulk copy may read up to three floats past a
-    // clip's end: the neighbour's samples or the pad below, never used: the kernel masks by the clip length).  512 clips
-    // cost 1 024 cudaMemcpyAsync calls otherwise: ~4 ms of host enqueue time on a 25 ms batch.
-    bool same_layout = true;
-    for (int i = 0; i < count; ++i) same_layout = same_layout && ((offsets[i] - offsets[0]) & 3) == 0 && offsets[i + 1] >= offsets[i];
-    std::vector<long long> doff(count + 1), dout(count + 1);
-    long long a = 0, o = 0;
-    std::vector<long long> Ts(count), Tps(count);
-    for (int i = 0; i < count; ++i) {
-        const long long n = offsets[i + 1] - offsets[i];
-        doff[i] = same_layout ? offsets[i] - offsets[0] : a;
-        a = same_layout ? ceil_to(offsets[i + 1] - offsets[0], 4) + 4 : a + ceil_to(n, 4) + 4;
-        dout[i] = o;
-        clip_shape(*this, n, mode, -1, kUnchecked, Ts[i], Tps[i], mel_lengths ? mel_lengths + i : nullptr,
-                   num_frames ? num_frames + i : nullptr);
-        o += std::max<long long>(Tps[i], 1) * cfg.n_mels;   // an empty clip returns one zero row, in every mode
-    }
-    doff[count] = a;
-    dout[count] = o;
-    int st = ensure_staging((size_t)a + 8, (size_t)o);
-    if (st != FA_OK) return st;
-    st = units.reserve(unit_bytes(count));
-    if (st != FA_OK) return st;
-    const int groups = std::min(count, 32);   // one H2D, one launch, one D2H per group: the last group's kernel + D2H is the pipeline's tail
-    st = ensure_events(2 * (size_t)groups);
-    if (st != FA_OK) return st;
-    cudaStream_t s_in = streams[0], s_k = streams[1], s_out = streams[2];
-    // all unit descriptors first (one small copy), then per group: H2D, kernel, D2H
-    MelUnit *h_units = units.host.data();
-    std::vector<int> g_first(groups + 1), g_units(groups + 1, 0), g_tiles(groups, 0);
-    int used = 0;
-    for (int g = 0; g < groups; ++g) {
-        const int c0 = (int)((long long)count * g / groups), c1 = (int)((long long)count * (g + 1) / groups);
-        g_first[g] = used;
-        int tiles = 0;
-        for (int i = c0; i < c1; ++i) {
-            if (!Ts[i]) continue;
-            h_units[used] = MelUnit{doff[i], offsets[i + 1] - offsets[i], dout[i], Tps[i], 0, Ts[i], last ? last[i] : 0.0f, tiles};
-            tiles += tiles_of(Ts[i]);
-            ++used;
-        }
-        g_tiles[g] = tiles;
-    }
-    g_first[groups] = used;
-    if (used) {
-        st = units.upload(used * sizeof(MelUnit), s_k);
-        if (st != FA_OK) return st;
-    }
-    float *const d_f32 = d_audio.data(), *const d_rows = d_out.data();
-    FA_CUDA_TRY(cudaMemsetAsync(d_rows, 0, (size_t)o * sizeof(float), s_k));
-    for (int g = 0; g < groups; ++g) {
-        const int c0 = (int)((long long)count * g / groups), c1 = (int)((long long)count * (g + 1) / groups);
-        if (same_layout) {
-            const long long n = offsets[c1] - offsets[c0];
-            if (n > 0)
-                FA_CUDA_TRY(cudaMemcpyAsync(d_f32 + doff[c0], audio + offsets[c0], n * sizeof(float), cudaMemcpyHostToDevice, s_in));
-        } else {
-            for (int i = c0; i < c1; ++i) {
-                const long long n = offsets[i + 1] - offsets[i];
-                if (n > 0)
-                    FA_CUDA_TRY(cudaMemcpyAsync(d_f32 + doff[i], audio + offsets[i], n * sizeof(float), cudaMemcpyHostToDevice, s_in));
-            }
-        }
-        FA_CUDA_TRY(cudaEventRecord(events[2 * g], s_in));
-        FA_CUDA_TRY(cudaStreamWaitEvent(s_k, events[2 * g], 0));
-        st = launch(units.device.data() + g_first[g], h_units + g_first[g], g_first[g + 1] - g_first[g], false, d_f32, d_rows,
-                    g_tiles[g], mode, layout, s_k, true);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaEventRecord(events[2 * g + 1], s_k));
-        FA_CUDA_TRY(cudaStreamWaitEvent(s_out, events[2 * g + 1], 0));
-        bool out_contiguous = c1 > c0;   // the caller's output offsets follow the packed device layout: one transfer
-        for (int i = c0; i < c1 && out_contiguous; ++i) out_contiguous = out_offsets[i] - out_offsets[c0] == dout[i] - dout[c0];
-        if (out_contiguous) {
-            FA_CUDA_TRY(cudaMemcpyAsync(out + out_offsets[c0], d_rows + dout[c0], (dout[c1] - dout[c0]) * sizeof(float),
-                                        cudaMemcpyDeviceToHost, s_out));
-        } else {
-            for (int i = c0; i < c1; ++i) {
-                const long long len = dout[i + 1] - dout[i];
-                FA_CUDA_TRY(cudaMemcpyAsync(out + out_offsets[i], d_rows + dout[i], len * sizeof(float), cudaMemcpyDeviceToHost, s_out));
-            }
-        }
-    }
-    FA_CUDA_TRY(cudaStreamSynchronize(s_out));
-    FA_CUDA_TRY(cudaStreamSynchronize(s_k));
-    return FA_OK;
+    return launch(units.device.data(), h_units, used, false, d_in, d_out_buf, mode, layout, stream);
 }
 
 } // namespace mel

@@ -1,50 +1,19 @@
-// Host-side plan + launch descriptors of the fused log-mel kernel (see mel_kernels.cu).
+// Host-side plan + launch descriptors of the fused log-mel kernel: the kernels, init, launch and the device entry points
+// are in mel_kernels.cu, the host-buffer pipelines in mel_pipeline.cu, the tables the plan uploads in mel_tables.cpp.
 #pragma once
 
 #include "fa_common.cuh"
+#include "mel_tables.h"
 #include "resample_plan.h"
 #include <cuda_runtime.h>
+#include <algorithm>
+#include <limits>
 #include <vector>
 
 namespace fa {
 namespace mel {
 
 struct cpx;
-
-// Mirrors the parameters of AudioMelSpectrogram.init (AudioMelSpectrogram.swift:59-70).
-struct MelConfig {
-    int32_t sample_rate;
-    int32_t n_mels;
-    int32_t n_fft;
-    int32_t hop_length;
-    int32_t win_length;
-    float preemph;
-    int32_t pad_to;
-    float log_floor;
-    int32_t log_floor_mode;    // 0 additive log(x + floor), 1 clamped log(max(x, floor))
-    int32_t window_periodic;
-    // fa_mel_ex_config (fa_mel_create_ex); the defaults are fa_mel_create's behaviour
-    int32_t fb_kind = 0;              // FA_MEL_FB_*
-    int32_t filter_sample_rate = 0;   // 0 = sample_rate
-    float f_min = 0.0f, f_max = 0.0f;
-    int32_t center_edge = 0;          // FA_MEL_EDGE_*
-    float spectrum_power = 2.0f;
-    float log_mean = 0.0f, log_std = 1.0f;
-
-    int filter_rate() const { return filter_sample_rate > 0 ? filter_sample_rate : sample_rate; }
-    bool reflect() const { return center_edge == 1; }
-    bool affine() const { return log_mean != 0.0f || log_std != 1.0f; }
-    // every ex field as fa_mel_create leaves it: the streams and the NeMo adapters accept only such handles
-    bool neutral() const {
-        return fb_kind == 0 && filter_rate() == sample_rate && f_min == 0.0f && f_max <= 0.0f && center_edge == 0 &&
-               spectrum_power == 2.0f && !affine();
-    }
-};
-
-// Spectrum the any-nFFT kernel feeds its filterbank: |X|^2 (the power tile holds 4|X|^2, the weights carry 1/4),
-// |X| or |X|^p (the tile holds the value itself, the weights are unscaled).
-enum { kSpecPower = 0, kSpecMagnitude = 1, kSpecGeneral = 2 };
-inline int spectrum_kind(float p) { return p == 2.0f ? kSpecPower : (p == 1.0f ? kSpecMagnitude : kSpecGeneral); }
 
 // One unit of work = a run of frames of one clip.  A long clip is cut into several units so that H2D copies,
 // kernels and D2H copies of successive units overlap; a batch of clips is simply many units in one launch.
@@ -101,7 +70,7 @@ struct MelPlan {
     int pt_len = 0, pt_cap = 0, raw_cap = 0;
     size_t smem_bytes = 0;
     int num_sms = 0;
-    int precision = 0;               // transform arithmetic: 0 = FP64 (one frame per warp), 1 = float32 frame pairs
+    int precision = FA_MEL_PRECISION_F64;   // transform arithmetic: FP64 (one frame per warp) or F32 (float32 frame pairs)
     int pipeline_chunks = 24;        // units a long host-buffer call is cut into (H2D / kernel / D2H overlap)
     bool zero_copy_out = false;      // time-major output in a pinned host buffer: the kernel stores straight into it
                                      // (opt-in: the staged copy is the default)
@@ -135,12 +104,13 @@ struct MelPlan {
     long long frame_count(long long n, int mode, long long expected) const;
     int ensure_staging(size_t audio_floats, size_t out_floats);
     int ensure_events(size_t count);
-    // kernel launch over `count` units at d_u (device) whose host mirror is h_u (read for the output alignment).
+    // kernel launch over `count` units at d_u (device) whose host mirror is h_u, numbered by number_tiles (the last unit
+    // gives the tile total; h_u is also read for the alignment of the audio and of the output rows).
     // inline_unit: a single unit travels in the kernel parameters and d_u is not read.
     int launch(const MelUnit *d_u, const MelUnit *h_u, int count, bool inline_unit, const float *d_audio_base,
-               float *d_out_base, int total_tiles, int mode, int layout, cudaStream_t stream, bool aligned16);
+               float *d_out_base, int mode, int layout, cudaStream_t stream);
 
-    // mode: 0 .center, 1 .prePadded, 2 legacy compute(); layout: 0 time-major, 1 mel-major
+    // mode: FA_MEL_PAD_* / FA_MEL_LEGACY_COMPUTE; layout: FA_MEL_TIME_MAJOR / FA_MEL_MEL_MAJOR
     int compute_device(const float *d_in, long long n, float last, int mode, long long expected, int layout,
                        float *d_out_buf, long long out_len, long long *mel_length, long long *num_frames,
                        cudaStream_t stream);
@@ -161,6 +131,20 @@ struct MelPlan {
     // torch-style frontends count their frames by their own rules (mel_adapters.cu).  last = 0.
     int launch_clip(const float *d_in, long long n, long long T, int layout, float *d_out_buf, cudaStream_t stream);
 };
+
+// Numbers a run of units that one launch covers: sets each unit's tile_begin and returns the run's tile total.
+int number_tiles(MelUnit *u, int count);
+
+// Shape rules of the entry points (mel_kernels.cu), shared with the host-buffer pipelines (mel_pipeline.cu).
+inline long long ceil_to(long long v, long long m) { return ((v + m - 1) / m) * m; }
+// bytes of the unit descriptors of a call with `count` units
+inline size_t unit_bytes(int count) { return (size_t)std::max(count, 64) * sizeof(MelUnit); }
+// Output shape of one clip, reported through mel_length / num_frames: T frames computed, Tp rows returned.  Empty input
+// gives T = 0 and one pad row (none in mode FA_MEL_LEGACY_COMPUTE), which the caller zeroes.  Fails when out_len floats
+// cannot hold Tp rows.
+int clip_shape(const MelPlan &p, long long n, int mode, long long expected, long long out_len, long long &T,
+               long long &Tp, long long *mel_length, long long *num_frames);
+constexpr long long kUnchecked = std::numeric_limits<long long>::max();   // batch calls take no output lengths
 
 // mel_stream.cu: live streams on one plan, SortformerDiarizer's incremental mel stream (SortformerDiarizer.swift:204-217,
 // :417-424, :842-901) for many sessions at once.  Per session, the samples not yet consumed by a frame (the carry, fewer
@@ -204,17 +188,6 @@ int cohere_features(MelPlan &p, const float *audio, long long n, long long fixed
                     long long *frames, long long *valid_frames);
 int styletts2_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames);
 int luxtts_features(MelPlan &p, const float *audio, long long n, float *out, long long out_len, long long *frames);
-
-void build_window(int length, bool periodic, std::vector<float> &w);
-void build_filterbank(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb);
-// fa_mel_create_ex's tables, each restating its Swift in that Swift's arithmetic (mel_kernels.cu)
-void build_window_cohere(int length, std::vector<float> &w);
-void build_filterbank_cohere(int n_fft, int n_mels, int sample_rate, float f_min, float f_max, std::vector<float> &fb);
-void build_filterbank_htk_f32(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb);
-void build_filterbank_htk_f64(int n_fft, int n_mels, int sample_rate, std::vector<float> &fb);
-// every fa_mel_ex_config field the kernels cannot honour, as fa_last_error text (FA_INVALID_ARGUMENT), before any
-// allocation
-int check_ex_config(const MelConfig &c);
 
 } // namespace mel
 } // namespace fa

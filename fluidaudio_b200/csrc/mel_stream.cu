@@ -254,7 +254,7 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     MelStreamJob *dj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(desc.device.data()) + units_bytes);
     const long long src0 = device ? 0 : offsets[0];   // a host push's samples land at d_audio[0]
     long long row = 0, a = 0;
-    int u = 0, j = 0, tiles = 0;
+    int u = 0, j = 0;
     for (int i = 0; i < count; ++i) {
         const int id = sessions[i];
         const Step &S = step[i];
@@ -270,18 +270,17 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         J.arena = a;
         const long long c1 = split ? S.first : emit;   // frames of the first unit
         const long long n1 = S.L + (split ? 0 : J.tail);
-        hu[u++] = MelUnit{a, n1, row * M, c1, 0, c1, 0.0f, tiles};   // .last: written by the ingest kernel
-        tiles += (int)((c1 + 15) / 16);
+        hu[u++] = MelUnit{a, n1, row * M, c1, 0, c1, 0.0f, 0};   // .last: written by the ingest kernel
         a += round_up4(n1);
         if (split) {
             J.arena2 = a;
             const long long n2 = S.L - J.consumed + J.tail;
-            hu[u++] = MelUnit{a, n2, (row + c1) * M, S.second, 0, S.second, 0.0f, tiles};
-            tiles += (int)((S.second + 15) / 16);
+            hu[u++] = MelUnit{a, n2, (row + c1) * M, S.second, 0, S.second, 0.0f, 0};
             a += round_up4(n2);
         }
         row += emit;
     }
+    number_tiles(hu, units);
 
     // ---- device work, all on the compute stream
     cudaStream_t s = p.streams[1];
@@ -303,7 +302,7 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     float *k_out = device ? out : p.d_out.data();
     if (units) {
         // `last` lives in the device units (written by the ingest kernel): the launch reads them from HBM, never inline
-        st = p.launch(du, hu, units, false, d_arena.data(), k_out, tiles, 1, 0, s, true);
+        st = p.launch(du, hu, units, false, d_arena.data(), k_out, FA_MEL_PAD_PREPADDED, FA_MEL_TIME_MAJOR, s);
         if (st != FA_OK) return st;
     }
     if (!device) {
