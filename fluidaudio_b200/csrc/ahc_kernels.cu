@@ -28,7 +28,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
-#include <mutex>
 #include <new>
 #include <vector>
 
@@ -1132,6 +1131,11 @@ int Solver::init(cudaStream_t s, int worker_limit) {
     }
     num_sms = prop.multiProcessorCount;
     max_workers = std::max(1, std::min(num_sms - 1, worker_limit > 0 ? worker_limit : num_sms - 1));
+    for (auto &e : ev) {
+        const int st2 = e.create();
+        if (st2 != FA_OK) return st2;
+    }
+    FA_CUDA_TRY(cudaFuncSetAttribute(ahc_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmemCap));
     return FA_OK;
 }
 
@@ -1228,12 +1232,6 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     P.idx16 = idx16 ? 1 : 0;
     P.smem_level = level;
 
-    Event ev[4];   // stage timing
-    for (auto &e : ev) {
-        st = e.create();
-        if (st != FA_OK) return st;
-    }
-
     FA_CUDA_TRY(cudaMemsetAsync(P.cmd, 0, 256, stream));
     FA_CUDA_TRY(cudaMemsetAsync(P.threshold, 0, 256, stream));
     FA_CUDA_TRY(cudaMemsetAsync(P.results, 0, 2 * sizeof(ResultSlot) * ((size_t)(max_workers + 1) << kSlotShift), stream));
@@ -1305,15 +1303,7 @@ int Solver::linkage_device(const double *d_rows, int N, int D, double *Z) {
     FA_CUDA_TRY(cudaMemcpyAsync(P.heap_where, h_where, idx_bytes * N, cudaMemcpyHostToDevice, stream));
     FA_CUDA_TRY(cudaMemcpyAsync(d_prob, &P, sizeof(Problem), cudaMemcpyHostToDevice, stream));
     FA_CUDA_TRY(cudaEventRecord(ev[2], stream));
-    {
-        static std::once_flag once;   // a per-function attribute: set it once to the maximum, solvers run concurrently
-        static cudaError_t attr_err = cudaSuccess;
-        std::call_once(once, [&]() {
-            attr_err = cudaFuncSetAttribute(ahc_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmemCap);
-        });
-        FA_CUDA_TRY(attr_err);
-        FA_CUDA_TRY(fa::launch_cooperative(ahc_merge_kernel, workers + 1, kWorkerThreads, smem, stream, d_prob));
-    }
+    FA_CUDA_TRY(fa::launch_cooperative(ahc_merge_kernel, workers + 1, kWorkerThreads, smem, stream, d_prob));
     FA_CUDA_TRY(cudaEventRecord(ev[3], stream));
     FA_CUDA_TRY(cudaMemcpyAsync(h_ma, P.merge_a, sizeof(int) * (N - 1), cudaMemcpyDeviceToHost, stream));
     FA_CUDA_TRY(cudaMemcpyAsync(h_mb, P.merge_b, sizeof(int) * (N - 1), cudaMemcpyDeviceToHost, stream));

@@ -64,7 +64,10 @@ struct Solver {
     DeviceBuffer<> d_pool;
     DeviceBuffer<double> d_input;   // staging of the caller's [N x D] rows when they come from the host
     PinnedBuffer<> h_pool;          // pinned host mirrors
+    Event ev[4];                    // stage timing (last_stage_ms)
 
+    // On the current device: the launch limits, the stage events and the merge kernel's shared-memory maximum (a function
+    // attribute holds per device).
     int init(cudaStream_t s, int worker_limit);
     // rows: device pointer to N x D row-major doubles (already normalised by the caller, as the reference requires).
     // Z: host buffer of (N-1) x 4 doubles.  Status codes follow FastClusterWrapper.h.

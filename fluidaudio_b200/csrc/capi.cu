@@ -5,8 +5,8 @@
 
 #include "ahc_plan.h"
 #include "assign_host.h"
+#include "cluster_plan.h"
 #include "mel_plan.h"
-#include "vbx_plan.h"
 #include "kmeans_plan.h"
 #include "reconstruct_host.h"
 
@@ -17,11 +17,7 @@
 #include <cstdio>
 #include <cstring>
 #include <memory>
-#include <mutex>
 #include <new>
-#include <set>
-#include <string>
-#include <thread>
 #include <vector>
 
 #define FA_API extern "C" __attribute__((visibility("default")))
@@ -63,339 +59,6 @@ static int require_device() {
     if (c <= 0) {
         set_error("no sm_90a (H100) device visible; fluidaudio_b200 has no CPU fallback");
         return FA_NO_DEVICE;
-    }
-    return FA_OK;
-}
-
-// ---- clustering context: one per concurrent caller, leased from a pool (the reference boundary is
-// synchronous, stateless and re-entrant: FastClusterWrapper.cpp keeps no state, SURVEY §8b) -------------
-struct ClusterContext {
-    int device = 0;
-    Stream stream;   // declared first, so destroyed last: after every buffer
-    ahc::Solver solver;
-    DeviceBuffer<> vbx_pool;    // scratch of VBx refinement, centroids and K-Means
-    DeviceBuffer<> cent_pool;   // the pipeline's gamma / pi / ELBOs / centroids
-    // pipeline buffers
-    DeviceBuffer<> d_buf;
-    PinnedBuffer<> h_buf;
-    Event ev[8];
-    bool ready = false;
-    int worker_limit = 0;
-
-    int init(int worker_lim) {
-        FA_CUDA_TRY(cudaGetDevice(&device));
-        int st = stream.create();
-        for (auto &e : ev)
-            if (st == FA_OK) st = e.create();
-        if (st != FA_OK) return st;
-        worker_limit = worker_lim;
-        st = solver.init(stream, worker_lim);
-        if (st != FA_OK) return st;
-        ready = true;
-        return FA_OK;
-    }
-};
-
-static std::mutex g_pool_mutex;
-static std::vector<std::unique_ptr<ClusterContext>> g_pool;   // idle contexts
-
-struct Lease {
-    std::unique_ptr<ClusterContext> ctx;
-    int status = FA_OK;
-    explicit Lease(int worker_limit = 0) {
-        int dev = 0;
-        const cudaError_t e = cudaGetDevice(&dev);
-        if (e != cudaSuccess) {
-            status = cuda_failure(e, "cudaGetDevice", __FILE__, __LINE__);
-            return;
-        }
-        {
-            std::lock_guard<std::mutex> lock(g_pool_mutex);
-            for (size_t i = 0; i < g_pool.size(); ++i)
-                if (g_pool[i]->device == dev && g_pool[i]->worker_limit == worker_limit) {
-                    ctx = std::move(g_pool[i]);
-                    g_pool.erase(g_pool.begin() + i);
-                    break;
-                }
-        }
-        if (!ctx) {
-            ctx.reset(new ClusterContext());
-            status = ctx->init(worker_limit);
-        }
-    }
-    ~Lease() {
-        if (ctx && ctx->ready && status != FA_CUDA_ERROR) {
-            std::lock_guard<std::mutex> lock(g_pool_mutex);
-            g_pool.push_back(std::move(ctx));
-        }
-    }
-};
-
-// Leases a context for `worker_limit`, runs body(ClusterContext &) on it and returns the body's status.  The status is
-// recorded on the lease, so a context whose call ended in FA_CUDA_ERROR is freed rather than pooled.
-template <typename Body> static int with_context(int worker_limit, Body &&body) {
-    Lease lease(worker_limit);
-    if (lease.status != FA_OK) return lease.status;
-    lease.status = body(*lease.ctx);
-    return lease.status;
-}
-
-static vbx::Config to_vbx(const fa_vbx_config &c) {
-    vbx::Config vc;
-    vc.Fa = c.Fa;
-    vc.Fb = c.Fb;
-    vc.max_iterations = c.max_iterations;
-    vc.epsilon = c.epsilon;
-    vc.init_smoothing = c.init_smoothing;
-    return vc;
-}
-
-// VBxOutput.assignedClusterCount: the distinct row-argmax winners among S speakers
-static int distinct_winners(const std::vector<int> &hard, int S) {
-    std::vector<char> seen(S, 0);
-    int count = 0;
-    for (const int h : hard)
-        if (h >= 0 && h < S && !seen[h]) {
-            seen[h] = 1;
-            ++count;
-        }
-    return count;
-}
-
-static float ms_between(cudaEvent_t a, cudaEvent_t b) {
-    float ms = 0;
-    cudaEventElapsedTime(&ms, a, b);
-    return ms;
-}
-
-// OfflineDiarizerManager.cluster(_:) :286-375 on one context.  All inputs are host pointers.
-static int cluster_pipeline(ClusterContext &C, const float *emb, const double *rho, size_t N, size_t E, size_t R,
-                            const double *psi, const fa_cluster_config &cfg, int32_t *labels, int32_t *initial_out,
-                            double *centroids_out, int32_t max_centroids, fa_cluster_info *info,
-                            const int32_t *chunk_index = nullptr) {
-    const auto wall0 = std::chrono::steady_clock::now();
-    cudaStream_t s = C.stream;
-    const int n = (int)N, e = (int)E, r = (int)R;
-    // ---- device arena and pinned host arena --------------------------------------------------------------------
-    float *d_emb32;
-    double *d_emb, *d_rho, *d_train, *d_train_rho, *d_norm;
-    unsigned char *d_ok;
-    int *d_idx, *d_init, *d_hard, *d_labels, *d_count;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_emb32 = c.take<float>(N * E);
-        d_emb = c.take<double>(N * E);
-        d_rho = c.take<double>(N * R);
-        d_ok = c.take<unsigned char>(N);
-        d_idx = c.take<int>(N);               // train idx
-        d_train = c.take<double>(N * E);
-        d_train_rho = c.take<double>(N * R);
-        d_norm = c.take<double>(N * E);       // normalised train
-        d_init = c.take<int>(N);              // init labels
-        d_hard = c.take<int>(N);
-        d_labels = c.take<int>(N);
-        d_count = c.take<int>(64);
-    }, 4096);
-    if (st != FA_OK) return st;
-    unsigned char *h_ok;
-    int *h_idx, *h_count;
-    int32_t *h_init;
-    double *h_Z;
-    st = carve_arena(C.h_buf, [&](Carver &c) {
-        h_ok = c.take<unsigned char>(N);
-        h_idx = c.take<int>(N);
-        h_init = c.take<int32_t>(N);
-        h_count = c.take<int>(16);
-        h_Z = c.take<double>(N > 1 ? (N - 1) * 4 : 4);
-    }, 4096);
-    if (st != FA_OK) return st;
-
-    FA_CUDA_TRY(cudaEventRecord(C.ev[0], s));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb32, emb, N * E * sizeof(float), cudaMemcpyHostToDevice, s));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_rho, rho, N * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    st = ahc::launch_widen_rows(d_emb32, d_emb, (long long)N * E, s);   // :286  Float -> Double
-    if (st != FA_OK) return st;
-    st = vbx::finite_rows_device(d_emb32, n, e, d_ok, s);               // :591-611
-    if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(h_ok, d_ok, N, cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
-    int Tn = 0;
-    for (int i = 0; i < n; ++i)
-        if (h_ok[i]) h_idx[Tn++] = i;
-    if (Tn == 0) {
-        for (int i = 0; i < n; ++i) h_idx[i] = i;
-        Tn = n;
-    }
-    const double *d_tr = d_emb, *d_tr_rho = d_rho;
-    if (Tn != n) {
-        FA_CUDA_TRY(cudaMemcpyAsync(d_idx, h_idx, Tn * sizeof(int), cudaMemcpyHostToDevice, s));
-        st = vbx::gather_rows_device(d_emb, d_idx, Tn, e, d_train, s);
-        if (st != FA_OK) return st;
-        st = vbx::gather_rows_device(d_rho, d_idx, Tn, r, d_train_rho, s);
-        if (st != FA_OK) return st;
-        d_tr = d_train;
-        d_tr_rho = d_train_rho;
-    }
-    // ---- AHC (:301-309) ---------------------------------------------------------------------------------
-    FA_CUDA_TRY(cudaEventRecord(C.ev[1], s));
-    float ms_norm = 0, ms_ahc = 0, ms_cut = 0;
-    if (Tn >= 2) {
-        st = ahc::launch_normalize_rows(d_tr, d_norm, Tn, e, s);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaEventRecord(C.ev[2], s));
-        st = C.solver.linkage_device(d_norm, Tn, e, h_Z);
-        FA_CUDA_TRY(cudaEventRecord(C.ev[3], s));
-        FA_CUDA_TRY(cudaEventSynchronize(C.ev[3]));
-        ms_norm = ms_between(C.ev[1], C.ev[2]);
-        ms_ahc = ms_between(C.ev[2], C.ev[3]);
-        const auto t0 = std::chrono::steady_clock::now();
-        if (st == FA_OK) {
-            ahc::dendrogram_cut(h_Z, Tn, cfg.threshold, h_init);
-        } else if (st == FA_RUNTIME_ERROR || st == FA_UNSUPPORTED) {
-            for (int i = 0; i < Tn; ++i) h_init[i] = i;   // AHCClustering.swift:52-55: FFI failure -> identity labels
-        } else {
-            return st;
-        }
-        ms_cut = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    } else {
-        for (int i = 0; i < Tn; ++i) h_init[i] = 0;
-    }
-    int S = 0;
-    for (int i = 0; i < Tn; ++i) S = std::max(S, h_init[i] + 1);   // labels are canonical 0..S-1
-    S = std::max(S, 1);
-    if (initial_out) {
-        for (int i = 0; i < n; ++i) initial_out[i] = -1;
-        for (int i = 0; i < Tn; ++i) initial_out[h_idx[i]] = h_init[i];
-    }
-    // ---- VBx (:311-343) -----------------------------------------------------------------------------------
-    FA_CUDA_TRY(cudaEventRecord(C.ev[4], s));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_init, h_init, Tn * sizeof(int), cudaMemcpyHostToDevice, s));
-    // arena for gamma / pi / elbos / centroids (depends on S, known only now), at least 1 MB
-    const vbx::Config vc = to_vbx(cfg.vbx);
-    st = C.cent_pool.grow((size_t)1 << 20);
-    if (st != FA_OK) return st;
-    double *d_gamma, *d_pi, *d_elbos, *d_cent, *d_cent_n;
-    st = carve_arena(C.cent_pool, [&](Carver &c) {
-        d_gamma = c.take<double>((size_t)Tn * S);
-        d_pi = c.take<double>(S);
-        d_elbos = c.take<double>(std::max(vc.max_iterations, 1));
-        d_cent = c.take<double>((size_t)S * E + E);
-        d_cent_n = c.take<double>((size_t)S * E + E);
-    }, 8192);
-    if (st != FA_OK) return st;
-    int iterations = 0;
-    std::vector<double> psi_eff(R, 1.0);   // VBxClustering.swift:71-76: identity when psi does not match
-    if (psi) std::memcpy(psi_eff.data(), psi, R * sizeof(double));
-    bool used_vbx = false;
-    if (Tn > 0) {
-        st = vbx::refine_device(C.vbx_pool, d_tr_rho, Tn, r, psi_eff.data(), d_init, S, vc, d_gamma, d_pi, d_elbos, d_hard,
-                                &iterations, s);
-        if (st != FA_OK) return st;
-        used_vbx = true;
-    }
-    // ---- speaker-count constraints (:311-336, VBxClustering.swift:685-733) ----------------------------------
-    bool adjusted = false;
-    int detected = S, K = 0;
-    if (used_vbx && (cfg.num_speakers != FA_NO_VALUE || cfg.min_speakers != FA_NO_VALUE || cfg.max_speakers != FA_NO_VALUE)) {
-        std::vector<int> hard(Tn);
-        FA_CUDA_TRY(cudaMemcpyAsync(hard.data(), d_hard, sizeof(int) * Tn, cudaMemcpyDeviceToHost, s));
-        FA_CUDA_TRY(cudaStreamSynchronize(s));
-        detected = distinct_winners(hard, S);
-        long long lo = 1, hi = Tn;
-        kmeans::resolve_constraints(Tn, cfg.num_speakers, cfg.min_speakers, cfg.max_speakers, &lo, &hi);
-        if (detected < lo || detected > hi) {
-            const int target = (int)(detected < lo ? lo : hi);
-            // the arena may have moved: re-carve (gamma / pi are not needed any more on this path)
-            st = carve_arena(C.cent_pool, [&](Carver &c) {
-                d_cent = c.take<double>((size_t)target * E + E);
-                d_cent_n = c.take<double>((size_t)target * E + E);
-            }, 8192);
-            if (st != FA_OK) return st;
-            int rows = 0;
-            st = kmeans::cluster_ninit_device(C.vbx_pool, d_tr, Tn, e, target, 100, 10, 0ull, d_hard, d_cent, &rows, nullptr, s);
-            if (st != FA_OK) return st;
-            st = ahc::launch_normalize_rows_keep(d_cent, d_cent_n, rows, e, s);   // normalize (:824-860) for the cosine
-            if (st != FA_OK) return st;
-            K = rows;
-            adjusted = true;
-        }
-    }
-    FA_CUDA_TRY(cudaEventRecord(C.ev[5], s));
-    // ---- centroids (:345-353) + assignment (:371-374) -----------------------------------------------------
-    if (!adjusted) {
-        st = vbx::centroids_device(C.vbx_pool, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
-        FA_CUDA_TRY(cudaStreamSynchronize(s));
-        K = *h_count;
-        if (K == 0 && used_vbx) {
-            // no speaker with pi > 1e-7: computeCentroidsFromClusters(initialClusters) (:687-690)
-            st = vbx::onehot_device(d_init, Tn, S, d_gamma, d_pi, s);
-            if (st != FA_OK) return st;
-            st = vbx::centroids_device(C.vbx_pool, d_tr, Tn, e, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, s);
-            if (st != FA_OK) return st;
-            FA_CUDA_TRY(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, s));
-            FA_CUDA_TRY(cudaStreamSynchronize(s));
-            K = *h_count;
-        }
-    }
-    if (K == 0) {
-        // computeFallbackCentroids: mean of all embeddings (:748-786)
-        st = vbx::mean_rows_device(d_emb, n, e, d_cent, s);
-        if (st != FA_OK) return st;
-        st = vbx::onehot_device(d_init, 0, 1, d_gamma, d_pi, s);   // pi[0] = 1
-        if (st != FA_OK) return st;
-        // OfflineDiarizerManager.normalize on the one centroid (:824-860: a zero row is kept)
-        st = ahc::launch_normalize_rows_keep(d_cent, d_cent_n, 1, e, s);
-        if (st != FA_OK) return st;
-        K = 1;
-    }
-    // constrained assignment (:357-369) needs the full N x K score matrix on the host; plain argmax (:371-374) does not
-    const bool constrained = chunk_index != nullptr && K > 1 && !adjusted;   // :357-360
-    double *d_scores = nullptr;
-    if (constrained) {
-        st = carve_arena(C.vbx_pool, [&](Carver &c) { d_scores = c.take<double>(N * (size_t)K); }, 1024);
-        if (st != FA_OK) return st;
-    }
-    st = vbx::assign_device(d_emb, n, e, d_cent_n, nullptr, K, d_labels, d_scores, s);
-    if (st != FA_OK) return st;
-    if (constrained) {
-        std::vector<double> h_scores(N * (size_t)K);
-        FA_CUDA_TRY(cudaMemcpyAsync(h_scores.data(), d_scores, h_scores.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-        FA_CUDA_TRY(cudaStreamSynchronize(s));
-        assign::constrained_assign(h_scores.data(), (long long)N, K, chunk_index, labels);
-    } else {
-        FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, s));
-    }
-    if (centroids_out && max_centroids > 0) {
-        const int kc = std::min(K, max_centroids);
-        FA_CUDA_TRY(cudaMemcpyAsync(centroids_out, d_cent, (size_t)kc * E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    }
-    FA_CUDA_TRY(cudaEventRecord(C.ev[6], s));
-    // VBxOutput.assignedClusterCount for the caller's info when no speaker-count constraint asked for it above: the
-    // row-argmax winners travel with the final synchronisation
-    std::vector<int> hard_info;
-    const bool count_winners = info && used_vbx && !adjusted && detected == S && Tn > 0 &&
-                               cfg.num_speakers == FA_NO_VALUE && cfg.min_speakers == FA_NO_VALUE && cfg.max_speakers == FA_NO_VALUE;
-    if (count_winners) {
-        hard_info.resize(Tn);
-        FA_CUDA_TRY(cudaMemcpyAsync(hard_info.data(), d_hard, sizeof(int) * Tn, cudaMemcpyDeviceToHost, s));
-    }
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
-    if (count_winners) detected = distinct_winners(hard_info, S);
-    if (info) {
-        info->training_count = Tn;
-        info->initial_clusters = S;
-        info->vbx_iterations = iterations;
-        info->centroid_count = K;
-        info->ms_normalize = ms_norm;
-        info->ms_ahc = ms_ahc;
-        info->ms_cut = ms_cut;
-        info->ms_vbx = ms_between(C.ev[4], C.ev[5]);
-        info->ms_assign = ms_between(C.ev[5], C.ev[6]);
-        info->ms_total =
-            std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
-        info->was_adjusted = adjusted ? 1 : 0;
-        info->detected_clusters = detected;
     }
     return FA_OK;
 }
@@ -1092,20 +755,7 @@ FA_API fa_status fa_l2_normalize_rows(const double *x, size_t rows, size_t dim, 
     if (rows == 0 || dim == 0) return FA_STATUS_OK;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
-        double *d_in, *d_out;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_in = c.take<double>(rows * dim);
-            d_out = c.take<double>(rows * dim);
-        }, 512);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(d_in, x, rows * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        st = ahc::launch_normalize_rows(d_in, d_out, (int)rows, (int)dim, C.stream);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, rows * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-        return FA_OK;
-    });
+    return (fa_status)with_context(0, [&](ClusterContext &C) { return l2_normalize_rows(C, x, rows, dim, out); });
     FA_GUARD_END
 }
 
@@ -1132,26 +782,8 @@ FA_API fa_status fa_ahc_cluster(const double *features, size_t count, size_t dim
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
-        double *d_in, *d_norm, *h_Z;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_in = c.take<double>(count * dim);
-            d_norm = c.take<double>(count * dim);
-        }, 512);
-        if (st != FA_OK) return st;
-        st = carve_arena(C.h_buf, [&](Carver &c) { h_Z = c.take<double>((count - 1) * 4); }, 512);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        st = ahc::launch_normalize_rows(d_in, d_norm, (int)count, (int)dim, C.stream);
-        if (st != FA_OK) return st;
-        st = C.solver.linkage_device(d_norm, (int)count, (int)dim, h_Z);
-        if (st == FA_RUNTIME_ERROR || st == FA_UNSUPPORTED) {      // FFI failure -> Array(0..<count) (:52-55)
-            for (size_t i = 0; i < count; ++i) labels[i] = (int32_t)i;
-            return FA_OK;
-        }
-        if (st != FA_OK) return st;
-        ahc::dendrogram_cut(h_Z, (long long)count, threshold, labels);
-        return FA_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) {
+        return ahc_cluster(C, features, count, dim, threshold, labels);
     });
     FA_GUARD_END
 }
@@ -1255,26 +887,9 @@ FA_API fa_status fa_kmeans_cluster(const double *emb, size_t N, size_t D, int32_
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
-        double *d_emb, *d_cent;
-        int *d_labels;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_emb = c.take<double>(N * D);
-            d_cent = c.take<double>((size_t)rows_needed * D);
-            d_labels = c.take<int>(N);
-        }, 1024);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        int rows = 0, best = 0;
-        st = kmeans::cluster_ninit_device(C.vbx_pool, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
-                                          d_labels, d_cent, &rows, &best, C.stream);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)rows * D * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-        if (centroid_rows) *centroid_rows = rows;
-        if (best_init) *best_init = best;
-        return FA_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) {
+        return kmeans_cluster(C, emb, N, D, num_clusters, max_iterations, n_init, base_seed, labels, centroids, centroid_rows,
+                              best_init);
     });
     FA_GUARD_END
 }
@@ -1285,34 +900,8 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
     if (!rho || !cfg || !gamma || !pi || !elbos || !hard || T == 0 || D == 0 || S <= 0) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
-        const int cap = std::max(cfg->max_iterations, 1);
-        double *d_x, *d_gamma, *d_pi, *d_elbos;
-        int *d_init, *d_hard;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_x = c.take<double>(T * D);
-            d_init = c.take<int>(T);
-            d_gamma = c.take<double>(T * (size_t)S);
-            d_pi = c.take<double>(S);
-            d_elbos = c.take<double>(cap);
-            d_hard = c.take<int>(T);
-        }, 1024);
-        if (st != FA_OK) return st;
-        std::vector<double> psi_eff(D, 1.0);
-        if (psi && psi_len == D) std::memcpy(psi_eff.data(), psi, D * sizeof(double));
-        FA_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        if (initial) FA_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
-        int its = 0;
-        st = vbx::refine_device(C.vbx_pool, d_x, (int)T, (int)D, psi_eff.data(), initial ? d_init : nullptr, S, to_vbx(*cfg),
-                                d_gamma, d_pi, d_elbos, d_hard, &its, C.stream);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(pi, d_pi, S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(elbos, d_elbos, cap * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(hard, d_hard, T * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-        if (iterations) *iterations = its;
-        return FA_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) {
+        return vbx_refine(C, rho, T, D, psi, psi_len, initial, S, *cfg, gamma, pi, elbos, hard, iterations);
     });
     FA_GUARD_END
 }
@@ -1323,32 +912,8 @@ FA_API fa_status fa_compute_centroids(const double *emb, size_t T, size_t dim, c
         return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
-        double *d_emb, *d_gamma, *d_pi, *d_cent, *d_cent_n;
-        int *d_count;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_emb = c.take<double>(T * dim);
-            d_gamma = c.take<double>(T * (size_t)S);
-            d_pi = c.take<double>(S);
-            d_cent = c.take<double>((size_t)S * dim);
-            d_cent_n = c.take<double>((size_t)S * dim);
-            d_count = c.take<int>(64);
-        }, 1024);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        st = vbx::centroids_device(C.vbx_pool, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream);
-        if (st != FA_OK) return st;
-        int K = 0;
-        FA_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-        *centroid_count = K;
-        if (K > 0) {
-            FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)K * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-            FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-        }
-        return FA_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) {
+        return compute_centroids(C, emb, T, dim, gamma, pi, S, centroids, centroid_count);
     });
     FA_GUARD_END
 }
@@ -1363,29 +928,8 @@ FA_API fa_status fa_assign_embeddings(const double *emb, size_t N, size_t dim, c
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) -> int {
-        double *d_emb, *d_craw, *d_cn, *d_scores;
-        int *d_labels;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_emb = c.take<double>(N * dim);
-            d_craw = c.take<double>((size_t)K * dim);
-            d_cn = c.take<double>((size_t)K * dim);
-            d_labels = c.take<int>(N);
-            d_scores = c.take<double>(scores ? N * (size_t)K : 1);
-        }, 1024);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(d_craw, centroids, (size_t)K * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-        // centroid normalisation (:793, :824-860; zero rows kept) with the same kernel the pipeline uses
-        st = ahc::launch_normalize_rows_keep(d_craw, d_cn, K, (int)dim, C.stream);
-        if (st != FA_OK) return st;
-        st = vbx::assign_device(d_emb, (int)N, (int)dim, d_cn, nullptr, K, d_labels, scores ? d_scores : nullptr, C.stream);
-        if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-        if (scores)
-            FA_CUDA_TRY(cudaMemcpyAsync(scores, d_scores, N * (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
-        return FA_OK;
+    return (fa_status)with_context(0, [&](ClusterContext &C) {
+        return assign_embeddings(C, emb, N, dim, centroids, K, labels, scores);
     });
     FA_GUARD_END
 }
@@ -1463,8 +1007,7 @@ FA_API fa_status fa_build_chunk_assignments(const int32_t *chunk_index, const in
     FA_GUARD_END
 }
 
-// Independent sets run on disjoint SM partitions: `lanes` host threads, each leasing a context whose merge kernel
-// is capped at (SMs / lanes) - 1 worker CTAs, pull sets from a shared counter.
+// The batch's argument checks; its lanes are cluster_batch (cluster_pipeline.cu).
 static fa_status cluster_batch_impl(const float *emb256, const double *rho, const int64_t *set_offsets,
                                     int32_t set_count, size_t emb_dim, size_t rho_dim, const double *psi,
                                     const fa_cluster_config *cfg, const int32_t *chunk_index, int32_t *labels,
@@ -1487,84 +1030,8 @@ static fa_status cluster_batch_impl(const float *emb256, const double *rho, cons
             if (set_offsets[m + 1] == set_offsets[m]) infos[m] = fa_cluster_info{};
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    int dev = 0;
-    FA_CUDA_TRY(cudaGetDevice(&dev));
-    cudaDeviceProp prop;
-    FA_CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    // Concurrency: see ahc::plan_batch_lanes
-    long long n_max = 0;
-    for (int m = 0; m < set_count; ++m) n_max = std::max<long long>(n_max, set_offsets[m + 1] - set_offsets[m]);
-    const ahc::BatchLanes plan = ahc::plan_batch_lanes(set_count, n_max, (int)emb_dim, prop.multiProcessorCount);
-    const int lanes = plan.lanes, worker_limit = plan.worker_limit;
-    std::atomic<int> next{0};
-    std::vector<int> status(lanes, FA_OK);
-    std::vector<std::string> messages(lanes);
-    // Each lane is a plain std::thread: nothing may escape it (an exception leaving a thread function is std::terminate,
-    // and FA_GUARD_* only covers the calling thread), so the body is wrapped and failures are reported through status[].
-    auto run_lane = [&](int lane) {
-        const cudaError_t e = cudaSetDevice(dev);
-        if (e != cudaSuccess) {
-            status[lane] = cuda_failure(e, "cudaSetDevice", __FILE__, __LINE__);
-            messages[lane] = fa::last_error();
-            return;
-        }
-        const int st = with_context(worker_limit, [&](ClusterContext &C) {
-            for (;;) {
-                const int m = next.fetch_add(1);
-                if (m >= set_count) return (int)FA_OK;
-                const int64_t a = set_offsets[m], b = set_offsets[m + 1];
-                if (b == a) continue;   // its info was zeroed above
-                const int st = cluster_pipeline(C, emb256 + (size_t)a * emb_dim, rho + (size_t)a * rho_dim, (size_t)(b - a),
-                                                emb_dim, rho_dim, psi, *cfg, labels + a, nullptr, nullptr, 0,
-                                                infos ? infos + m : nullptr, chunk_index ? chunk_index + a : nullptr);
-                if (st != FA_OK) return st;
-            }
-        });
-        if (st != FA_OK) {
-            status[lane] = st;
-            messages[lane] = fa::last_error();
-        }
-    };
-    auto run = [&](int lane) noexcept {
-        try {
-            run_lane(lane);
-        } catch (const std::bad_alloc &) {
-            status[lane] = FA_ALLOCATION_FAILURE;
-            try { messages[lane] = "host allocation failed"; } catch (...) {}
-        } catch (const std::exception &ex) {
-            status[lane] = FA_RUNTIME_ERROR;
-            try { messages[lane] = std::string("exception: ") + ex.what(); } catch (...) {}
-        } catch (...) {
-            status[lane] = FA_UNKNOWN_ERROR;
-        }
-        if (status[lane] != FA_OK) next.store(set_count);   // the other lanes stop taking new sets
-    };
-    // threads already started are always joined, also when starting a later one fails
-    struct Joiner {
-        std::vector<std::thread> t;
-        ~Joiner() {
-            for (auto &x : t)
-                if (x.joinable()) x.join();
-        }
-    } threads;
-    threads.t.reserve(lanes);
-    int started = 1;
-    try {
-        for (int l = 1; l < lanes; ++l) {
-            threads.t.emplace_back(run, l);
-            ++started;
-        }
-    } catch (...) {   // std::system_error: run with the lanes that did start
-    }
-    (void)started;
-    run(0);
-    for (auto &t : threads.t) t.join();
-    for (int l = 0; l < lanes; ++l)
-        if (status[l] != FA_OK) {
-            fa::set_error("%s", messages[l].c_str());
-            return (fa_status)status[l];
-        }
-    return FA_STATUS_OK;
+    return (fa_status)cluster_batch(emb256, rho, set_offsets, set_count, emb_dim, rho_dim, psi, *cfg, chunk_index, labels,
+                                    infos);
     FA_GUARD_END
 }
 

@@ -15,7 +15,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <mutex>
 #include <vector>
 
 namespace fa {
@@ -728,14 +727,6 @@ __global__ void __launch_bounds__(kARows) assign_tiled_kernel(const double *__re
     if (n < N) labels[n] = best;
 }
 
-__global__ void onehot_kernel(const int *__restrict__ labels, int T, int S, double *__restrict__ gamma,
-                              double *__restrict__ pi) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < S) pi[t] = 1.0;
-    if (t >= T) return;
-    for (int s = 0; s < S; ++s) gamma[(size_t)t * S + s] = (labels[t] == s) ? 1.0 : 0.0;
-}
-
 __global__ void finite_rows_kernel(const float *__restrict__ emb, int N, int E, unsigned char *__restrict__ ok) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= N) return;
@@ -752,19 +743,20 @@ __global__ void gather_rows_kernel(const double *__restrict__ src, const int *__
     dst[i] = src[(size_t)idx[r] * dim + k];
 }
 
-__global__ void mean_rows_kernel(const double *__restrict__ src, int rows, int dim, double *__restrict__ out) {
-    const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= dim) return;
-    double acc = 0.0;
-    for (int r = 0; r < rows; ++r) acc += src[(size_t)r * dim + k];
-    out[k] = acc * (1.0 / (double)rows);
-}
-
 // ------------------------------------------------------------------------------------------------ host side
 static size_t fused_smem_bytes(int S, int D) {
     return sizeof(double) * ((size_t)S * D + 2 * (size_t)S + (size_t)kEThreads * S + kEThreads);
 }
 static bool fused_path(int S, int D) { return S <= kFusedMaxS && fused_smem_bytes(S, D) <= 200 * 1024; }
+
+int set_smem_limits() {
+    FA_CUDA_TRY(cudaFuncSetAttribute(vbx_estep_kernel2, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    FA_CUDA_TRY(cudaFuncSetAttribute(vbx_partials0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    FA_CUDA_TRY(cudaFuncSetAttribute(vbx_estep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    FA_CUDA_TRY(cudaFuncSetAttribute(centroid_acc16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(double) * kCBlock * kFusedMaxS)));
+    return FA_OK;
+}
 
 // d_x: [T x D] device, h_psi: [D] HOST (already identity-substituted by the caller if lengths mismatch),
 // d_init: [T] device labels (or nullptr), d_gamma [T x S], d_pi [S], d_elbos [max(max_it,1)], d_hard [T].
@@ -830,14 +822,6 @@ int refine_device(DeviceBuffer<> &pool, const double *d_x, int T, int D, const d
     }
     FA_CUDA_TRY(fa::launch(vbx_init_kernel, (T + 127) / 128, 128, 0, stream, d, d_init, cfg.init_smoothing));
     if (fused_path(S, D)) {
-        static std::once_flag once_f;
-        static cudaError_t attr_err_f = cudaSuccess;
-        std::call_once(once_f, [&]() {
-            attr_err_f = cudaFuncSetAttribute(vbx_estep_kernel2, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-            if (attr_err_f == cudaSuccess)
-                attr_err_f = cudaFuncSetAttribute(vbx_partials0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        });
-        FA_CUDA_TRY(attr_err_f);
         const size_t tile_bytes = sizeof(double) * (size_t)D * (kEThreads + 1);
         const bool use_tile = fused_smem_bytes(S, D) + tile_bytes <= 200 * 1024;
         const size_t fsmem = fused_smem_bytes(S, D) + (use_tile ? tile_bytes : 0);
@@ -852,12 +836,6 @@ int refine_device(DeviceBuffer<> &pool, const double *d_x, int T, int D, const d
         const size_t esmem_full = sizeof(double) * ((size_t)S * D + 2 * S + kEThreads);
         const bool alpha_smem = esmem_full <= 200 * 1024;
         const size_t esmem = alpha_smem ? esmem_full : sizeof(double) * kEThreads;
-        static std::once_flag once;   // per-function attribute shared by concurrent callers: set once to the maximum
-        static cudaError_t attr_err = cudaSuccess;
-        std::call_once(once, [&]() {
-            attr_err = cudaFuncSetAttribute(vbx_estep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        });
-        FA_CUDA_TRY(attr_err);
         for (int it = 0; it < max_it; ++it) {
             FA_CUDA_TRY(fa::launch(vbx_accumulate_kernel, d.chunks, 256, 0, stream, d));
             FA_CUDA_TRY(fa::launch(vbx_update_kernel, 1, 256, 0, stream, d));
@@ -888,13 +866,6 @@ int centroids_device(DeviceBuffer<> &pool, const double *d_emb, int T, int E, co
     }, 2048);
     if (st != FA_OK) return st;
     if (S <= kFusedMaxS) {
-        static std::once_flag once_c;
-        static cudaError_t attr_err_c = cudaSuccess;
-        std::call_once(once_c, [&]() {
-            attr_err_c = cudaFuncSetAttribute(centroid_acc16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)(sizeof(double) * kCBlock * kFusedMaxS));
-        });
-        FA_CUDA_TRY(attr_err_c);
         const unsigned tiles = (unsigned)((S * E + 255) / 256);
         FA_CUDA_TRY(fa::launch(centroid_acc16_kernel, chunks, 256, sizeof(double) * (size_t)kCBlock * S, stream, d_emb, d_gamma,
                                T, E, S, pnum, pden));
@@ -916,12 +887,6 @@ int assign_device(const double *d_emb, int N, int E, const double *d_cent_n, con
     return FA_OK;
 }
 
-int onehot_device(const int *d_labels, int T, int S, double *d_gamma, double *d_pi, cudaStream_t stream) {
-    const int n = std::max(T, S);
-    FA_CUDA_TRY(fa::launch(onehot_kernel, (n + 127) / 128, 128, 0, stream, d_labels, T, S, d_gamma, d_pi));
-    return FA_OK;
-}
-
 int finite_rows_device(const float *d_emb, int N, int E, unsigned char *d_ok, cudaStream_t stream) {
     FA_CUDA_TRY(fa::launch(finite_rows_kernel, (N + 127) / 128, 128, 0, stream, d_emb, N, E, d_ok));
     return FA_OK;
@@ -931,11 +896,6 @@ int gather_rows_device(const double *d_src, const int *d_idx, int rows, int dim,
     const long long total = (long long)rows * dim;
     if (total <= 0) return FA_OK;
     FA_CUDA_TRY(fa::launch(gather_rows_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, d_src, d_idx, rows, dim, d_dst));
-    return FA_OK;
-}
-
-int mean_rows_device(const double *d_src, int rows, int dim, double *d_out, cudaStream_t stream) {
-    FA_CUDA_TRY(fa::launch(mean_rows_kernel, (dim + 127) / 128, 128, 0, stream, d_src, rows, dim, d_out));
     return FA_OK;
 }
 

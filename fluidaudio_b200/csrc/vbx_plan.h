@@ -15,6 +15,10 @@ struct Config {
     double init_smoothing = 7.0; // VBxClustering.swift:131
 };
 
+// Opts the kernels below that take more than 48 KB of dynamic shared memory in to their maxima.  A function attribute
+// holds for the device current when it is set: call it on every device the kernels run on.
+int set_smem_limits();
+
 // `pool`: the scratch arena, reused across calls (grown on demand).
 int refine_device(DeviceBuffer<> &pool, const double *d_x, int T, int D, const double *h_psi, const int *d_init, int S,
                   const Config &cfg, double *d_gamma, double *d_pi, double *d_elbos, int *d_hard, int *iterations_host,
@@ -23,10 +27,8 @@ int centroids_device(DeviceBuffer<> &pool, const double *d_emb, int T, int E, co
                      int S, double *d_cent, double *d_cent_n, int *d_count, cudaStream_t stream);
 int assign_device(const double *d_emb, int N, int E, const double *d_cent_n, const int *d_count, int K_fixed,
                   int *d_labels, double *d_scores, cudaStream_t stream);
-int onehot_device(const int *d_labels, int T, int S, double *d_gamma, double *d_pi, cudaStream_t stream);
 int finite_rows_device(const float *d_emb, int N, int E, unsigned char *d_ok, cudaStream_t stream);
 int gather_rows_device(const double *d_src, const int *d_idx, int rows, int dim, double *d_dst, cudaStream_t stream);
-int mean_rows_device(const double *d_src, int rows, int dim, double *d_out, cudaStream_t stream);
 
 } // namespace vbx
 } // namespace fa

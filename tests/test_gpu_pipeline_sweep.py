@@ -1,4 +1,4 @@
-"""The clustering pipeline (``cluster_pipeline`` in ``capi.cu``) and its batch entry points on every branch (run with
+"""The clustering pipeline (``cluster_pipeline`` in ``cluster_pipeline.cu``) and its batch entry points on every branch (run with
 ``-m gpu``).
 
 The C ABI is called through ctypes, so NULL outputs, ``max_centroids`` and ``init_smoothing`` are reachable.  Every case
@@ -32,8 +32,8 @@ Each case names the branch it must take, and the launch-count delta (``pipeline_
 | speaker count satisfied | ``min_speakers_1`` | was_adjusted 0 |
 | speaker count violated -> K-Means + normalisation | ``num_speakers_1_chunks`` | was_adjusted 1; K-Means launches + 1 |
 | non-finite rho in a training row | ``rho_nan``, ``rho_nan_chunks`` | every E-step row falls back to uniform gamma: S identical centroids, every score tied, label 0 |
-| no speaker with pi > 1e-7 -> one-hot recompute | unreachable | VBx renormalises pi to sum 1 and falls back to 1/S when the sum is not finite, so some pi >= 1/S > 1e-7 for any S an arena can hold |
-| K == 0 after that -> mean of all rows | unreachable | the one-hot recompute gives pi = 1 to all S >= 1 speakers, and K-Means returns min(target, Tn) >= 1 rows |
+| no speaker with pi > 1e-7 -> one-hot recompute | removed: unreachable, see Proof | VBx renormalises pi to sum 1 and falls back to 1/S when the sum is not finite, so some pi >= 1/S > 1e-7 for any S an arena can hold |
+| K == 0 after that -> mean of all rows | removed: unreachable, see Proof | the one-hot recompute would give pi = 1 to all S >= 1 speakers, and K-Means returns min(target, Tn) >= 1 rows; the pipeline reports K == 0 as an internal FA_RUNTIME_ERROR |
 | constrained assignment (chunks, K > 1, not adjusted) | ``nan_emb_chunks``, ``chunk_overflow``, ``rho_nan_chunks`` | labels equal ``fa_constrained_assign``; -2 where a chunk has more local speakers than clusters |
 | chunks with K == 1, or adjusted -> plain argmax | ``k1_chunks``, ``num_speakers_1_chunks`` | no -2 label |
 | NULL initial / centroids / info, max_centroids | ``test_null_outputs...``, ``test_max_centroids...`` | same labels; the first min(K, max) rows byte-equal, the rest untouched |
@@ -185,7 +185,7 @@ def compose(case):
     if not adjusted:
         cents = centroids(gamma, pi)
     K = cents.shape[0]
-    assert K > 0, "no speaker with pi > 1e-7"   # the pipeline's one-hot recompute, unreachable (module docstring)
+    assert K > 0, "no speaker with pi > 1e-7"   # an internal error in the pipeline, unreachable (module docstring)
     labels, scores = np.zeros(N, np.int32), np.zeros((N, max(K, 1)))
     _ok(L.fa_assign_embeddings(feats.ctypes.data, N, E, cents.ctypes.data, K, labels.ctypes.data, scores.ctypes.data),
         "fa_assign_embeddings")
