@@ -69,6 +69,17 @@ class ReconstructConfig(C.Structure):
                 ("min_segment_duration", C.c_double), ("exclusive_segments", C.c_int32), ("reserved", C.c_int32)]
 
 
+class SegConfig(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("speech_onset_threshold", C.c_float), ("window_duration", C.c_double),
+                ("step_ratio", C.c_double)]
+
+
+class EmbedPlanConfig(C.Structure):
+    _fields_ = [("exclude_overlap", C.c_int32), ("skip_threshold", C.c_float), ("min_segment_duration", C.c_double),
+                ("weight_frames", C.c_int32), ("audio_sample_count", C.c_int32), ("fbank_batch", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 # every symbol include/fluidaudio_b200.h and include/FastClusterWrapper.h declare (tests check the export table)
 EXPORTED_SYMBOLS = [
     "fa_version", "fa_last_error", "fa_device_count", "fa_set_device", "fa_device_synchronize",
@@ -87,6 +98,9 @@ EXPORTED_SYMBOLS = [
     "fa_hungarian_solve", "fa_max_score_assignment", "fa_constrained_assign", "fa_build_chunk_assignments",
     "fa_export_shape", "fa_export_read", "fa_export_write", "fa_kmeans_cluster", "fa_speaker_constraints_resolve",
     "fa_reconstruct_default_config", "fa_build_segments", "fa_build_speaker_database",
+    "fa_seg_default_config", "fa_embed_plan_default_config", "fa_seg_window_count", "fa_seg_windows",
+    "fa_seg_windows_device", "fa_seg_decode", "fa_seg_decode_device", "fa_embedding_plan", "fa_embedding_plan_device",
+    "fa_embed_windows", "fa_embed_windows_device", "fa_weight_resample",
     "fastcluster_compute_centroid_linkage",
 ]
 
@@ -189,6 +203,21 @@ def load():
     L.fa_export_shape.argtypes = [C.c_char_p, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     L.fa_export_read.argtypes = [C.c_char_p, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.fa_export_write.argtypes = [C.c_char_p, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.fa_seg_default_config.argtypes = [C.POINTER(SegConfig)]
+    L.fa_seg_default_config.restype = None
+    L.fa_embed_plan_default_config.argtypes = [C.POINTER(EmbedPlanConfig)]
+    L.fa_embed_plan_default_config.restype = None
+    L.fa_seg_window_count.argtypes = [i64, C.POINTER(SegConfig), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
+    L.fa_seg_windows.argtypes = [vp, i64, C.POINTER(SegConfig), i32, i32, vp, vp]
+    L.fa_seg_windows_device.argtypes = L.fa_seg_windows.argtypes
+    L.fa_seg_decode.argtypes = [vp, i32, i32, i32, C.POINTER(SegConfig), vp, vp, vp, C.POINTER(i64)]
+    L.fa_seg_decode_device.argtypes = L.fa_seg_decode.argtypes
+    L.fa_embedding_plan.argtypes = [vp, i32, i32, i32, vp, i32, f64, i64, C.POINTER(SegConfig),
+                                    C.POINTER(EmbedPlanConfig)] + [vp] * 11 + [C.POINTER(i32), vp]
+    L.fa_embedding_plan_device.argtypes = L.fa_embedding_plan.argtypes
+    L.fa_embed_windows.argtypes = [vp, i64, vp, i32, vp, i32, C.POINTER(SegConfig), i32, vp]
+    L.fa_embed_windows_device.argtypes = L.fa_embed_windows.argtypes
+    L.fa_weight_resample.argtypes = [vp, i64, i32, i32, vp]
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

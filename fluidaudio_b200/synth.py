@@ -77,3 +77,63 @@ def synthetic_plda(emb: np.ndarray, rho_dim: int = 128, seed: int = 1234) -> tup
     rho = (unit - unit.mean(axis=0, keepdims=True)) @ W
     psi = (0.1 + 10.0 * np.exp(-np.arange(rho_dim) / 32.0)).astype(np.float32).astype(np.float64)
     return np.ascontiguousarray(rho), psi
+
+
+def segmentation_logits(duration_s: float, speakers: int = 3, seed: int = 5, frames: int = 589, classes: int = 7,
+                        sample_rate: int = 16000, window_duration: float = 10.0, step_ratio: float = 0.2,
+                        margin: float = 6.0, noise: float = 1.0) -> tuple[np.ndarray, dict]:
+    """Powerset logits a segmentation network could emit for a synthetic conversation, and the conversation itself.
+
+    A seeded turn-taking timeline (turns of 2.5-6 s, a third of them starting up to 1 s before the previous one ends, a
+    fifth preceded by 0.5-1.5 s of silence) is cut into the analysis windows of OfflineSegmentationProcessor (a window
+    every ``window_duration * step_ratio`` seconds, the last ones reaching past the end of the audio, where they are
+    silent).  Inside a window the global speakers take local slots 0..2 in order of first appearance (a fourth is
+    dropped, as a 3-speaker powerset model would); frame f is labelled by who speaks at offset + f * frame_duration, and
+    its logits are ``noise`` * N(0, 1) with ``margin`` added to the class of that speaker set.
+
+    Returns (logits float32 [chunks, frames, classes], truth) with truth = dict(turns float64 [n, 3] rows (speaker,
+    start, end), chunk_offsets, frame_duration, total_samples, slot_speaker int32 [chunks, 3] (global speaker of each
+    local slot, -1 = unused), labels int32 [chunks, frames] (the powerset class of every frame)).
+    """
+    rng = np.random.default_rng(seed)
+    turns, t, prev = [], 0.0, -1
+    while t < duration_s:
+        if turns and rng.random() < 0.2:
+            t += rng.uniform(0.5, 1.5)
+        elif turns and rng.random() < 1.0 / 3.0:
+            t -= rng.uniform(0.3, 1.0)
+        who = int(rng.integers(speakers))
+        if who == prev and speakers > 1:
+            who = (who + 1) % speakers
+        length = rng.uniform(2.5, 6.0)
+        if t < duration_s:
+            turns.append((who, max(t, 0.0), min(t + length, duration_s)))
+        t, prev = t + length, who
+    turns = np.asarray(turns, np.float64).reshape(-1, 3)
+    total_samples = int(round(duration_s * sample_rate))
+    window = int(sample_rate * window_duration)
+    step = max(1, int(window * step_ratio))
+    offsets = np.arange(0, total_samples, step, dtype=np.float64) / sample_rate
+    frame_duration = window_duration / frames
+    class_of_bits = np.array([0, 1, 2, 4, 3, 5, 6, 7])   # bit s = local speaker s -> {}, {0}, {1}, {0,1}, {2}, {0,2}, {1,2}, {0,1,2}
+    chunks = offsets.size
+    labels = np.zeros((chunks, frames), np.int32)
+    slot_speaker = np.full((chunks, 3), -1, np.int32)
+    for c, off in enumerate(offsets):
+        times = off + np.arange(frames) * frame_duration
+        active = np.zeros((frames, speakers), bool)
+        for who, a, b in turns[(turns[:, 2] > off) & (turns[:, 1] < off + window_duration)]:
+            active[:, int(who)] |= (times >= a) & (times < b) & (times < duration_s)
+        order = [k for k in np.argsort([np.argmax(active[:, k]) if active[:, k].any() else frames + k
+                                        for k in range(speakers)], kind="stable") if active[:, k].any()][:3]
+        slot_speaker[c, :len(order)] = order
+        who_bits = np.zeros(frames, np.int64)
+        for s, k in enumerate(order):
+            who_bits |= active[:, k].astype(np.int64) << s
+        labels[c] = np.minimum(class_of_bits[who_bits], classes - 1)
+    logits = (noise * rng.standard_normal((chunks, frames, classes))).astype(np.float32)
+    np.put_along_axis(logits, labels[..., None].astype(np.int64),
+                      np.take_along_axis(logits, labels[..., None].astype(np.int64), 2) + np.float32(margin), 2)
+    truth = dict(turns=turns, chunk_offsets=offsets, frame_duration=frame_duration, total_samples=total_samples,
+                 slot_speaker=slot_speaker, labels=labels)
+    return logits, truth

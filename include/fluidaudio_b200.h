@@ -26,6 +26,10 @@
  *                        KMeansClustering.swift:39-130,212-223, SpeakerCountConstraints.swift:27-85,
  *                        VBxClustering.swift:685-733 (refineWithConstraints)
  *   fa_build_segments    Diarizer/Offline/Utils/OfflineReconstruction.swift:24-253, 359-505
+ *   fa_seg_* / fa_embedding_plan / fa_embed_windows / fa_weight_resample
+ *                        Diarizer/Offline/Segmentation/OfflineSegmentationProcessor.swift:55-56,118-190,321-405,
+ *                        Diarizer/Offline/Extraction/OfflineEmbeddingExtractor.swift:421-707, WeightInterpolation.swift
+ *                        (the arithmetic of OfflineDiarizerManager.prepare around the two networks)
  *   fa_export_*          OfflineDiarizerManager.swift:913-955 (exportEmbeddings: the JSON dump of TimedEmbedding +
  *                        cluster, OfflineDiarizerTypes.swift:706-716) — the backend's on-disk input format
  */
@@ -383,7 +387,8 @@ fa_status fa_build_chunk_assignments(const int32_t *chunk_index, const int32_t *
  * fa_build_chunk_assignments [hard_rows x num_speakers] (-2 = inactive); centroid_count: centroids.count.
  * Output: *segment_count segments sorted by start (speakerId = "S<cluster+1>", embedding = centroid[cluster]); when
  * segment_cap is too small the first segment_cap are written and FA_STATUS_OUTPUT_TOO_SMALL is returned.  Host code; the
- * zero-vote re-embed pass (off by default, needs the embedding model) is not part of it. */
+ * zero-vote re-embed pass (off by default, needs the embedding model) is not part of it.  speaker_weights and
+ * chunk_offsets are what fa_seg_decode and fa_seg_windows produce. */
 typedef struct {
     double frame_duration, window_duration, min_gap_duration, seg_min_duration_off, seg_min_duration_on, min_segment_duration;
     int32_t exclusive_segments;
@@ -400,6 +405,94 @@ fa_status fa_build_segments(const float *speaker_weights, int32_t num_chunks, in
  * embeddings (a segment's embedding is Float(centroids[cluster])); segment_counts [K]; speakers without segment stay zero. */
 fa_status fa_build_speaker_database(const int32_t *seg_cluster, int32_t segment_count, const double *centroids, int32_t K,
                                     int32_t dim, float *database, int32_t *segment_counts);
+
+/* ---- offline diarization, prepare stage -------------------------------------------------------------------
+ * The arithmetic of OfflineDiarizerManager.prepare around the two networks (which run outside this library):
+ *   audio -> fa_seg_windows -> segmentation network -> fa_seg_decode -> fa_embedding_plan (+ fa_embed_windows)
+ *         -> embedding network, PLDA -> fa_diarize_cluster_chunks -> fa_build_chunk_assignments -> fa_build_segments.
+ * Reference (under Sources/FluidAudio/Diarizer/Offline): Segmentation/OfflineSegmentationProcessor.swift:55-56,118-190,
+ * 303,321-405; Extraction/OfflineEmbeddingExtractor.swift:338-351,381-387,421-707,807-842; Extraction/
+ * WeightInterpolation.swift:19-146; Utils/VDSPOperations.swift:142-155.
+ *
+ * Each call runs on a stream of the calling thread and has finished when it returns.  The `_device` twins take device
+ * pointers for the large buffers (audio, windows, logits, log-probabilities, weights and every per-entry output) and
+ * leave them on the device; work queued on other streams that produces their inputs must have finished before the
+ * call.  Small arrays (chunk offsets, chunk indices, the histogram, counts) are host memory in both.
+ * Weights, class histogram, entries, frames, times and both weight matrices equal the reference bit for bit for the
+ * binary weights fa_seg_decode produces; log-probabilities depend on expf / logf (Apple's vvexpf is closed) and sums of
+ * non-binary weights on a summation order (vDSP's is closed): both are "parity unpinned", see DESIGN §2. */
+typedef struct {
+    int32_t sample_rate;            /* 16000 */
+    float speech_onset_threshold;   /* 0.5 */
+    double window_duration;         /* 10.0 s */
+    double step_ratio;              /* 0.2, in (0, 1] */
+} fa_seg_config;
+typedef struct {
+    int32_t exclude_overlap;        /* 1: embeddingExcludeOverlap */
+    float skip_threshold;           /* EmbeddingSkipStrategy.maskSimilarity(threshold); < 0 = .none (default) */
+    double min_segment_duration;    /* 1.0 s */
+    int32_t weight_frames;          /* weightFrameCount of the embedding network: 589 */
+    int32_t audio_sample_count;     /* audioSampleCount of the fbank input: 160000 */
+    int32_t fbank_batch;            /* min(modelBatchLimit, 32): 32 */
+    int32_t reserved;
+} fa_embed_plan_config;
+void fa_seg_default_config(fa_seg_config *cfg);                 /* OfflineDiarizerConfig.Segmentation.community */
+void fa_embed_plan_default_config(fa_embed_plan_config *cfg);   /* OfflineDiarizerConfig.Embedding.community */
+
+/* samplesPerWindow, samplesPerStep and the number of windows stride(from: 0, to: total_samples, by: step) yields
+ * (0 for no samples).  Outputs may be NULL.  Host arithmetic. */
+fa_status fa_seg_window_count(int64_t total_samples, const fa_seg_config *cfg, int32_t *chunks, int64_t *window,
+                              int64_t *step);
+/* Windows first_chunk .. first_chunk + chunk_count - 1: out_windows [chunk_count x window], samples past the end of the
+ * audio zero; chunk_offsets [chunk_count] (host, may be NULL) = offset / sample_rate.  total_samples == 0 is the
+ * reference's noSpeechDetected: FA_STATUS_RUNTIME_ERROR.  One launch. */
+fa_status fa_seg_windows(const float *audio, int64_t total_samples, const fa_seg_config *cfg, int32_t first_chunk,
+                         int32_t chunk_count, float *out_windows, double *chunk_offsets);
+fa_status fa_seg_windows_device(const float *d_audio, int64_t total_samples, const fa_seg_config *cfg,
+                                int32_t first_chunk, int32_t chunk_count, float *d_out_windows, double *chunk_offsets);
+/* logits [chunks x frames x classes], classes 1 .. 16 (classes past the 8 powerset classes decode as class 7, as the
+ * reference does; a NaN logit never wins the argmax).  log_probs [chunks x frames x classes] (may be NULL);
+ * speaker_weights [chunks x frames x 3]; class_histogram [8] and speech_frames (host, may be NULL).  One launch. */
+fa_status fa_seg_decode(const float *logits, int32_t chunks, int32_t frames, int32_t classes, const fa_seg_config *cfg,
+                        float *log_probs, float *speaker_weights, int64_t *class_histogram, int64_t *speech_frames);
+fa_status fa_seg_decode_device(const float *d_logits, int32_t chunks, int32_t frames, int32_t classes,
+                               const fa_seg_config *cfg, float *d_log_probs, float *d_speaker_weights,
+                               int64_t *class_histogram, int64_t *speech_frames);
+/* Which (chunk, local speaker) pairs get an embedding, and with which weights.  speaker_weights [chunks x frames x
+ * speakers]; chunk_offsets (host) as in fa_build_segments: a missing or non-finite offset is chunk * window_duration;
+ * frame_duration <= 0 means window_duration / max(1, frames).  Entries come chunk-major, speaker-minor; each per-entry
+ * array has capacity chunks * speakers and may be NULL; rows of skipped pairs are not written.  reuse_of[i] is the entry
+ * whose embedding entry i reuses under the skip strategy, else -1.  frame_weights [entries x frames] is
+ * TimedEmbedding.frameWeights, model_weights [entries x weight_frames] the embedding network's weights input.
+ * counters [4] (host, may be NULL): masks evaluated, empty, fallback, skipped.  Two launches, three with the skip
+ * strategy.  frames * (speakers + 1) floats must fit a CTA's shared memory (FA_STATUS_UNSUPPORTED otherwise). */
+fa_status fa_embedding_plan(const float *speaker_weights, int32_t chunks, int32_t frames, int32_t speakers,
+                            const double *chunk_offsets, int32_t offsets_count, double frame_duration,
+                            int64_t total_samples, const fa_seg_config *seg_cfg, const fa_embed_plan_config *plan_cfg,
+                            int32_t *chunk_index, int32_t *speaker_index, int32_t *start_frame, int32_t *end_frame,
+                            double *start_time, double *end_time, float *mask_sum, int32_t *used_fallback,
+                            int32_t *reuse_of, float *frame_weights, float *model_weights, int32_t *entry_count,
+                            int64_t *counters);
+fa_status fa_embedding_plan_device(const float *d_speaker_weights, int32_t chunks, int32_t frames, int32_t speakers,
+                                   const double *chunk_offsets, int32_t offsets_count, double frame_duration,
+                                   int64_t total_samples, const fa_seg_config *seg_cfg,
+                                   const fa_embed_plan_config *plan_cfg, int32_t *d_chunk_index, int32_t *d_speaker_index,
+                                   int32_t *d_start_frame, int32_t *d_end_frame, double *d_start_time, double *d_end_time,
+                                   float *d_mask_sum, int32_t *d_used_fallback, int32_t *d_reuse_of,
+                                   float *d_frame_weights, float *d_model_weights, int32_t *entry_count,
+                                   int64_t *counters);
+/* The fbank input of chunks chunk_index[0 .. count) (host; NULL = chunks 0 .. count - 1): out [count x
+ * audio_sample_count], row i = min(chunk length, audio_sample_count) samples from round(offset * sample_rate) clamped
+ * to the audio, zeros after them (a chunk without audio gives a zero row).  One launch. */
+fa_status fa_embed_windows(const float *audio, int64_t total_samples, const double *chunk_offsets, int32_t offsets_count,
+                           const int32_t *chunk_index, int32_t count, const fa_seg_config *cfg,
+                           int32_t audio_sample_count, float *out);
+fa_status fa_embed_windows_device(const float *d_audio, int64_t total_samples, const double *chunk_offsets,
+                                  int32_t offsets_count, const int32_t *chunk_index, int32_t count,
+                                  const fa_seg_config *cfg, int32_t audio_sample_count, float *d_out);
+/* WeightInterpolation.resample2D: rows [row_count x in_len] -> out [row_count x out_len] (host buffers), the input
+ * itself when the lengths match.  Non-positive lengths give FA_STATUS_INVALID_ARGUMENT (the reference returns []). */
+fa_status fa_weight_resample(const float *rows, int64_t row_count, int32_t in_len, int32_t out_len, float *out);
 
 /* KMeansClustering.clusterWithCentroidsNInit (Diarizer/Offline/Clustering/KMeansClustering.swift:39-130) on raw
  * embeddings [N x D]: labels [N], centroids (normalised space) [min(num_clusters, N) x D] -> *centroid_rows rows;
