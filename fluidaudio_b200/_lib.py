@@ -80,6 +80,19 @@ class EmbedPlanConfig(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class SortformerConfig(C.Structure):
+    _fields_ = [("chunk_len", C.c_int32), ("chunk_left_context", C.c_int32), ("chunk_right_context", C.c_int32),
+                ("fifo_len", C.c_int32), ("spkcache_len", C.c_int32), ("spkcache_update_period", C.c_int32),
+                ("spkcache_sil_frames_per_spk", C.c_int32), ("silence_threshold", C.c_float),
+                ("pred_score_threshold", C.c_float), ("scores_boost_latest", C.c_float), ("strong_boost_rate", C.c_float),
+                ("weak_boost_rate", C.c_float), ("min_pos_scores_rate", C.c_float)]
+
+
+class SortformerSessionInfo(C.Structure):
+    _fields_ = [("spkcache_length", C.c_int32), ("fifo_length", C.c_int32), ("has_spkcache_preds", C.c_int32),
+                ("has_fifo_preds", C.c_int32), ("chunks", C.c_int64), ("silence_frames", C.c_int64)]
+
+
 # every symbol include/fluidaudio_b200.h and include/FastClusterWrapper.h declare (tests check the export table)
 EXPORTED_SYMBOLS = [
     "fa_version", "fa_last_error", "fa_device_count", "fa_set_device", "fa_device_synchronize",
@@ -101,6 +114,10 @@ EXPORTED_SYMBOLS = [
     "fa_seg_default_config", "fa_embed_plan_default_config", "fa_seg_window_count", "fa_seg_windows",
     "fa_seg_windows_device", "fa_seg_decode", "fa_seg_decode_device", "fa_embedding_plan", "fa_embedding_plan_device",
     "fa_embed_windows", "fa_embed_windows_device", "fa_weight_resample",
+    "fa_sortformer_default_config", "fa_sortformer_resolve_config", "fa_sortformer_step", "fa_sortformer_create",
+    "fa_sortformer_destroy", "fa_sortformer_open", "fa_sortformer_close", "fa_sortformer_update",
+    "fa_sortformer_update_device", "fa_sortformer_model_inputs", "fa_sortformer_model_inputs_device",
+    "fa_sortformer_session_state",
     "fastcluster_compute_centroid_linkage",
 ]
 
@@ -218,6 +235,20 @@ def load():
     L.fa_embed_windows.argtypes = [vp, i64, vp, i32, vp, i32, C.POINTER(SegConfig), i32, vp]
     L.fa_embed_windows_device.argtypes = L.fa_embed_windows.argtypes
     L.fa_weight_resample.argtypes = [vp, i64, i32, i32, vp]
+    SF = C.POINTER(SortformerConfig)
+    L.fa_sortformer_default_config.argtypes = [SF, i32]
+    L.fa_sortformer_resolve_config.argtypes = [SF, i32, SF, C.POINTER(i32)]
+    L.fa_sortformer_step.argtypes = [SF, i32, vp, i32, i32, i32, i32, vp]
+    L.fa_sortformer_create.argtypes = [SF, i32, C.POINTER(vp)]
+    L.fa_sortformer_destroy.argtypes = [vp]
+    L.fa_sortformer_destroy.restype = None
+    L.fa_sortformer_open.argtypes = [vp, C.POINTER(i32)]
+    L.fa_sortformer_close.argtypes = [vp, i32]
+    L.fa_sortformer_update.argtypes = [vp, i32, vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, vp, sz, vp, vp]
+    L.fa_sortformer_update_device.argtypes = L.fa_sortformer_update.argtypes
+    L.fa_sortformer_model_inputs.argtypes = [vp, i32, vp, vp, vp, vp, vp]
+    L.fa_sortformer_model_inputs_device.argtypes = L.fa_sortformer_model_inputs.argtypes
+    L.fa_sortformer_session_state.argtypes = [vp, i32, C.POINTER(SortformerSessionInfo), vp, vp, vp, vp, vp]
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

@@ -137,3 +137,38 @@ def segmentation_logits(duration_s: float, speakers: int = 3, seed: int = 5, fra
     truth = dict(turns=turns, chunk_offsets=offsets, frame_duration=frame_duration, total_samples=total_samples,
                  slot_speaker=slot_speaker, labels=labels)
     return logits, truth
+
+
+SORTFORMER_MODES = ("turns", "quantized", "silence", "never_silent")
+
+
+def sortformer_chunk(rng: np.random.Generator, mode: str, spkcache_length: int, fifo_length: int, core: int, lc: int,
+                     rc: int) -> tuple[np.ndarray, np.ndarray]:
+    """One Sortformer model output for a session holding ``spkcache_length`` + ``fifo_length`` state rows: (chunk
+    embeddings [lc + core + rc x 512], probabilities [spkcache + fifo + lc + core + rc x 4]), every row drawn afresh
+    (the model re-predicts the cache and FIFO rows each call).
+
+    ``turns``: speakers take turns with silence, single-speaker and overlapped stretches; ``quantized``: the same on a
+    1/8 grid (exact ties, exact 0.25 / 0.5 / 0.75); ``silence``: every frame's probabilities sum below 0.2;
+    ``never_silent``: some speaker is above 0.5 in every frame."""
+    rows = spkcache_length + fifo_length + lc + core + rc
+    emb = rng.normal(0.0, 1.0, size=(lc + core + rc, 512)).astype(np.float32)
+    if mode == "silence":
+        return emb, rng.uniform(0.0, 0.045, size=(rows, 4)).astype(np.float32)
+    state = rng.integers(0, 4, size=rows)   # 0 silence, 1 single speaker, 2 overlap, 3 single speaker (longer turns)
+    state = np.repeat(state[::3], 3)[:rows] if rows else state
+    who = np.repeat(rng.integers(0, 4, size=(rows + 4) // 4), 4)[:rows]
+    other = (who + 1 + rng.integers(0, 3, size=rows)) % 4
+    p = rng.uniform(0.0, 0.3, size=(rows, 4))
+    speak = state > 0
+    if mode == "never_silent":
+        speak[:] = True
+    idx = np.arange(rows)
+    p[~speak] = rng.uniform(0.0, 0.05, size=(int((~speak).sum()), 4))
+    p[idx[speak], who[speak]] = rng.uniform(0.55, 1.0, size=int(speak.sum()))
+    both = state == 2
+    p[idx[both], other[both]] = rng.uniform(0.5, 0.95, size=int(both.sum()))
+    if mode == "quantized":
+        p = np.round(p * 8.0) / 8.0
+        emb = np.round(emb * 4.0) / 4.0
+    return emb, p.astype(np.float32)

@@ -535,6 +535,97 @@ fa_status fa_diarize_cluster_batch_chunks(const float *emb256, const double *rho
                                           const fa_cluster_config *cfg, const int32_t *chunk_index, int32_t *labels,
                                           fa_cluster_info *infos);
 
+/* ---- Sortformer streaming state: SortformerStateUpdater.swift (Diarizer/Sortformer), the state of
+ * SortformerTypes.swift:270-327 and the padded model inputs of SortformerModelInference.swift:266-303, for many live
+ * sessions in HBM.  numSpeakers = 4, preEncoderDims = 512 and maxIndex = 99999 are constants, as in the reference.
+ *
+ * fa_sortformer_config holds the `var` fields of SortformerConfig (SortformerTypes.swift:31-97).
+ * fa_sortformer_default_config writes one of the reference's eight static configs (FA_SORTFORMER_*; an unknown preset
+ * gives FA_STATUS_INVALID_ARGUMENT).  fa_sortformer_resolve_config applies the init's clamps (chunkLen >= 1,
+ * spkcacheLen >= (1 + sil) * 4, update period in [chunkLen, fifoLen + chunkLen]) and create's checks: contexts, fifoLen
+ * and sil >= 0, finite thresholds and rates, and (spkcacheLen + fifoLen + max_core + sil) * 4 < maxIndex.  max_core
+ * (<= 0: chunkLen) is the largest coreFrames a push may carry; it sizes each session's FIFO (fifoLen + max_core rows) and
+ * speaker cache before compression (spkcacheLen + fifoLen + max_core rows).  Neither needs a device.
+ *
+ * fa_sortformer_step plans one streamingUpdate from lengths alone, as every push does per session before anything runs:
+ * lengths_in = {spkcacheLength, fifoLength, spkcachePreds exists}; out = {coreFrames, popOutLength (0: no overflow),
+ * compression, spkcacheLength, fifoLength, spkcachePreds exists} after it.  FA_STATUS_INVALID_ARGUMENT when the reference
+ * throws insufficientPredsLength / insufficientChunkLength (pred_rows < spkcache + fifo + lc + core + rc), a context is
+ * negative, or coreFrames = emb_length - lc - rc is outside [0, max_core].
+ *
+ * Sessions (like fa_mel_stream_*): fa_sortformer_open returns the lowest free id with a fresh state (empty cache and
+ * FIFO, no predictions, silence mean 0, count 0); close frees it.  Sessions and the handle are not thread-safe.
+ *
+ * fa_sortformer_update: session sessions[i] takes batch row i of the model's outputs, chunk_embs [count x emb_rows x
+ * 512] with emb_lengths[i] valid rows (chunk_pre_encoder_lengths, host memory), preds [count x pred_rows x 4]
+ * (probabilities) and left_context[i] / right_context[i].  NULL left_context is the streaming rule (chunk index > 0 ?
+ * chunkLeftContext : 0, SortformerDiarizer.swift:553); NULL right_context is chunkRightContext.  Each session runs
+ * streamingUpdate exactly: fifoPreds refresh, FIFO append, pop into the silence profile and the cache, compressSpkcache.
+ * Its confirmed rows [coreFrames x 4] and tentative rows [rc x 4] are packed in call order into confirmed / tentative
+ * (*_len floats); confirmed_rows[i] / tentative_rows[i] receive the counts.  Duplicate or closed sessions, the step's
+ * errors above and outputs too small give FA_STATUS_INVALID_ARGUMENT before any state changes.  One push is one
+ * descriptor upload and ONE kernel launch whatever the count (host variant: plus its copies and one synchronisation).
+ * fa_sortformer_update_device takes d_chunk_embs / d_preds / d_confirmed / d_tentative in HBM and is asynchronous on the
+ * handle's stream (the row counts are returned on return).
+ *
+ * fa_sortformer_model_inputs: the next model call's inputs for count sessions: spkcache [count x spkcacheLen x 512] and
+ * fifo [count x fifoLen x 512], rows [0, length) of the state then zeros; the lengths go to spkcache_lengths /
+ * fifo_lengths (host, may be NULL).  ONE kernel launch; _device writes d_spkcache / d_fifo asynchronously.
+ *
+ * fa_sortformer_session_state reads one session back (tests, checkpoints, inspection): spkcache [spkcacheLength x 512],
+ * spkcache_preds [spkcacheLength x 4] (written only when info->has_spkcache_preds), fifo [fifoLength x 512], fifo_preds
+ * [fifoLength x 4], mean_silence [512]; any pointer may be NULL.  Synchronous. */
+enum {
+    FA_SORTFORMER_DEFAULT = 0,
+    FA_SORTFORMER_FAST_V2 = 1,
+    FA_SORTFORMER_FAST_V2_1 = 2,
+    FA_SORTFORMER_BALANCED_V2 = 3,
+    FA_SORTFORMER_BALANCED_V2_1 = 4,
+    FA_SORTFORMER_HIGH_CONTEXT_V2 = 5,
+    FA_SORTFORMER_HIGH_CONTEXT_V2_1 = 6,
+    FA_SORTFORMER_EFFICIENT_V2_1 = 7,
+};
+typedef struct {
+    int32_t chunk_len, chunk_left_context, chunk_right_context, fifo_len, spkcache_len, spkcache_update_period,
+        spkcache_sil_frames_per_spk;
+    float silence_threshold, pred_score_threshold, scores_boost_latest, strong_boost_rate, weak_boost_rate,
+        min_pos_scores_rate;
+} fa_sortformer_config;
+typedef struct {
+    int32_t spkcache_length, fifo_length, has_spkcache_preds, has_fifo_preds;
+    int64_t chunks, silence_frames;
+} fa_sortformer_session_info;
+typedef struct fa_sortformer fa_sortformer;
+
+fa_status fa_sortformer_default_config(fa_sortformer_config *cfg, int32_t preset);
+fa_status fa_sortformer_resolve_config(const fa_sortformer_config *cfg, int32_t max_core_frames,
+                                       fa_sortformer_config *resolved, int32_t *resolved_max_core);
+fa_status fa_sortformer_step(const fa_sortformer_config *cfg, int32_t max_core_frames, const int32_t *lengths_in,
+                             int32_t emb_length, int32_t pred_rows, int32_t left_context, int32_t right_context,
+                             int32_t *out);
+fa_status fa_sortformer_create(const fa_sortformer_config *cfg, int32_t max_core_frames, fa_sortformer **out);
+void fa_sortformer_destroy(fa_sortformer *h);
+fa_status fa_sortformer_open(fa_sortformer *h, int32_t *session);
+fa_status fa_sortformer_close(fa_sortformer *h, int32_t session);
+fa_status fa_sortformer_update(fa_sortformer *h, int32_t count, const int32_t *sessions, const float *chunk_embs,
+                               int32_t emb_rows, const float *preds, int32_t pred_rows, const int32_t *emb_lengths,
+                               const int32_t *left_context, const int32_t *right_context, float *confirmed,
+                               size_t confirmed_len, float *tentative, size_t tentative_len, int64_t *confirmed_rows,
+                               int64_t *tentative_rows);
+fa_status fa_sortformer_update_device(fa_sortformer *h, int32_t count, const int32_t *sessions,
+                                      const float *d_chunk_embs, int32_t emb_rows, const float *d_preds,
+                                      int32_t pred_rows, const int32_t *emb_lengths, const int32_t *left_context,
+                                      const int32_t *right_context, float *d_confirmed, size_t confirmed_len,
+                                      float *d_tentative, size_t tentative_len, int64_t *confirmed_rows,
+                                      int64_t *tentative_rows);
+fa_status fa_sortformer_model_inputs(fa_sortformer *h, int32_t count, const int32_t *sessions, float *spkcache,
+                                     float *fifo, int32_t *spkcache_lengths, int32_t *fifo_lengths);
+fa_status fa_sortformer_model_inputs_device(fa_sortformer *h, int32_t count, const int32_t *sessions, float *d_spkcache,
+                                            float *d_fifo, int32_t *spkcache_lengths, int32_t *fifo_lengths);
+fa_status fa_sortformer_session_state(fa_sortformer *h, int32_t session, fa_sortformer_session_info *info,
+                                      float *spkcache, float *spkcache_preds, float *fifo, float *fifo_preds,
+                                      float *mean_silence);
+
 #ifdef __cplusplus
 }
 #endif
