@@ -79,7 +79,6 @@ static int create_timer(Event (&ev)[2]) {
 struct MelHandle {
     mel::MelPlan plan;
     mel::MelStreamSet sessions;   // fa_mel_stream_*: live streams on this plan
-    int device = 0;
 };
 
 } // namespace fa
@@ -234,7 +233,6 @@ static fa_status create_mel(const mel::MelConfig &c, fa_mel **out) {
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
     std::unique_ptr<MelHandle> h(new MelHandle());
-    FA_CUDA_TRY(cudaGetDevice(&h->device));
     const int st = h->plan.init(c);
     if (st != FA_OK) return (fa_status)st;
     *out = reinterpret_cast<fa_mel *>(h.release());

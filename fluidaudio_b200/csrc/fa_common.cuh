@@ -129,6 +129,27 @@ int carve_arena(GrowBuffer<T, Pinned> &buf, Layout &&layout, size_t slack = 0) {
     return FA_OK;
 }
 
+// Moves a session set's two per-slot device arrays (a_slot and b_slot elements per slot) into buffers of `grown` slots,
+// keeping the first `slots`.  Both are allocated before anything is copied: a failed allocation changes neither.  The
+// copies queue behind the set's pushes on `stream` and complete before the swap.
+template <typename A, typename B>
+int grow_slots(int slots, int grown, cudaStream_t stream, DeviceBuffer<A> &a, size_t a_slot, DeviceBuffer<B> &b,
+               size_t b_slot) {
+    DeviceBuffer<A> na;
+    DeviceBuffer<B> nb;
+    int st = na.grow((size_t)grown * a_slot * sizeof(A));
+    if (st == FA_OK) st = nb.grow((size_t)grown * b_slot * sizeof(B));
+    if (st != FA_OK) return st;
+    if (slots) {
+        FA_CUDA_TRY(cudaMemcpyAsync(na.data(), a.data(), (size_t)slots * a_slot * sizeof(A), cudaMemcpyDeviceToDevice, stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(nb.data(), b.data(), (size_t)slots * b_slot * sizeof(B), cudaMemcpyDeviceToDevice, stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(stream));
+    }
+    a = std::move(na);
+    b = std::move(nb);
+    return FA_OK;
+}
+
 // Owned stream and event: empty until create() succeeds, and usable wherever the raw handle is.
 struct StreamDestroy {
     void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }

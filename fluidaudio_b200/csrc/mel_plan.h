@@ -5,6 +5,7 @@
 #include "fa_common.cuh"
 #include "mel_tables.h"
 #include "resample_plan.h"
+#include "session_table.h"
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <limits>
@@ -152,13 +153,17 @@ constexpr long long kUnchecked = std::numeric_limits<long long>::max();   // bat
 // advances any number of sessions with one ingest launch and one mel launch.
 struct MelStreamJob;
 
+// A session's host counters: samples carried in d_carry, real samples received, frames emitted, finished.
+struct MelSession {
+    long long carry_len, received, emitted;
+    bool finished;
+};
+
 struct MelStreamSet {
     int capacity = 0;                    // floats per session in d_carry: round_up4(nFFT/2 + win/2)
-    int slots = 0;                       // sessions d_carry / d_last hold
+    SessionTable<MelSession> table;
     DeviceBuffer<float> d_carry;         // [slots x capacity]
     DeviceBuffer<float> d_last;          // [slots] lastAudioSample
-    std::vector<long long> carry_len, received, emitted;
-    std::vector<uint8_t> live, finished;
     // push staging: descriptors (units, then jobs) and the arena the ingest kernel assembles every emitting session's
     // contiguous input in
     UploadStage<> desc;
@@ -167,7 +172,6 @@ struct MelStreamSet {
     static int check_config(const MelConfig &c);   // pad_to <= 1 and hop <= win, or FA_INVALID_ARGUMENT
     int open(MelPlan &p, int *session);
     int close(int session);
-    bool valid(int session) const { return session >= 0 && session < slots && live[session]; }
     // rows the next push of `n` samples (finish 0/1) to `session` emits
     long long frames(const MelPlan &p, int session, long long n, bool finish) const;
     // Session sessions[i] receives audio[offsets[i] .. offsets[i+1]); its frames[i] rows start at row sum_{j<i} frames[j]

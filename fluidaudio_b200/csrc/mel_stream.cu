@@ -86,13 +86,12 @@ static inline long long round_up4(long long v) { return (v + 3) & ~3LL; }
 
 // Frames of one push: `first` from addAudio's preprocessAudioToFeaturesLocked (:847-854), `second` from
 // padAndEmitRemainingMelLocked (:876-883) when the push finishes the session.  Integer division truncates like Swift's.
-static void push_frames(const MelConfig &c, long long received, long long emitted, bool finished, long long n, bool fin,
-                        long long &first, long long &second) {
+static void push_frames(const MelConfig &c, const MelSession &m, long long n, bool fin, long long &first, long long &second) {
     first = second = 0;
-    if (finished) return;   // shouldDropAudioLocked
-    const long long r = received + n, half_win = c.win_length / 2;
-    if (r >= half_win) first = std::max(0LL, (r - half_win) / c.hop_length + 1 - emitted);
-    if (fin && r > 0) second = std::max(0LL, 1 + (r + c.n_fft - c.win_length) / c.hop_length - emitted - first);
+    if (m.finished) return;   // shouldDropAudioLocked
+    const long long r = m.received + n, half_win = c.win_length / 2;
+    if (r >= half_win) first = std::max(0LL, (r - half_win) / c.hop_length + 1 - m.emitted);
+    if (fin && r > 0) second = std::max(0LL, 1 + (r + c.n_fft - c.win_length) / c.hop_length - m.emitted - first);
 }
 
 int MelStreamSet::check_config(const MelConfig &c) {
@@ -117,53 +116,23 @@ int MelStreamSet::open(MelPlan &p, int *session) {
     const int half = p.cfg.n_fft / 2;
     capacity = (int)round_up4(half + p.cfg.win_length / 2);
     cudaStream_t s = p.streams[1];
-    int id = 0;
-    while (id < slots && live[id]) ++id;   // ids are dense from 0: the lowest closed one is reused
-    if (id == slots) {
-        // grow into fresh buffers, keeping the live sessions' carries and `last` (queued pushes finish first: same
-        // stream); a failure leaves the live sessions as they were
-        const int grown = std::max(64, 2 * slots);
-        DeviceBuffer<float> c, l;
-        st = c.grow((size_t)grown * capacity * sizeof(float));
-        if (st == FA_OK) st = l.grow((size_t)grown * sizeof(float));
-        if (st != FA_OK) return st;
-        if (slots) {
-            FA_CUDA_TRY(cudaMemcpyAsync(c.data(), d_carry.data(), (size_t)slots * capacity * sizeof(float),
-                                        cudaMemcpyDeviceToDevice, s));
-            FA_CUDA_TRY(cudaMemcpyAsync(l.data(), d_last.data(), (size_t)slots * sizeof(float), cudaMemcpyDeviceToDevice, s));
-            FA_CUDA_TRY(cudaStreamSynchronize(s));
-        }
-        d_carry = std::move(c);
-        d_last = std::move(l);
-        slots = grown;
-        for (auto *v : {&carry_len, &received, &emitted}) v->resize(grown, 0);
-        live.resize(grown, 0);
-        finished.resize(grown, 0);
-    }
+    auto grow = [&](int grown) { return grow_slots(table.slots(), grown, s, d_carry, capacity, d_last, 1); };
     // resetMelStreamLocked (:204-217): the buffer is nFFT/2 zeros, lastAudioSample 0, counters cleared
-    FA_CUDA_TRY(cudaMemsetAsync(d_carry.data() + (size_t)id * capacity, 0, (size_t)half * sizeof(float), s));
-    FA_CUDA_TRY(cudaMemsetAsync(d_last.data() + id, 0, sizeof(float), s));
-    carry_len[id] = half;
-    received[id] = emitted[id] = 0;
-    finished[id] = 0;
-    live[id] = 1;
-    *session = id;
-    return FA_OK;
+    auto init = [&](int id) -> int {
+        FA_CUDA_TRY(cudaMemsetAsync(d_carry.data() + (size_t)id * capacity, 0, (size_t)half * sizeof(float), s));
+        FA_CUDA_TRY(cudaMemsetAsync(d_last.data() + id, 0, sizeof(float), s));
+        table[id].carry_len = half;
+        return FA_OK;
+    };
+    return table.open(64, grow, init, session);
 }
 
-int MelStreamSet::close(int session) {
-    if (!valid(session)) {
-        fa::set_error("mel stream: session %d is not open", session);
-        return FA_INVALID_ARGUMENT;
-    }
-    live[session] = 0;
-    return FA_OK;
-}
+int MelStreamSet::close(int session) { return table.close(session, "mel stream"); }
 
 long long MelStreamSet::frames(const MelPlan &p, int session, long long n, bool finish) const {
-    if (!valid(session) || n < 0) return -1;
+    if (!table.valid(session) || n < 0) return -1;
     long long first, second;
-    push_frames(p.cfg, received[session], emitted[session], finished[session] != 0, n, finish, first, second);
+    push_frames(p.cfg, table[session], n, finish, first, second);
     return first + second;
 }
 
@@ -176,28 +145,17 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         return FA_INVALID_ARGUMENT;
     }
     if (count == 0) return FA_OK;
-    // every argument is checked before any state changes: a failed push leaves every session as it was
     if (offsets[0] < 0) {
         fa::set_error("mel stream push: offsets[0] is negative (%lld)", offsets[0]);
         return FA_INVALID_ARGUMENT;
     }
-    std::vector<uint8_t> seen(slots, 0);
-    for (int i = 0; i < count; ++i) {
-        const int id = sessions[i];
-        if (!valid(id)) {
-            fa::set_error("mel stream push: session %d is not open", id);
-            return FA_INVALID_ARGUMENT;
-        }
-        if (seen[id]) {
-            fa::set_error("mel stream push: session %d appears twice", id);
-            return FA_INVALID_ARGUMENT;
-        }
-        seen[id] = 1;
+    int st = table.check(count, sessions, "mel stream push");
+    if (st != FA_OK) return st;
+    for (int i = 0; i < count; ++i)
         if (offsets[i + 1] < offsets[i]) {
             fa::set_error("mel stream push: offsets decrease at %d (%lld > %lld)", i, offsets[i], offsets[i + 1]);
             return FA_INVALID_ARGUMENT;
         }
-    }
     const long long total_new = offsets[count] - offsets[0];
     if (total_new > 0 && !audio) {
         fa::set_error("mel stream push: audio is null");
@@ -208,19 +166,22 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         bool fin;
     };
     std::vector<Step> step(count);
+    std::vector<MelSession> next(count);
     long long rows = 0, arena = 0;
     int units = 0, jobs = 0;
     const long long bound = half + c.win_length / 2;   // carried samples stay below this (DESIGN §4.1c)
     for (int i = 0; i < count; ++i) {
         const int id = sessions[i];
+        const MelSession &m = table[id];
         Step &S = step[i];
         const long long n = offsets[i + 1] - offsets[i];
         S.fin = finish && finish[i];
-        push_frames(c, received[id], emitted[id], finished[id] != 0, n, S.fin, S.first, S.second);
-        S.L = carry_len[id] + n;
+        push_frames(c, m, n, S.fin, S.first, S.second);
+        S.L = m.carry_len + n;
         rows += S.first + S.second;
-        if (finished[id]) continue;
         const long long consumed = S.first * hop, tail = S.second ? half : 0;
+        next[i] = m.finished ? m : MelSession{S.L - consumed, m.received + n, m.emitted + S.first + S.second, S.fin};
+        if (m.finished) continue;
         if (consumed > S.L || (!S.fin && S.L - consumed >= bound)) {
             fa::set_error("internal: mel stream carry bound (session %d: %lld samples, %lld consumed)", id, S.L, consumed);
             return FA_RUNTIME_ERROR;
@@ -242,7 +203,7 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     // ---- buffers
     const size_t units_bytes = (((size_t)units * sizeof(MelUnit)) + 15) & ~size_t(15);
     const size_t desc_bytes = units_bytes + (size_t)jobs * sizeof(MelStreamJob);
-    int st = desc.reserve(std::max<size_t>(desc_bytes, 4096));
+    st = desc.reserve(std::max<size_t>(desc_bytes, 4096));
     if (st == FA_OK) st = d_arena.grow((size_t)std::max(arena, 1024LL) * sizeof(float));
     if (st == FA_OK && !device) st = p.ensure_staging((size_t)std::max(total_new, 0LL) + 8, (size_t)rows * M);
     if (st != FA_OK) return st;
@@ -259,9 +220,9 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         const int id = sessions[i];
         const Step &S = step[i];
         const long long n = offsets[i + 1] - offsets[i], emit = S.first + S.second;
-        if (finished[id] || (emit == 0 && (n == 0 || S.fin))) continue;
+        if (table[id].finished || (emit == 0 && (n == 0 || S.fin))) continue;
         MelStreamJob &J = hj[j++];
-        J = MelStreamJob{offsets[i] - src0, n, -1, -1, id, (int)carry_len[id], 0, 0, -1, S.fin ? 1 : 0};
+        J = MelStreamJob{offsets[i] - src0, n, -1, -1, id, (int)table[id].carry_len, 0, 0, -1, S.fin ? 1 : 0};
         if (emit == 0) continue;
         const bool split = S.first > 0 && S.second > 0;
         J.consumed = (int)(S.first * hop);
@@ -310,17 +271,8 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         FA_CUDA_TRY(cudaStreamSynchronize(s));
     }
 
-    // ---- commit the host-side state
-    for (int i = 0; i < count; ++i) {
-        const int id = sessions[i];
-        const Step &S = step[i];
-        frames_out[i] = S.first + S.second;
-        if (finished[id]) continue;
-        received[id] += offsets[i + 1] - offsets[i];
-        emitted[id] += S.first + S.second;
-        carry_len[id] = S.L - S.first * hop;
-        if (S.fin) finished[id] = 1;
-    }
+    table.commit(count, sessions, next.data());
+    for (int i = 0; i < count; ++i) frames_out[i] = step[i].first + step[i].second;
     return FA_OK;
 }
 

@@ -3,10 +3,8 @@
 #pragma once
 
 #include "fa_common.cuh"
+#include "session_table.h"
 #include "sortformer_core.cuh"
-
-#include <cstdint>
-#include <vector>
 
 namespace fa {
 namespace sortformer {
@@ -66,10 +64,15 @@ struct SessionInfo {
     long long chunks, silence_frames;
 };
 
+// A session's host mirror (sortformer_streams.cu): parity is the current cache buffer, chunks the updates so far.
+struct SortformerSession {
+    int spk_len, fifo_len, fifo_head, parity, has_preds;
+    long long chunks;
+};
+
 class SortformerSet {
   public:
     Config cfg{};
-    int device = 0;
 
     int init(const Config &resolved);
     int open(int *session);
@@ -82,20 +85,15 @@ class SortformerSet {
                      int *fifo_lengths);
     int state(int session, SessionInfo *info, float *spkcache, float *spkcache_preds, float *fifo, float *fifo_preds,
               float *mean);
-    bool valid(int id) const { return id >= 0 && id < slots && live[id]; }
 
   private:
     Arena arena{};
     Stream stream;
-    int slots = 0;
+    SessionTable<SortformerSession> table;
     DeviceBuffer<float> d_state;
     DeviceBuffer<long long> d_silence;
     UploadStage<> update_desc, input_desc;
     DeviceBuffer<float> d_embs, d_preds, d_out, d_inputs;   // staging of the host-buffer variants
-    std::vector<int> spk_len, fifo_len, fifo_head, parity, has_preds;
-    std::vector<long long> chunks;
-    std::vector<uint8_t> live;
-    int check_sessions(int count, const int *sessions, const char *where) const;
 };
 
 } // namespace sortformer

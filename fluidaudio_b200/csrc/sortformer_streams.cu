@@ -106,73 +106,24 @@ int plan_step(const Config &c, int spk, int fifo, int has_preds, int emb_length,
 int SortformerSet::init(const Config &resolved) {
     cfg = resolved;
     arena.init(cfg);
-    FA_CUDA_TRY(cudaGetDevice(&device));
     int st = stream.create();
     if (st == FA_OK) st = set_update_smem(cfg);
     return st;
 }
 
 int SortformerSet::open(int *session) {
-    int id = 0;
-    while (id < slots && live[id]) ++id;   // ids are dense from 0: the lowest closed one is reused
-    if (id == slots) {
-        // grow into fresh buffers, keeping the live sessions (queued pushes finish first: same stream); a failure
-        // leaves them as they were
-        const int grown = std::max(16, 2 * slots);
-        DeviceBuffer<float> s;
-        DeviceBuffer<long long> n;
-        int st = s.grow((size_t)grown * arena.stride * sizeof(float));
-        if (st == FA_OK) st = n.grow((size_t)grown * sizeof(long long));
-        if (st != FA_OK) return st;
-        if (slots) {
-            FA_CUDA_TRY(cudaMemcpyAsync(s.data(), d_state.data(), (size_t)slots * arena.stride * sizeof(float),
-                                        cudaMemcpyDeviceToDevice, stream));
-            FA_CUDA_TRY(cudaMemcpyAsync(n.data(), d_silence.data(), (size_t)slots * sizeof(long long),
-                                        cudaMemcpyDeviceToDevice, stream));
-            FA_CUDA_TRY(cudaStreamSynchronize(stream));
-        }
-        d_state = std::move(s);
-        d_silence = std::move(n);
-        slots = grown;
-        for (auto *v : {&spk_len, &fifo_len, &fifo_head, &parity, &has_preds}) v->resize(grown, 0);
-        chunks.resize(grown, 0);
-        live.resize(grown, 0);
-    }
+    auto grow = [&](int grown) { return grow_slots(table.slots(), grown, stream, d_state, arena.stride, d_silence, 1); };
     // SortformerStreamingState.init (SortformerTypes.swift:301-315): empty cache and FIFO, no predictions, mean zero
-    FA_CUDA_TRY(cudaMemsetAsync(d_state.data() + (size_t)id * arena.stride + arena.mean, 0, kDims * sizeof(float), stream));
-    FA_CUDA_TRY(cudaMemsetAsync(d_silence.data() + id, 0, sizeof(long long), stream));
-    spk_len[id] = fifo_len[id] = fifo_head[id] = parity[id] = has_preds[id] = 0;
-    chunks[id] = 0;
-    live[id] = 1;
-    *session = id;
-    return FA_OK;
+    auto init = [&](int id) -> int {
+        FA_CUDA_TRY(cudaMemsetAsync(d_state.data() + (size_t)id * arena.stride + arena.mean, 0, kDims * sizeof(float),
+                                    stream));
+        FA_CUDA_TRY(cudaMemsetAsync(d_silence.data() + id, 0, sizeof(long long), stream));
+        return FA_OK;
+    };
+    return table.open(16, grow, init, session);
 }
 
-int SortformerSet::close(int session) {
-    if (!valid(session)) {
-        fa::set_error("sortformer: session %d is not open", session);
-        return FA_INVALID_ARGUMENT;
-    }
-    live[session] = 0;
-    return FA_OK;
-}
-
-int SortformerSet::check_sessions(int count, const int *sessions, const char *where) const {
-    std::vector<uint8_t> seen(slots, 0);
-    for (int i = 0; i < count; ++i) {
-        const int id = sessions[i];
-        if (!valid(id)) {
-            fa::set_error("%s: session %d is not open", where, id);
-            return FA_INVALID_ARGUMENT;
-        }
-        if (seen[id]) {
-            fa::set_error("%s: session %d appears twice", where, id);
-            return FA_INVALID_ARGUMENT;
-        }
-        seen[id] = 1;
-    }
-    return FA_OK;
-}
+int SortformerSet::close(int session) { return table.close(session, "sortformer"); }
 
 int SortformerSet::update(int count, const int *sessions, const float *embs, int emb_rows, const float *preds,
                           int pred_rows, const int *emb_lengths, const int *left, const int *right, bool on_device,
@@ -185,24 +136,27 @@ int SortformerSet::update(int count, const int *sessions, const float *embs, int
         return FA_INVALID_ARGUMENT;
     }
     if (count == 0) return FA_OK;
-    // every argument is checked before any state changes: a failed push leaves every session as it was
-    int st = check_sessions(count, sessions, "sortformer update");
+    int st = table.check(count, sessions, "sortformer update");
     if (st != FA_OK) return st;
     std::vector<Step> step(count);
+    std::vector<SortformerSession> next(count);
     std::vector<int> lcs(count), rcs(count);
     long long conf = 0, tent = 0;
     for (int i = 0; i < count; ++i) {
-        const int id = sessions[i];
+        const SortformerSession &m = table[sessions[i]];
         // SortformerDiarizer.swift:553-554: the streaming rule when no context is given
-        lcs[i] = left ? left[i] : (chunks[id] > 0 ? cfg.left_context : 0);
+        lcs[i] = left ? left[i] : (m.chunks > 0 ? cfg.left_context : 0);
         rcs[i] = right ? right[i] : cfg.right_context;
         if (emb_lengths[i] > emb_rows) {
             fa::set_error("sortformer update: emb_lengths[%d] = %d exceeds emb_rows %d", i, emb_lengths[i], emb_rows);
             return FA_INVALID_ARGUMENT;
         }
-        st = plan_step(cfg, spk_len[id], fifo_len[id], has_preds[id], emb_lengths[i], pred_rows, lcs[i], rcs[i], step[i]);
+        st = plan_step(cfg, m.spk_len, m.fifo_len, m.has_preds, emb_lengths[i], pred_rows, lcs[i], rcs[i], step[i]);
         if (st != FA_OK) return st;
-        conf += step[i].core;
+        const Step &S = step[i];
+        next[i] = SortformerSession{S.spkcache_after, S.fifo_after, (m.fifo_head + S.pop) % cfg.fifo_rows(),
+                                    m.parity ^ S.compress, S.has_preds_after, m.chunks + 1};
+        conf += S.core;
         tent += rcs[i];
     }
     if ((conf > 0 && (!confirmed || confirmed_len < conf * kSpeakers)) ||
@@ -230,10 +184,11 @@ int SortformerSet::update(int count, const int *sessions, const float *embs, int
     long long co = 0, to = 0;
     for (int i = 0; i < count; ++i) {
         const int id = sessions[i];
+        const SortformerSession &m = table[id];
         const Step &S = step[i];
         hj[i] = UpdateJob{(long long)id * arena.stride, id, (long long)i * emb_rows * kDims,
-                          (long long)i * pred_rows * kSpeakers, co * kSpeakers, to * kSpeakers, spk_len[id], fifo_len[id],
-                          fifo_head[id], parity[id], lcs[i], rcs[i], S.core, S.pop, S.compress, S.init_preds};
+                          (long long)i * pred_rows * kSpeakers, co * kSpeakers, to * kSpeakers, m.spk_len, m.fifo_len,
+                          m.fifo_head, m.parity, lcs[i], rcs[i], S.core, S.pop, S.compress, S.init_preds};
         co += S.core;
         to += rcs[i];
     }
@@ -261,19 +216,10 @@ int SortformerSet::update(int count, const int *sessions, const float *embs, int
         FA_CUDA_TRY(cudaStreamSynchronize(stream));
     }
 
-    // ---- commit the host-side mirror
-    const int FR = cfg.fifo_rows();
+    table.commit(count, sessions, next.data());
     for (int i = 0; i < count; ++i) {
-        const int id = sessions[i];
-        const Step &S = step[i];
-        confirmed_rows[i] = S.core;
+        confirmed_rows[i] = step[i].core;
         tentative_rows[i] = rcs[i];
-        fifo_head[id] = (fifo_head[id] + S.pop) % FR;
-        fifo_len[id] = S.fifo_after;
-        spk_len[id] = S.spkcache_after;
-        has_preds[id] = S.has_preds_after;
-        parity[id] ^= S.compress;
-        ++chunks[id];
     }
     return FA_OK;
 }
@@ -285,7 +231,7 @@ int SortformerSet::model_inputs(int count, const int *sessions, bool on_device, 
         return FA_INVALID_ARGUMENT;
     }
     if (count == 0) return FA_OK;
-    int st = check_sessions(count, sessions, "sortformer model inputs");
+    int st = table.check(count, sessions, "sortformer model inputs");
     if (st != FA_OK) return st;
     const size_t desc_bytes = (size_t)count * sizeof(InputJob);
     const long long cache_floats = (long long)count * cfg.spkcache_len * kDims;
@@ -295,10 +241,10 @@ int SortformerSet::model_inputs(int count, const int *sessions, bool on_device, 
     if (st != FA_OK) return st;
     InputJob *hj = static_cast<InputJob *>(input_desc.host.data());
     for (int i = 0; i < count; ++i) {
-        const int id = sessions[i];
-        hj[i] = InputJob{(long long)id * arena.stride, spk_len[id], fifo_len[id], fifo_head[id], parity[id]};
-        if (spkcache_lengths) spkcache_lengths[i] = spk_len[id];
-        if (fifo_lengths) fifo_lengths[i] = fifo_len[id];
+        const SortformerSession &m = table[sessions[i]];
+        hj[i] = InputJob{(long long)sessions[i] * arena.stride, m.spk_len, m.fifo_len, m.fifo_head, m.parity};
+        if (spkcache_lengths) spkcache_lengths[i] = m.spk_len;
+        if (fifo_lengths) fifo_lengths[i] = m.fifo_len;
     }
     float *c_out = on_device ? spkcache : d_inputs.data();
     float *f_out = on_device ? fifo : d_inputs.data() + cache_floats;
@@ -317,20 +263,21 @@ int SortformerSet::model_inputs(int count, const int *sessions, bool on_device, 
 
 int SortformerSet::state(int session, SessionInfo *info, float *spkcache, float *spkcache_preds, float *fifo,
                          float *fifo_preds, float *mean) {
-    if (!valid(session) || !info) {
+    if (!table.valid(session) || !info) {
         fa::set_error("sortformer state: session %d is not open (or info is null)", session);
         return FA_INVALID_ARGUMENT;
     }
-    const int id = session, FR = cfg.fifo_rows(), head = fifo_head[id], n = fifo_len[id];
+    const SortformerSession &m = table[session];
+    const int id = session, FR = cfg.fifo_rows(), head = m.fifo_head, n = m.fifo_len;
     const float *st = d_state.data() + (size_t)id * arena.stride;
     auto d2h = [&](float *dst, const float *src, size_t floats) {
         return floats ? cudaMemcpyAsync(dst, src, floats * sizeof(float), cudaMemcpyDeviceToHost, stream) : cudaSuccess;
     };
     // the FIFO ring's rows [head, head + n) in two runs
     const int first = std::min(n, FR - head);
-    if (spkcache) FA_CUDA_TRY(d2h(spkcache, st + arena.cache[parity[id]], (size_t)spk_len[id] * kDims));
-    if (spkcache_preds && has_preds[id])
-        FA_CUDA_TRY(d2h(spkcache_preds, st + arena.cache_preds[parity[id]], (size_t)spk_len[id] * kSpeakers));
+    if (spkcache) FA_CUDA_TRY(d2h(spkcache, st + arena.cache[m.parity], (size_t)m.spk_len * kDims));
+    if (spkcache_preds && m.has_preds)
+        FA_CUDA_TRY(d2h(spkcache_preds, st + arena.cache_preds[m.parity], (size_t)m.spk_len * kSpeakers));
     if (fifo) {
         FA_CUDA_TRY(d2h(fifo, st + arena.fifo + (size_t)head * kDims, (size_t)first * kDims));
         FA_CUDA_TRY(d2h(fifo + (size_t)first * kDims, st + arena.fifo, (size_t)(n - first) * kDims));
@@ -343,7 +290,7 @@ int SortformerSet::state(int session, SessionInfo *info, float *spkcache, float 
     long long sil = 0;
     FA_CUDA_TRY(cudaMemcpyAsync(&sil, d_silence.data() + id, sizeof(long long), cudaMemcpyDeviceToHost, stream));
     FA_CUDA_TRY(cudaStreamSynchronize(stream));
-    *info = SessionInfo{spk_len[id], n, has_preds[id], chunks[id] > 0 ? 1 : 0, chunks[id], sil};
+    *info = SessionInfo{m.spk_len, n, m.has_preds, m.chunks > 0 ? 1 : 0, m.chunks, sil};
     return FA_OK;
 }
 
