@@ -93,6 +93,29 @@ class SortformerSessionInfo(C.Structure):
                 ("has_fifo_preds", C.c_int32), ("chunks", C.c_int64), ("silence_frames", C.c_int64)]
 
 
+class TimelineConfig(C.Structure):
+    _fields_ = [("num_speakers", C.c_int32), ("frame_duration_seconds", C.c_float), ("onset_threshold", C.c_float),
+                ("offset_threshold", C.c_float), ("onset_pad_frames", C.c_int32), ("offset_pad_frames", C.c_int32),
+                ("min_frames_on", C.c_int32), ("min_frames_off", C.c_int32), ("activity_type", C.c_int32),
+                ("max_stored_frames", C.c_int32)]
+
+
+class TimelineScratch(C.Structure):
+    _fields_ = [("start_frame", C.c_int64), ("end_frame", C.c_int64), ("unmerged_start_frame", C.c_int64),
+                ("active_frame_count", C.c_int64), ("unmerged_active_frame_count", C.c_int64),
+                ("activity_sum", C.c_float), ("unmerged_activity_sum", C.c_float), ("speaking", C.c_int32),
+                ("has_segment", C.c_int32)]
+
+
+class TimelineSessionInfo(C.Structure):
+    _fields_ = [("finalized_frames", C.c_int64), ("stored_frames", C.c_int64), ("tentative_frames", C.c_int64)]
+
+
+# fa_diarizer_timeline_segment as a numpy record
+TIMELINE_SEGMENT = np.dtype([("start_frame", np.int64), ("end_frame", np.int64), ("activity", np.float32),
+                             ("speaker", np.int32)])
+
+
 # every symbol include/fluidaudio_b200.h and include/FastClusterWrapper.h declare (tests check the export table)
 EXPORTED_SYMBOLS = [
     "fa_version", "fa_last_error", "fa_device_count", "fa_set_device", "fa_device_synchronize",
@@ -118,6 +141,11 @@ EXPORTED_SYMBOLS = [
     "fa_sortformer_destroy", "fa_sortformer_open", "fa_sortformer_close", "fa_sortformer_update",
     "fa_sortformer_update_device", "fa_sortformer_model_inputs", "fa_sortformer_model_inputs_device",
     "fa_sortformer_session_state",
+    "fa_diarizer_timeline_default_config", "fa_diarizer_timeline_config_from_seconds",
+    "fa_diarizer_timeline_segment_bound", "fa_diarizer_timeline_create", "fa_diarizer_timeline_destroy",
+    "fa_diarizer_timeline_open", "fa_diarizer_timeline_close", "fa_diarizer_timeline_push",
+    "fa_diarizer_timeline_push_device", "fa_diarizer_timeline_finalize", "fa_diarizer_timeline_reset",
+    "fa_diarizer_timeline_clear_speaker", "fa_diarizer_timeline_session_state",
     "fastcluster_compute_centroid_linkage",
 ]
 
@@ -249,6 +277,22 @@ def load():
     L.fa_sortformer_model_inputs.argtypes = [vp, i32, vp, vp, vp, vp, vp]
     L.fa_sortformer_model_inputs_device.argtypes = L.fa_sortformer_model_inputs.argtypes
     L.fa_sortformer_session_state.argtypes = [vp, i32, C.POINTER(SortformerSessionInfo), vp, vp, vp, vp, vp]
+    TC = C.POINTER(TimelineConfig)
+    L.fa_diarizer_timeline_default_config.argtypes = [TC, i32, i32, f32]
+    L.fa_diarizer_timeline_config_from_seconds.argtypes = [TC, f32, f32, f32, f32]
+    L.fa_diarizer_timeline_segment_bound.argtypes = [i32, i32, vp, vp, C.POINTER(i64), C.POINTER(i64)]
+    L.fa_diarizer_timeline_create.argtypes = [TC, i32, C.POINTER(vp)]
+    L.fa_diarizer_timeline_destroy.argtypes = [vp]
+    L.fa_diarizer_timeline_destroy.restype = None
+    L.fa_diarizer_timeline_open.argtypes = [vp, C.POINTER(i32)]
+    L.fa_diarizer_timeline_close.argtypes = [vp, i32]
+    L.fa_diarizer_timeline_push.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, sz, vp, sz, vp, vp]
+    L.fa_diarizer_timeline_push_device.argtypes = L.fa_diarizer_timeline_push.argtypes
+    L.fa_diarizer_timeline_finalize.argtypes = [vp, i32, vp]
+    L.fa_diarizer_timeline_reset.argtypes = [vp, i32, vp]
+    L.fa_diarizer_timeline_clear_speaker.argtypes = [vp, i32, i32]
+    L.fa_diarizer_timeline_session_state.argtypes = [vp, i32, C.POINTER(TimelineSessionInfo), vp, vp,
+                                                     C.POINTER(TimelineScratch)]
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

@@ -15,6 +15,7 @@
 #pragma once
 
 #include "fa_common.cuh"
+#include "fa_float.cuh"
 
 #include <cfloat>
 #include <cmath>
@@ -28,27 +29,7 @@ constexpr float kActiveThreshold = 1e-3f;   // overlapThreshold (:306), also fir
 constexpr float kMinActiveRatio = 0.2f;     // minActiveRatio (:519)
 constexpr int kSumLanes = 256;         // lanes of ordered_sum, = threads of a mask CTA
 
-#if defined(__CUDA_ARCH__)
-FA_HD float f_add(float a, float b) { return __fadd_rn(a, b); }
-FA_HD float f_sub(float a, float b) { return __fsub_rn(a, b); }
-FA_HD float f_mul(float a, float b) { return __fmul_rn(a, b); }
-FA_HD float f_div(float a, float b) { return __fdiv_rn(a, b); }
-FA_HD float f_sqrt(float a) { return __fsqrt_rn(a); }
-FA_HD double d_add(double a, double b) { return __dadd_rn(a, b); }
-FA_HD double d_mul(double a, double b) { return __dmul_rn(a, b); }
-#else
-FA_HD float f_add(float a, float b) { return a + b; }
-FA_HD float f_sub(float a, float b) { return a - b; }
-FA_HD float f_mul(float a, float b) { return a * b; }
-FA_HD float f_div(float a, float b) { return a / b; }
-FA_HD float f_sqrt(float a) { return std::sqrt(a); }
-FA_HD double d_add(double a, double b) { return a + b; }
-FA_HD double d_mul(double a, double b) { return a * b; }
-#endif
-
-// Swift.min(x, y) = y < x ? y : x and Swift.max(x, y) = y >= x ? y : x
-FA_HD float swift_min(float x, float y) { return y < x ? y : x; }
-FA_HD float swift_max(float x, float y) { return y >= x ? y : x; }
+using namespace fa::fp;   // f_* / d_* and swift_min / swift_max (fa_float.cuh)
 
 // Speakers of powerset class k as a bit mask (bit s = local speaker s).
 FA_HD unsigned powerset_speakers(int k) {

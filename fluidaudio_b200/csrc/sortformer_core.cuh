@@ -21,6 +21,7 @@
 #pragma once
 
 #include "fa_common.cuh"
+#include "fa_float.cuh"
 
 #include <cmath>
 
@@ -32,19 +33,7 @@ constexpr int kDims = 512;       // preEncoderDims (let)
 constexpr int kMaxIndex = 99999; // maxIndex (let)
 constexpr float kLn2 = 0.693147182f;   // logf(2) = -logf(0.5), correctly rounded
 
-#if defined(__CUDA_ARCH__)
-FA_HD float f_add(float a, float b) { return __fadd_rn(a, b); }
-FA_HD float f_sub(float a, float b) { return __fsub_rn(a, b); }
-FA_HD float f_mul(float a, float b) { return __fmul_rn(a, b); }
-FA_HD float f_div(float a, float b) { return __fdiv_rn(a, b); }
-#else
-FA_HD float f_add(float a, float b) { return a + b; }
-FA_HD float f_sub(float a, float b) { return a - b; }
-FA_HD float f_mul(float a, float b) { return a * b; }
-FA_HD float f_div(float a, float b) { return a / b; }
-#endif
-FA_HD float f_log(float x) { return (float)log((double)x); }
-FA_HD float f_log1p(float x) { return (float)log1p((double)x); }
+using namespace fa::fp;   // f_add / f_sub / f_mul / f_div / f_log / f_log1p (fa_float.cuh)
 
 // Resolved configuration: the fields of fa_sortformer_config after the init's clamps, plus the derived top-k sizes.
 struct Config {

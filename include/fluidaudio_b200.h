@@ -30,6 +30,7 @@
  *                        Diarizer/Offline/Segmentation/OfflineSegmentationProcessor.swift:55-56,118-190,321-405,
  *                        Diarizer/Offline/Extraction/OfflineEmbeddingExtractor.swift:421-707, WeightInterpolation.swift
  *                        (the arithmetic of OfflineDiarizerManager.prepare around the two networks)
+ *   fa_diarizer_timeline_*  Diarizer/DiarizerTimeline.swift:801-1336 (addChunk, finalize, reset, updateSegments)
  *   fa_export_*          OfflineDiarizerManager.swift:913-955 (exportEmbeddings: the JSON dump of TimedEmbedding +
  *                        cluster, OfflineDiarizerTypes.swift:706-716) — the backend's on-disk input format
  */
@@ -625,6 +626,113 @@ fa_status fa_sortformer_model_inputs_device(fa_sortformer *h, int32_t count, con
 fa_status fa_sortformer_session_state(fa_sortformer *h, int32_t session, fa_sortformer_session_info *info,
                                       float *spkcache, float *spkcache_preds, float *fifo, float *fifo_preds,
                                       float *mean_silence);
+
+/* ---- Diarizer timelines: the numeric core of DiarizerTimeline (Sources/FluidAudio/Diarizer/DiarizerTimeline.swift),
+ * which turns frame-wise speaker probabilities (Sortformer, LS-EEND, ...) into speech segments, for many live sessions
+ * in HBM.  Speaker identity (names, ids, enrollment) and the per-speaker segment lists stay with the caller, as in the
+ * reference's DiarizerSpeaker.  Unrelated to fa_build_segments, the offline diarizer's reconstruction.
+ *
+ * fa_diarizer_timeline_config holds DiarizerTimelineConfig's numeric fields (:9-164) with maxStoredFrames required
+ * (the reference's nil, unlimited, is not offered).  fa_diarizer_timeline_default_config writes a preset:
+ * FA_TIMELINE_PRESET_DEFAULT is default(numSpeakers:frameDurationSeconds:) with the given values, thresholds 0.5, no
+ * padding or minimum durations, sigmoids; FA_TIMELINE_PRESET_SORTFORMER is sortformerDefault (4 speakers, 0.08 s).
+ * Both store FA_TIMELINE_DEFAULT_STORED_FRAMES rows.  fa_diarizer_timeline_config_from_seconds sets the four frame
+ * counts from seconds as the seconds initialiser (:139-163) does: Int(round(seconds / frameDurationSeconds)) in float32,
+ * rounding half away from zero; FA_STATUS_INVALID_ARGUMENT when a result is not finite or outside int32 (Swift traps).
+ * Neither needs a device.
+ *
+ * fa_diarizer_timeline_create checks the config (numSpeakers in 1..32; pads and minimum durations >= 0; finite
+ * thresholds and frame duration; a known activity type; maxStoredFrames >= 0) and max_tentative_rows >= 0, the most
+ * tentative rows one push may carry per session.  Sessions (like fa_sortformer_*): fa_diarizer_timeline_open returns
+ * the lowest free id with a fresh timeline; close frees it.  Sessions and the handle are not thread-safe.
+ *
+ * fa_diarizer_timeline_push: session sessions[i] takes finalized_rows[i] rows of `finalized` and tentative_rows[i] rows
+ * of `tentative` ([rows x numSpeakers] each, packed in call order: the layout fa_sortformer_update[_device] writes, so
+ * its buffers and row counts pass straight through).  Each session runs addChunk (:827-872) exactly: the finalized rows
+ * join the stored predictions (trimmed to maxStoredFrames, skipped when it is 0), the tentative rows replace the
+ * session's, then updateSegments runs over the finalized rows from the finalized cursor, keeping its scratch, and over
+ * the tentative rows on a copy of it with the trailing tentative segment.  The new segments go to finalized_segments and
+ * tentative_segments; in each list a session's segments are speaker-major, then in frame order within a speaker, and
+ * sessions follow in call order; finalized_counts[i] / tentative_counts[i] receive each session's counts.  The outputs
+ * must hold the bound fa_diarizer_timeline_segment_bound gives for the row counts (*_capacity in segments).  Duplicate
+ * or closed sessions, more than max_tentative_rows tentative rows (or more than 2^30 finalized rows) in a session, and
+ * outputs below the bound give FA_STATUS_INVALID_ARGUMENT before any state changes.  One push is one descriptor upload
+ * and TWO kernel launches whatever the count; the host variant returns after at most two synchronisations, one for the
+ * counts and one for exactly the segments.
+ * fa_diarizer_timeline_push_device takes every row, segment and count buffer in HBM and is asynchronous on the
+ * handle's stream.  The input rows must be complete when it is called: rows another handle wrote (for instance
+ * fa_sortformer_update_device) are ready after fa_device_synchronize; the library does not order streams across handles.
+ *
+ * fa_diarizer_timeline_segment_bound: the segments a push of these row counts may emit, per list: a session of n
+ * finalized and m tentative rows contributes numSpeakers * (n > 0 ? n / 2 + 1 : 0) finalized and
+ * numSpeakers * ((m + 1) / 2 + 1) tentative segments.  No device.
+ *
+ * fa_diarizer_timeline_finalize (:877-891): each session's tentative rows join the stored ones and the finalized cursor
+ * passes them.  At most one kernel launch, none when no named session holds tentative rows.  The per-speaker move of
+ * tentative segments to finalized ones is the caller's.  fa_diarizer_timeline_reset (:921-934): no predictions,
+ * cursor 0, fresh scratches.  fa_diarizer_timeline_clear_speaker: a fresh scratch for one speaker slot, as
+ * removeSpeaker(clearCurrentSegment: true) and upsertSpeaker(transferCurrentSegment: false) do (:1108-1111,
+ * :1134-1136).  rebuild (:945-1003) is reset, push and, when isComplete, finalize.
+ *
+ * fa_diarizer_timeline_session_state reads one session back (tests, the caller's probability queries): info, the stored
+ * rows [stored_frames x numSpeakers] (frames finalized_frames - stored_frames .. finalized_frames - 1), the tentative
+ * rows [tentative_frames x numSpeakers] and the numSpeakers scratches; any pointer but info may be NULL.  Synchronous. */
+enum { FA_TIMELINE_SIGMOIDS = 0, FA_TIMELINE_LOGITS = 1 };
+enum { FA_TIMELINE_PRESET_DEFAULT = 0, FA_TIMELINE_PRESET_SORTFORMER = 1 };
+#define FA_TIMELINE_DEFAULT_STORED_FRAMES 7500
+typedef struct {
+    int32_t num_speakers;
+    float frame_duration_seconds, onset_threshold, offset_threshold;
+    int32_t onset_pad_frames, offset_pad_frames, min_frames_on, min_frames_off;
+    int32_t activity_type;       /* FA_TIMELINE_SIGMOIDS or FA_TIMELINE_LOGITS */
+    int32_t max_stored_frames;
+} fa_diarizer_timeline_config;
+typedef struct {
+    int64_t start_frame, end_frame;
+    float activity;
+    int32_t speaker;
+} fa_diarizer_timeline_segment;
+/* SegmentScratch (:649-661); a `.min` frame reads INT64_MIN */
+typedef struct {
+    int64_t start_frame, end_frame, unmerged_start_frame, active_frame_count, unmerged_active_frame_count;
+    float activity_sum, unmerged_activity_sum;
+    int32_t speaking, has_segment;
+} fa_diarizer_timeline_scratch;
+typedef struct {
+    int64_t finalized_frames, stored_frames, tentative_frames;
+} fa_diarizer_timeline_session_info;
+typedef struct fa_diarizer_timeline fa_diarizer_timeline;
+
+fa_status fa_diarizer_timeline_default_config(fa_diarizer_timeline_config *cfg, int32_t preset, int32_t num_speakers,
+                                              float frame_duration_seconds);
+fa_status fa_diarizer_timeline_config_from_seconds(fa_diarizer_timeline_config *cfg, float onset_pad_seconds,
+                                                   float offset_pad_seconds, float min_duration_on,
+                                                   float min_duration_off);
+fa_status fa_diarizer_timeline_segment_bound(int32_t num_speakers, int32_t count, const int64_t *finalized_rows,
+                                             const int64_t *tentative_rows, int64_t *finalized_bound,
+                                             int64_t *tentative_bound);
+fa_status fa_diarizer_timeline_create(const fa_diarizer_timeline_config *cfg, int32_t max_tentative_rows,
+                                      fa_diarizer_timeline **out);
+void fa_diarizer_timeline_destroy(fa_diarizer_timeline *h);
+fa_status fa_diarizer_timeline_open(fa_diarizer_timeline *h, int32_t *session);
+fa_status fa_diarizer_timeline_close(fa_diarizer_timeline *h, int32_t session);
+fa_status fa_diarizer_timeline_push(fa_diarizer_timeline *h, int32_t count, const int32_t *sessions,
+                                    const float *finalized, const int64_t *finalized_rows, const float *tentative,
+                                    const int64_t *tentative_rows, fa_diarizer_timeline_segment *finalized_segments,
+                                    size_t finalized_capacity, fa_diarizer_timeline_segment *tentative_segments,
+                                    size_t tentative_capacity, int64_t *finalized_counts, int64_t *tentative_counts);
+fa_status fa_diarizer_timeline_push_device(fa_diarizer_timeline *h, int32_t count, const int32_t *sessions,
+                                           const float *d_finalized, const int64_t *finalized_rows,
+                                           const float *d_tentative, const int64_t *tentative_rows,
+                                           fa_diarizer_timeline_segment *d_finalized_segments, size_t finalized_capacity,
+                                           fa_diarizer_timeline_segment *d_tentative_segments, size_t tentative_capacity,
+                                           int64_t *d_finalized_counts, int64_t *d_tentative_counts);
+fa_status fa_diarizer_timeline_finalize(fa_diarizer_timeline *h, int32_t count, const int32_t *sessions);
+fa_status fa_diarizer_timeline_reset(fa_diarizer_timeline *h, int32_t count, const int32_t *sessions);
+fa_status fa_diarizer_timeline_clear_speaker(fa_diarizer_timeline *h, int32_t session, int32_t speaker);
+fa_status fa_diarizer_timeline_session_state(fa_diarizer_timeline *h, int32_t session,
+                                             fa_diarizer_timeline_session_info *info, float *stored, float *tentative,
+                                             fa_diarizer_timeline_scratch *scratch);
 
 #ifdef __cplusplus
 }
