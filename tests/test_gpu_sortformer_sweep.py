@@ -13,6 +13,7 @@ import pytest
 
 from fluidaudio_b200 import _lib, synth
 from fluidaudio_b200.sortformer import SortformerConfig, SortformerStreams
+from sortformer_cases import Harness, chunks_needed, same_state
 
 D, S = 512, 4
 MODES = synth.SORTFORMER_MODES + ("offline",)
@@ -24,112 +25,6 @@ def O():
     oracle_sortformer.build()
     oracle_sortformer.lib()
     return oracle_sortformer
-
-
-def bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
-
-
-def chunks_needed(cfg, compressions=3):
-    first = cfg.spkcache_len + cfg.fifo_len + cfg.spkcache_update_period
-    return -(-(first + (compressions - 1) * cfg.spkcache_update_period) // cfg.chunk_len) + 2
-
-
-def same_state(a, b):
-    assert (a.spkcache_length, a.fifo_length, a.has_spkcache_preds, a.has_fifo_preds, a.silence_frames, a.chunks) == \
-        (b.spkcache_length, b.fifo_length, b.has_spkcache_preds, b.has_fifo_preds, b.silence_frames, b.chunks)
-    for k in ("spkcache", "fifo", "mean_silence"):
-        assert np.array_equal(bits(getattr(a, k)), bits(getattr(b, k))), k
-    for k in ("spkcache_preds", "fifo_preds"):
-        x, y = getattr(a, k), getattr(b, k)
-        assert (x is None) == (y is None), k
-        if x is not None:
-            assert np.array_equal(bits(x), bits(y)), k
-
-
-class Harness:
-    def __init__(self, O, cfg, seed, max_core=0):
-        self.O, self.cfg = O, cfg
-        self.h = SortformerStreams(cfg, max_core)
-        self.rng = np.random.default_rng(seed)
-        self.ref, self.mode = {}, {}
-
-    def open(self, mode):
-        sid = self.h.open()
-        assert sid not in self.ref
-        self.ref[sid], self.mode[sid] = self.O.Session(vars(self.h.config)), mode
-        return sid
-
-    def close(self, sid):
-        self.h.close(sid)
-        del self.ref[sid], self.mode[sid]
-
-    def contexts(self, sid, streaming_rule):
-        c, ref = self.h.config, self.ref[sid]
-        lc = c.chunk_left_context if ref.chunks > 0 else 0
-        core, rc = c.chunk_len, c.chunk_right_context
-        if self.mode[sid] == "offline" and not streaming_rule and self.rng.random() < 0.3:   # a short (last) chunk
-            core, rc = int(self.rng.integers(1, c.chunk_len + 1)), int(self.rng.integers(0, c.chunk_right_context + 1))
-        return core, lc, rc
-
-    def push(self, ids, device, streaming_rule):
-        batch, outs = [], []
-        for sid in ids:
-            core, lc, rc = self.contexts(sid, streaming_rule)
-            n = self.ref[sid].lengths()
-            gen = "turns" if self.mode[sid] == "offline" else self.mode[sid]
-            emb, preds = synth.sortformer_chunk(self.rng, gen, n.spkcache_length, n.fifo_length, core, lc, rc)
-            batch.append((emb, preds, lc, rc))
-        er = max(b[0].shape[0] for b in batch)
-        pr = max(b[1].shape[0] for b in batch)
-        E = np.full((len(ids), er, D), np.nan, np.float32)   # rows past a session's own are never read
-        P = np.full((len(ids), pr, S), np.nan, np.float32)
-        for i, (emb, preds, _, _) in enumerate(batch):
-            E[i, :emb.shape[0]], P[i, :preds.shape[0]] = emb, preds
-        el = np.array([b[0].shape[0] for b in batch], np.int32)
-        lcs = None if streaming_rule else np.array([b[2] for b in batch], np.int32)
-        rcs = None if streaming_rule else np.array([b[3] for b in batch], np.int32)
-        for sid, (emb, preds, lc, rc) in zip(ids, batch):
-            st, conf, tent = self.ref[sid].update(emb, preds, lc, rc)
-            assert st == 0
-            outs.append((conf, tent))
-        if device:
-            bufs = [_lib.DeviceBuffer(a.nbytes) for a in (E, P)]
-            for b, a in zip(bufs, (E, P)):
-                b.upload(a)
-            dc, dt = _lib.DeviceBuffer(4 * len(ids) * er * S), _lib.DeviceBuffer(4 * len(ids) * er * S)
-            cr, tr = self.h.update_device(ids, bufs[0], er, bufs[1], pr, dc, dt, el, lcs, rcs)
-            _lib.synchronize()
-            call = dc.download(len(ids) * er * S, np.float32)
-            tall = dt.download(len(ids) * er * S, np.float32)
-            conf = SortformerStreams._split(call, cr)
-            tent = SortformerStreams._split(tall, tr)
-            for b in bufs + [dc, dt]:
-                b.free()
-        else:
-            conf, tent = self.h.update(ids, E, P, el, lcs, rcs)
-        for (rc_, rt), c, t in zip(outs, conf, tent):
-            assert np.array_equal(bits(c), bits(rc_)) and np.array_equal(bits(t), bits(rt))
-        self.check_inputs(ids, device)
-        for sid in ids:
-            same_state(self.h.state(sid), self.ref[sid].state())
-
-    def check_inputs(self, ids, device):
-        c = self.h.config
-        if device:
-            dsc, dff = _lib.DeviceBuffer(4 * len(ids) * c.spkcache_len * D), _lib.DeviceBuffer(4 * len(ids) * max(c.fifo_len, 1) * D)
-            sl, fl = self.h.model_inputs_device(ids, dsc, dff)
-            _lib.synchronize()
-            sc = dsc.download((len(ids), c.spkcache_len, D), np.float32)
-            ff = dff.download((len(ids), c.fifo_len, D), np.float32)
-            dsc.free()
-            dff.free()
-        else:
-            sc, ff, sl, fl = self.h.model_inputs(ids)
-        for i, sid in enumerate(ids):
-            rsc, rff, rsl, rfl = self.ref[sid].model_inputs()
-            assert (sl[i], fl[i]) == (rsl, rfl)
-            assert np.array_equal(bits(sc[i]), bits(rsc)) and np.array_equal(bits(ff[i]), bits(rff))
 
 
 @pytest.mark.gpu

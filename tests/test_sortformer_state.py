@@ -5,7 +5,8 @@
 * the configuration: the eight presets and the init's clamps;
 * ``sortformer_core.cuh`` — the arithmetic the kernel runs — compiled for the host (``tests/emul/sortformer_emul.cpp``)
   against the oracle, bit for bit, compression by compression, over seeded streams of every preset;
-* the host length mirror against the oracle's lengths at every step.
+* the host length mirror against the oracle's lengths at every step;
+* the host build against the oracle over the edge configurations and adversarial predictions of ``sortformer_cases``.
 """
 import ctypes as C
 import os
@@ -15,6 +16,7 @@ import zlib
 import numpy as np
 import pytest
 
+import sortformer_cases as cases
 from fluidaudio_b200 import _lib, synth
 from fluidaudio_b200.sortformer import PRESETS, SortformerConfig, step_lengths
 
@@ -216,3 +218,35 @@ def test_emulation_and_mirror_match_the_oracle(O, lib, emul, name, mode):
         assert count[0] > 0
     if mode == "never_silent":
         assert count[0] == 0 and not mean.any()
+
+
+@pytest.mark.parametrize("edge", cases.EDGE_CONFIGS, ids=cases.EDGE_IDS)
+def test_emulation_matches_the_oracle_on_edge_configs(O, lib, emul, edge):
+    """the host build against the oracle over the edge configurations, every generator including the adversarial
+    ones, compression by compression"""
+    cfg, resolved, max_core = cases.edge_config(edge)
+    K = resolved.spkcache_len
+    for mode in edge.modes:
+        rng = np.random.default_rng(zlib.crc32(f"{edge.name}/{mode}".encode()))
+        s = O.Session(vars(cfg))
+        mean, count = np.zeros(512, np.float32), np.zeros(1, np.int64)
+        compressions = 0
+        while compressions < 3:
+            assert s.chunks < 2000
+            n = s.lengths()
+            core, lc, rc = cases.contexts(rng, resolved, max_core, s.chunks, edge.offline)
+            emb, preds = cases.chunk(rng, mode, resolved, n.spkcache_length, n.fifo_length, core, lc, rc)
+            assert s.update(emb, preds, lc, rc)[0] == 0
+            pop_e, pop_p = s.last_pop()
+            emul.sortformer_emul_silence(pop_e.ctypes.data, pop_p.ctypes.data, pop_p.shape[0],
+                                         resolved.silence_threshold, mean.ctypes.data, count.ctypes.data)
+            assert np.array_equal(bits(mean), bits(s.state().mean_silence)) and count[0] == s.lengths().silence_frames
+            comp = s.last_compression()
+            if comp is None:
+                continue
+            compressions += 1
+            (sc, dis, strong, weak), slot = run_emulated(emul, cfg, K, comp)
+            for got, ref in ((sc, comp.scores), (dis, comp.disabled), (strong, comp.strong), (weak, comp.weak)):
+                assert np.array_equal(bits(got), bits(ref))
+            assert np.array_equal(slot < 0, comp.is_disabled.astype(bool))
+            assert np.array_equal(slot[slot >= 0], comp.indices[slot >= 0])
