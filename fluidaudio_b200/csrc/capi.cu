@@ -5,6 +5,7 @@
 
 #include "ahc_plan.h"
 #include "assign_host.h"
+#include "call_context.h"
 #include "cluster_plan.h"
 #include "mel_plan.h"
 #include "kmeans_plan.h"
@@ -607,7 +608,9 @@ FA_API fa_status fa_mel_normalize_per_feature(float *x, int64_t frames, int32_t 
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)mel::normalize_per_feature_host(x, (long long)frames, n_mels, (long long)valid);
+    return (fa_status)with_context(0, [&](CallContext &C) {
+        return mel::normalize_per_feature_host(C, x, (long long)frames, n_mels, (long long)valid);
+    });
     FA_GUARD_END
 }
 
@@ -650,22 +653,25 @@ FA_API fa_status fa_audio_resample(const void *pcm, int64_t frames, const fa_aud
         if (st != FA_OK) return (fa_status)st;
     }
     const size_t bytes = (size_t)frames * f.channels * (f.format == resample::kPcmI16 ? 2 : 4);
-    Stream s;
-    DeviceBuffer<> d_pcm;
-    DeviceBuffer<float> d_tab, d_out;
-    int st = s.create();
-    if (st == FA_OK) st = d_pcm.grow(bytes + 16);
-    if (st == FA_OK) st = d_out.grow((size_t)n * sizeof(float));
-    if (st == FA_OK) st = d_tab.grow(d.table.size() * sizeof(float));
-    if (st != FA_OK) return (fa_status)st;
-    if (!d.table.empty())
-        FA_CUDA_TRY(cudaMemcpyAsync(d_tab.data(), d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_pcm.data(), pcm, bytes, cudaMemcpyHostToDevice, s));
-    st = resample::launch_convert(d_pcm.data(), frames, f, d, d_tab.data(), d_out.data(), 0, n, s);
-    if (st != FA_OK) return (fa_status)st;
-    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out.data(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
-    return FA_STATUS_OK;
+    return (fa_status)with_context(0, [&](CallContext &C) -> int {
+        char *d_pcm = nullptr;
+        float *d_tab = nullptr, *d_out = nullptr;
+        int st = carve_arena(C.d_buf, [&](Carver &c) {
+            d_pcm = c.take<char>(bytes + 16);
+            d_tab = c.take<float>(d.table.size());
+            d_out = c.take<float>((size_t)n);
+        });
+        if (st != FA_OK) return st;
+        if (!d.table.empty())
+            FA_CUDA_TRY(cudaMemcpyAsync(d_tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice,
+                                        C.stream));
+        FA_CUDA_TRY(cudaMemcpyAsync(d_pcm, pcm, bytes, cudaMemcpyHostToDevice, C.stream));
+        st = resample::launch_convert(d_pcm, frames, f, d, d_tab, d_out, 0, n, C.stream);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, C.stream));
+        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        return FA_OK;
+    });
     FA_GUARD_END
 }
 
@@ -733,7 +739,7 @@ FA_API fastcluster_wrapper_status fastcluster_compute_centroid_linkage(const dou
     if (pointCount == 1) return FASTCLUSTER_WRAPPER_SUCCESS;
     try {
         if (require_device() != FA_OK) return FASTCLUSTER_WRAPPER_RUNTIME_ERROR;
-        return to_fc(with_context(0, [&](ClusterContext &C) {
+        return to_fc(with_context(0, [&](CallContext &C) {
             return C.solver.linkage_host(data, pointCount, dimension, dendrogramOut, dendrogramLength);
         }));
     } catch (const std::bad_alloc &) {
@@ -756,7 +762,7 @@ FA_API fa_status fa_l2_normalize_rows(const double *x, size_t rows, size_t dim, 
     if (rows == 0 || dim == 0) return FA_STATUS_OK;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) { return l2_normalize_rows(C, x, rows, dim, out); });
+    return (fa_status)with_context(0, [&](CallContext &C) { return l2_normalize_rows(C, x, rows, dim, out); });
     FA_GUARD_END
 }
 
@@ -783,7 +789,7 @@ FA_API fa_status fa_ahc_cluster(const double *features, size_t count, size_t dim
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) {
+    return (fa_status)with_context(0, [&](CallContext &C) {
         return ahc_cluster(C, features, count, dim, threshold, labels);
     });
     FA_GUARD_END
@@ -888,7 +894,7 @@ FA_API fa_status fa_kmeans_cluster(const double *emb, size_t N, size_t D, int32_
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) {
+    return (fa_status)with_context(0, [&](CallContext &C) {
         return kmeans_cluster(C, emb, N, D, num_clusters, max_iterations, n_init, base_seed, labels, centroids, centroid_rows,
                               best_init);
     });
@@ -901,7 +907,7 @@ FA_API fa_status fa_vbx_refine(const double *rho, size_t T, size_t D, const doub
     if (!rho || !cfg || !gamma || !pi || !elbos || !hard || T == 0 || D == 0 || S <= 0) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) {
+    return (fa_status)with_context(0, [&](CallContext &C) {
         return vbx_refine(C, rho, T, D, psi, psi_len, initial, S, *cfg, gamma, pi, elbos, hard, iterations);
     });
     FA_GUARD_END
@@ -913,7 +919,7 @@ FA_API fa_status fa_compute_centroids(const double *emb, size_t T, size_t dim, c
         return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) {
+    return (fa_status)with_context(0, [&](CallContext &C) {
         return compute_centroids(C, emb, T, dim, gamma, pi, S, centroids, centroid_count);
     });
     FA_GUARD_END
@@ -929,7 +935,7 @@ FA_API fa_status fa_assign_embeddings(const double *emb, size_t N, size_t dim, c
     }
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) {
+    return (fa_status)with_context(0, [&](CallContext &C) {
         return assign_embeddings(C, emb, N, dim, centroids, K, labels, scores);
     });
     FA_GUARD_END
@@ -946,7 +952,7 @@ static fa_status diarize_cluster(const float *emb256, const double *rho, size_t 
     if (N > 0x7fffffffull / 4) return FA_STATUS_INDEX_OVERFLOW;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)with_context(0, [&](ClusterContext &C) {
+    return (fa_status)with_context(0, [&](CallContext &C) {
         return cluster_pipeline(C, emb256, rho, N, emb_dim, rho_dim, psi, *cfg, labels, initial, centroids, max_centroids,
                                 info, chunk_index);
     });
@@ -1121,7 +1127,9 @@ static fa_status seg_windows(bool on_device, const float *audio, int64_t total_s
         desc[i] = prepare::WindowDesc{offset, std::max(0LL, std::min(window, (long long)total_samples - offset))};
         if (chunk_offsets) chunk_offsets[i] = (double)offset / (double)c.sample_rate;
     }
-    return (fa_status)prepare::gather_windows(on_device, audio, total_samples, desc.data(), chunk_count, window, out);
+    return (fa_status)with_context(0, [&](CallContext &C) {
+        return prepare::gather_windows(C, on_device, audio, total_samples, desc.data(), chunk_count, window, out);
+    });
     FA_GUARD_END
 }
 FA_API fa_status fa_seg_windows(const float *audio, int64_t total_samples, const fa_seg_config *cfg, int32_t first_chunk,
@@ -1153,7 +1161,9 @@ static fa_status embed_windows(bool on_device, const float *audio, int64_t total
         desc[i] = prepare::embed_window(prepare::resolve_chunk_offset(chunk_offsets, offsets_count, chunk, c),
                                         total_samples, c, audio_sample_count);
     }
-    return (fa_status)prepare::gather_windows(on_device, audio, total_samples, desc.data(), count, audio_sample_count, out);
+    return (fa_status)with_context(0, [&](CallContext &C) {
+        return prepare::gather_windows(C, on_device, audio, total_samples, desc.data(), count, audio_sample_count, out);
+    });
     FA_GUARD_END
 }
 FA_API fa_status fa_embed_windows(const float *audio, int64_t total_samples, const double *chunk_offsets,
@@ -1183,8 +1193,10 @@ static fa_status seg_decode(bool on_device, const float *logits, int32_t chunks,
     if (!logits || !speaker_weights) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)prepare::seg_decode(on_device, logits, chunks, frames, classes, c.speech_onset_threshold, log_probs,
-                                          speaker_weights, histogram, speech_frames);
+    return (fa_status)with_context(0, [&](CallContext &C) {
+        return prepare::seg_decode(C, on_device, logits, chunks, frames, classes, c.speech_onset_threshold, log_probs,
+                                   speaker_weights, histogram, speech_frames);
+    });
     FA_GUARD_END
 }
 FA_API fa_status fa_seg_decode(const float *logits, int32_t chunks, int32_t frames, int32_t classes,
@@ -1227,8 +1239,10 @@ static fa_status embedding_plan(bool on_device, const float *weights, int32_t ch
     p.weight_frames = plan_cfg->weight_frames;
     p.audio_sample_count = plan_cfg->audio_sample_count;
     p.fbank_batch = plan_cfg->fbank_batch;
-    return (fa_status)prepare::embedding_plan(on_device, weights, chunks, frames, speakers, chunk_offsets, offsets_count,
-                                              frame_duration, total_samples, c, p, out, entry_count, counters);
+    return (fa_status)with_context(0, [&](CallContext &C) {
+        return prepare::embedding_plan(C, on_device, weights, chunks, frames, speakers, chunk_offsets, offsets_count,
+                                       frame_duration, total_samples, c, p, out, entry_count, counters);
+    });
     FA_GUARD_END
 }
 FA_API fa_status fa_embedding_plan(const float *speaker_weights, int32_t chunks, int32_t frames, int32_t speakers,
@@ -1263,7 +1277,9 @@ FA_API fa_status fa_weight_resample(const float *rows, int64_t row_count, int32_
     if (!rows || !out) return FA_STATUS_INVALID_ARGUMENT;
     API_REQUIRE_DEVICE();
     FA_GUARD_BEGIN
-    return (fa_status)prepare::weight_resample(rows, row_count, in_len, out_len, out);
+    return (fa_status)with_context(0, [&](CallContext &C) {
+        return prepare::weight_resample(C, rows, row_count, in_len, out_len, out);
+    });
     FA_GUARD_END
 }
 

@@ -1,4 +1,4 @@
-// Clustering host code: the context pool, the diarization pipeline (OfflineDiarizerManager.cluster(_:) :286-375) in its
+// Clustering host code: the diarization pipeline (OfflineDiarizerManager.cluster(_:) :286-375) in its
 // steps, the batch lanes and the standalone stages.  The kernels are in ahc_kernels.cu, vbx_kernels.cu and kmeans_kernels.cu.
 #include "cluster_plan.h"
 #include "assign_host.h"
@@ -9,67 +9,11 @@
 #include <atomic>
 #include <chrono>
 #include <cstring>
-#include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
 
 namespace fa {
-
-int ClusterContext::init(int worker_lim) {
-    FA_CUDA_TRY(cudaGetDevice(&device));
-    int st = stream.create();
-    for (auto &e : ev)
-        if (st == FA_OK) st = e.create();
-    if (st == FA_OK) st = vbx::set_smem_limits();
-    if (st == FA_OK) st = solver.init(stream, worker_lim);
-    if (st != FA_OK) return st;
-    worker_limit = worker_lim;
-    ready = true;
-    return FA_OK;
-}
-
-static std::mutex g_pool_mutex;
-static std::vector<std::unique_ptr<ClusterContext>> g_pool;   // idle contexts
-
-struct Lease {
-    std::unique_ptr<ClusterContext> ctx;
-    int status = FA_OK;
-    explicit Lease(int worker_limit) {
-        int dev = 0;
-        const cudaError_t e = cudaGetDevice(&dev);
-        if (e != cudaSuccess) {
-            status = cuda_failure(e, "cudaGetDevice", __FILE__, __LINE__);
-            return;
-        }
-        {
-            std::lock_guard<std::mutex> lock(g_pool_mutex);
-            for (size_t i = 0; i < g_pool.size(); ++i)
-                if (g_pool[i]->device == dev && g_pool[i]->worker_limit == worker_limit) {
-                    ctx = std::move(g_pool[i]);
-                    g_pool.erase(g_pool.begin() + i);
-                    break;
-                }
-        }
-        if (!ctx) {
-            ctx.reset(new ClusterContext());
-            status = ctx->init(worker_limit);
-        }
-    }
-    ~Lease() {
-        if (ctx && ctx->ready && status != FA_CUDA_ERROR) {
-            std::lock_guard<std::mutex> lock(g_pool_mutex);
-            g_pool.push_back(std::move(ctx));
-        }
-    }
-};
-
-int with_context(int worker_limit, const std::function<int(ClusterContext &)> &body) {
-    Lease lease(worker_limit);
-    if (lease.status != FA_OK) return lease.status;
-    lease.status = body(*lease.ctx);
-    return lease.status;
-}
 
 static vbx::Config to_vbx(const fa_vbx_config &c) {
     vbx::Config vc;
@@ -90,7 +34,7 @@ static float ms_between(cudaEvent_t a, cudaEvent_t b) {
 // One pipeline call: its arguments, in the order cluster_pipeline initialises them, then the state its steps share.  The
 // steps run in order on the context's stream, and the first failure ends the call.
 struct Pipeline {
-    ClusterContext &C;
+    CallContext &C;
     const float *emb;
     const double *rho;
     size_t N, E, R;
@@ -353,7 +297,7 @@ struct Pipeline {
     }
 };
 
-int cluster_pipeline(ClusterContext &C, const float *emb, const double *rho, size_t N, size_t E, size_t R,
+int cluster_pipeline(CallContext &C, const float *emb, const double *rho, size_t N, size_t E, size_t R,
                      const double *psi, const fa_cluster_config &cfg, int32_t *labels, int32_t *initial_out,
                      double *centroids_out, int32_t max_centroids, fa_cluster_info *info, const int32_t *chunk_index) {
     return Pipeline{C, emb, rho, N, E, R, psi, cfg, labels, initial_out, centroids_out, max_centroids, info, chunk_index}
@@ -385,7 +329,7 @@ int cluster_batch(const float *emb, const double *rho, const int64_t *set_offset
             if (e != cudaSuccess) {
                 status[lane] = cuda_failure(e, "cudaSetDevice", __FILE__, __LINE__);
             } else {
-                status[lane] = with_context(worker_limit, [&](ClusterContext &C) {
+                status[lane] = with_context(worker_limit, [&](CallContext &C) {
                     for (;;) {
                         const int m = next.fetch_add(1);
                         if (m >= set_count) return (int)FA_OK;
@@ -429,7 +373,7 @@ int cluster_batch(const float *emb, const double *rho, const int64_t *set_offset
     return FA_OK;
 }
 
-int l2_normalize_rows(ClusterContext &C, const double *x, size_t rows, size_t dim, double *out) {
+int l2_normalize_rows(CallContext &C, const double *x, size_t rows, size_t dim, double *out) {
     double *d_in, *d_out;
     int st = carve_arena(C.d_buf, [&](Carver &c) {
         d_in = c.take<double>(rows * dim);
@@ -445,7 +389,7 @@ int l2_normalize_rows(ClusterContext &C, const double *x, size_t rows, size_t di
 }
 
 // AHCClustering.cluster (AHCClustering.swift:20-67) for count >= 2 and dim >= 1
-int ahc_cluster(ClusterContext &C, const double *features, size_t count, size_t dim, double threshold, int32_t *labels) {
+int ahc_cluster(CallContext &C, const double *features, size_t count, size_t dim, double threshold, int32_t *labels) {
     double *d_in, *d_norm, *h_Z;
     int st = carve_arena(C.d_buf, [&](Carver &c) {
         d_in = c.take<double>(count * dim);
@@ -468,7 +412,7 @@ int ahc_cluster(ClusterContext &C, const double *features, size_t count, size_t 
 }
 
 // KMeansClustering.clusterWithCentroidsNInit for N >= 1, D >= 1 and num_clusters >= 1: min(num_clusters, N) centroid rows
-int kmeans_cluster(ClusterContext &C, const double *emb, size_t N, size_t D, int32_t num_clusters, int32_t max_iterations,
+int kmeans_cluster(CallContext &C, const double *emb, size_t N, size_t D, int32_t num_clusters, int32_t max_iterations,
                    int32_t n_init, uint64_t base_seed, int32_t *labels, double *centroids, int32_t *centroid_rows,
                    int32_t *best_init) {
     const size_t rows_needed = std::min<size_t>((size_t)num_clusters, N);
@@ -493,7 +437,7 @@ int kmeans_cluster(ClusterContext &C, const double *emb, size_t N, size_t D, int
     return FA_OK;
 }
 
-int vbx_refine(ClusterContext &C, const double *rho, size_t T, size_t D, const double *psi, size_t psi_len,
+int vbx_refine(CallContext &C, const double *rho, size_t T, size_t D, const double *psi, size_t psi_len,
                const int32_t *initial, int32_t S, const fa_vbx_config &cfg, double *gamma, double *pi, double *elbos,
                int32_t *hard, int32_t *iterations) {
     const int cap = std::max(cfg.max_iterations, 1);
@@ -525,7 +469,7 @@ int vbx_refine(ClusterContext &C, const double *rho, size_t T, size_t D, const d
     return FA_OK;
 }
 
-int compute_centroids(ClusterContext &C, const double *emb, size_t T, size_t dim, const double *gamma, const double *pi,
+int compute_centroids(CallContext &C, const double *emb, size_t T, size_t dim, const double *gamma, const double *pi,
                       int32_t S, double *centroids, int32_t *centroid_count) {
     double *d_emb, *d_gamma, *d_pi, *d_cent, *d_cent_n;
     int *d_count;
@@ -555,7 +499,7 @@ int compute_centroids(ClusterContext &C, const double *emb, size_t T, size_t dim
 }
 
 // OfflineDiarizerManager.assignEmbeddings (:789-883) for N >= 1 and K >= 1
-int assign_embeddings(ClusterContext &C, const double *emb, size_t N, size_t dim, const double *centroids, int32_t K,
+int assign_embeddings(CallContext &C, const double *emb, size_t N, size_t dim, const double *centroids, int32_t K,
                       int32_t *labels, double *scores) {
     double *d_emb, *d_craw, *d_cn, *d_scores;
     int *d_labels;

@@ -12,6 +12,7 @@
 // one thread per mel bin walks the frames in order with individually rounded float32 operations, so the result is the
 // reference's arithmetic exactly; loads are coalesced across bins.  Sizes are tiny (<= 512 bins x a few thousand
 // frames), the point is fusion with the producer, not throughput.
+#include "call_context.h"
 #include "fa_common.cuh"
 #include "mel_plan.h"
 
@@ -76,16 +77,17 @@ __global__ void per_feature_norm_inplace_kernel(float *x, long long T, int M, lo
     for (long long t = 0; t < T; ++t) x[t * M + m] = t < valid ? __fdiv_rn(__fsub_rn(x[t * M + m], mean), sd) : 0.0f;
 }
 
-// host buffer in, host buffer out (x: [T x M] time-major, normalised in place); valid >= 1
-int normalize_per_feature_host(float *x, long long T, int M, long long valid) {
-    DeviceBuffer<float> d;
-    const size_t bytes = sizeof(float) * (size_t)T * M;
-    const int st = d.grow(bytes);
+// host buffer in, host buffer out (x: [T x M] time-major, normalised in place), staged in the context's d_buf; valid >= 1
+int normalize_per_feature_host(CallContext &C, float *x, long long T, int M, long long valid) {
+    float *d = nullptr;
+    const size_t count = (size_t)T * M;
+    const int st = carve_arena(C.d_buf, [&](Carver &c) { d = c.take<float>(count); });
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpy(d.data(), x, bytes, cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(fa::launch(per_feature_norm_inplace_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, 0, d.data(),
+    FA_CUDA_TRY(cudaMemcpyAsync(d, x, count * sizeof(float), cudaMemcpyHostToDevice, C.stream));
+    FA_CUDA_TRY(fa::launch(per_feature_norm_inplace_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, C.stream, d,
                            T, M, valid));
-    FA_CUDA_TRY(cudaMemcpy(x, d.data(), bytes, cudaMemcpyDeviceToHost));
+    FA_CUDA_TRY(cudaMemcpyAsync(x, d, count * sizeof(float), cudaMemcpyDeviceToHost, C.stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     return FA_OK;
 }
 

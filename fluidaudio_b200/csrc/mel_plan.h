@@ -12,6 +12,8 @@
 #include <vector>
 
 namespace fa {
+struct CallContext;   // call_context.h
+
 namespace mel {
 
 struct cpx;
@@ -182,7 +184,7 @@ struct MelStreamSet {
 };
 
 // mel_adapters.cu: device epilogues for the callers directly behind AudioMelSpectrogram (host buffers in and out)
-int normalize_per_feature_host(float *x, long long T, int M, long long valid);   // mel_adapters.cu
+int normalize_per_feature_host(CallContext &C, float *x, long long T, int M, long long valid);
 int unified_features(MelPlan &p, const float *window, long long n, long long valid_count, float *out, long long out_len,
                      long long *total_frames, int *valid_frames);
 int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean, long long *cmn_count, float *out,

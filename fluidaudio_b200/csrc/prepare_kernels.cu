@@ -13,6 +13,7 @@
 // fa_seg_decode is one launch; fa_embedding_plan is two, three with the skip strategy, whatever the chunk count.
 #include "prepare_plan.h"
 
+#include "call_context.h"
 #include "prepare_core.cuh"
 
 #include <algorithm>
@@ -347,29 +348,6 @@ __global__ void __launch_bounds__(kThreads) weight_resample_kernel(const float *
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-// The calling thread's stream, descriptor stage and scratch, made on first use and remade when the thread moves to
-// another device.
-struct Context {
-    int device = -1;
-    Stream stream;
-    UploadStage<> stage;
-    DeviceBuffer<> scratch;
-};
-
-int context(Context *&out) {
-    static thread_local Context ctx;
-    int dev = 0;
-    FA_CUDA_TRY(cudaGetDevice(&dev));
-    if (ctx.device != dev) {
-        ctx = Context();
-        const int st = ctx.stream.create();
-        if (st != FA_OK) return st;
-        ctx.device = dev;
-    }
-    out = &ctx;
-    return FA_OK;
-}
-
 template <typename Kernel> int allow_smem(Kernel kernel, size_t bytes, const char *what) {
     if (bytes > kMaxDynamicSmem) {
         set_error("%s: %zu bytes of shared memory per chunk exceed %zu", what, bytes, kMaxDynamicSmem);
@@ -380,14 +358,13 @@ template <typename Kernel> int allow_smem(Kernel kernel, size_t bytes, const cha
     return FA_OK;
 }
 
-// A device copy of a host array for the host-buffer calls (null and empty arrays stay null).
-template <typename T> int to_device(DeviceBuffer<> &buf, const T *host, size_t count, cudaStream_t s, const T *&dev) {
+// A device copy of a host array for the host-buffer calls, in its staging carved from the context's d_buf (null and
+// empty arrays stay null).
+template <typename T> int to_device(T *staging, const T *host, size_t count, cudaStream_t s, const T *&dev) {
     dev = nullptr;
     if (!host || !count) return FA_OK;
-    const int st = buf.grow(count * sizeof(T));
-    if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(buf.data(), host, count * sizeof(T), cudaMemcpyHostToDevice, s));
-    dev = static_cast<const T *>(buf.data());
+    FA_CUDA_TRY(cudaMemcpyAsync(staging, host, count * sizeof(T), cudaMemcpyHostToDevice, s));
+    dev = staging;
     return FA_OK;
 }
 
@@ -419,53 +396,54 @@ WindowDesc embed_window(double chunk_offset, long long total_samples, const SegC
     return WindowDesc{start, start < end ? std::min<long long>(end - start, audio_sample_count) : 0};
 }
 
-int gather_windows(bool on_device, const float *audio, long long total_samples, const WindowDesc *desc, int count,
-                   long long row_len, float *out) {
-    Context *ctx = nullptr;
-    int st = context(ctx);
-    if (st != FA_OK) return st;
-    const cudaStream_t s = ctx->stream;
+int gather_windows(CallContext &C, bool on_device, const float *audio, long long total_samples, const WindowDesc *desc,
+                   int count, long long row_len, float *out) {
+    const cudaStream_t s = C.stream;
     const size_t desc_bytes = (size_t)count * sizeof(WindowDesc), out_floats = (size_t)count * (size_t)row_len;
-    if ((st = ctx->stage.reserve(desc_bytes)) != FA_OK) return st;
-    std::copy(desc, desc + count, static_cast<WindowDesc *>(ctx->stage.host.data()));
-    if ((st = ctx->stage.upload(desc_bytes, s)) != FA_OK) return st;
-    DeviceBuffer<> in_buf, out_buf;
+    int st = C.stage.reserve(desc_bytes);
+    if (st != FA_OK) return st;
+    std::copy(desc, desc + count, static_cast<WindowDesc *>(C.stage.host.data()));
+    if ((st = C.stage.upload(desc_bytes, s)) != FA_OK) return st;
     const float *d_audio = audio;
     float *d_out = out;
     if (!on_device) {
-        if ((st = to_device(in_buf, audio, (size_t)total_samples, s, d_audio)) != FA_OK) return st;
-        if ((st = out_buf.grow(out_floats * sizeof(float))) != FA_OK) return st;
-        d_out = static_cast<float *>(out_buf.data());
+        float *audio_stage = nullptr;
+        st = carve_arena(C.d_buf, [&](Carver &c) {
+            audio_stage = c.take<float>((size_t)total_samples);
+            d_out = c.take<float>(out_floats);
+        });
+        if (st != FA_OK) return st;
+        if ((st = to_device(audio_stage, audio, (size_t)total_samples, s, d_audio)) != FA_OK) return st;
     }
     const unsigned tiles = (unsigned)std::min<long long>(16, (row_len + 4 * kThreads - 1) / (4 * kThreads));
     FA_CUDA_TRY(launch(seg_windows_kernel, dim3((unsigned)count, std::max(1u, tiles)), dim3(kThreads), 0, s, d_audio,
-                       static_cast<const WindowDesc *>(ctx->stage.device.data()), row_len, d_out));
+                       static_cast<const WindowDesc *>(C.stage.device.data()), row_len, d_out));
     if (!on_device) FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, out_floats * sizeof(float), cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     return FA_OK;
 }
 
-int seg_decode(bool on_device, const float *logits, int chunks, int frames, int classes, float onset, float *log_probs,
-               float *speaker_weights, int64_t histogram[8], int64_t *speech_frames) {
-    Context *ctx = nullptr;
-    int st = context(ctx);
-    if (st != FA_OK) return st;
-    const cudaStream_t s = ctx->stream;
+int seg_decode(CallContext &C, bool on_device, const float *logits, int chunks, int frames, int classes, float onset,
+               float *log_probs, float *speaker_weights, int64_t histogram[8], int64_t *speech_frames) {
+    const cudaStream_t s = C.stream;
     const long long total = (long long)chunks * frames;
     const size_t in_floats = (size_t)total * classes, w_floats = (size_t)total * kDecodeSpeakers;
     constexpr size_t kTallyBytes = (kPowersetClasses + 1) * sizeof(unsigned long long);
-    if ((st = ctx->scratch.grow(kTallyBytes)) != FA_OK) return st;
-    auto *tallies = static_cast<unsigned long long *>(ctx->scratch.data());
+    int st = C.scratch.grow(kTallyBytes);
+    if (st != FA_OK) return st;
+    auto *tallies = static_cast<unsigned long long *>(C.scratch.data());
     FA_CUDA_TRY(cudaMemsetAsync(tallies, 0, kTallyBytes, s));
-    DeviceBuffer<> in_buf, lp_buf, w_buf;
     const float *d_logits = logits;
     float *d_lp = log_probs, *d_w = speaker_weights;
     if (!on_device) {
-        if ((st = to_device(in_buf, logits, in_floats, s, d_logits)) != FA_OK) return st;
-        if (log_probs && (st = lp_buf.grow(in_floats * sizeof(float))) != FA_OK) return st;
-        if ((st = w_buf.grow(w_floats * sizeof(float))) != FA_OK) return st;
-        d_lp = log_probs ? static_cast<float *>(lp_buf.data()) : nullptr;
-        d_w = static_cast<float *>(w_buf.data());
+        float *logits_stage = nullptr;
+        st = carve_arena(C.d_buf, [&](Carver &c) {
+            logits_stage = c.take<float>(in_floats);
+            if (log_probs) d_lp = c.take<float>(in_floats);
+            d_w = c.take<float>(w_floats);
+        });
+        if (st != FA_OK) return st;
+        if ((st = to_device(logits_stage, logits, in_floats, s, d_logits)) != FA_OK) return st;
     }
     const size_t smem = sizeof(float) * kThreads * ((size_t)(classes | 1) + kDecodeSpeakers);
     FA_CUDA_TRY(launch(seg_decode_kernel, dim3((unsigned)((total + kThreads - 1) / kThreads)), dim3(kThreads), smem, s,
@@ -482,14 +460,11 @@ int seg_decode(bool on_device, const float *logits, int chunks, int frames, int 
     return FA_OK;
 }
 
-int embedding_plan(bool on_device, const float *speaker_weights, int chunks, int frames, int speakers,
+int embedding_plan(CallContext &C, bool on_device, const float *speaker_weights, int chunks, int frames, int speakers,
                    const double *chunk_offsets, int offsets_count, double frame_duration, long long total_samples,
                    const SegConfig &seg, const PlanConfig &plan, const PlanOutputs &out, int32_t *entry_count,
                    int64_t counters[4]) {
-    Context *ctx = nullptr;
-    int st = context(ctx);
-    if (st != FA_OK) return st;
-    const cudaStream_t s = ctx->stream;
+    const cudaStream_t s = C.stream;
     const size_t pairs = (size_t)chunks * speakers, w_floats = pairs * frames;
     const bool reuse = plan.skip_threshold >= 0.0f;
 
@@ -504,9 +479,10 @@ int embedding_plan(bool on_device, const float *speaker_weights, int chunks, int
     // per chunk: its offset and whether it reaches the embedding stage; then the reaching chunks in order (FBANK batches
     // are counted over those)
     const size_t desc_bytes = ((size_t)chunks * sizeof(ChunkDesc) + 255) & ~size_t(255);
-    if ((st = ctx->stage.reserve(desc_bytes + (size_t)chunks * sizeof(int))) != FA_OK) return st;
-    auto *desc = static_cast<ChunkDesc *>(ctx->stage.host.data());
-    int *active = reinterpret_cast<int *>(static_cast<char *>(ctx->stage.host.data()) + desc_bytes);
+    int st = C.stage.reserve(desc_bytes + (size_t)chunks * sizeof(int));
+    if (st != FA_OK) return st;
+    auto *desc = static_cast<ChunkDesc *>(C.stage.host.data());
+    int *active = reinterpret_cast<int *>(static_cast<char *>(C.stage.host.data()) + desc_bytes);
     int active_count = 0;
     for (int c = 0; c < chunks; ++c) {
         desc[c].offset = resolve_chunk_offset(chunk_offsets, offsets_count, c, seg);
@@ -514,15 +490,17 @@ int embedding_plan(bool on_device, const float *speaker_weights, int chunks, int
         desc[c].pad = 0;
         if (desc[c].active) active[active_count++] = c;
     }
-    if ((st = ctx->stage.upload(desc_bytes + (size_t)chunks * sizeof(int), s)) != FA_OK) return st;
-    const auto *d_desc = static_cast<const ChunkDesc *>(ctx->stage.device.data());
-    const int *d_active = reinterpret_cast<const int *>(static_cast<const char *>(ctx->stage.device.data()) + desc_bytes);
+    if ((st = C.stage.upload(desc_bytes + (size_t)chunks * sizeof(int), s)) != FA_OK) return st;
+    const auto *d_desc = static_cast<const ChunkDesc *>(C.stage.device.data());
+    const int *d_active = reinterpret_cast<const int *>(static_cast<const char *>(C.stage.device.data()) + desc_bytes);
 
-    // the host-buffer call packs into device arrays of full capacity and copies the emitted entries back
+    // the host-buffer call stages the weights and packs into device arrays of full capacity, then copies the emitted
+    // entries back
     PlanOutputs d = out;
-    DeviceBuffer<> in_buf, out_buf;
     const float *d_weights = speaker_weights;
+    float *weights_stage = nullptr;
     auto host_layout = [&](Carver &c) {
+        weights_stage = c.take<float>(w_floats);
         if (out.chunk_index) d.chunk_index = c.take<int32_t>(pairs);
         if (out.speaker_index) d.speaker_index = c.take<int32_t>(pairs);
         if (out.start_frame) d.start_frame = c.take<int32_t>(pairs);
@@ -536,14 +514,14 @@ int embedding_plan(bool on_device, const float *speaker_weights, int chunks, int
         if (out.model_weights) d.model_weights = c.take<float>(pairs * plan.weight_frames);
     };
     if (!on_device) {
-        if ((st = to_device(in_buf, speaker_weights, w_floats, s, d_weights)) != FA_OK) return st;
-        if ((st = carve_arena(out_buf, host_layout)) != FA_OK) return st;
+        if ((st = carve_arena(C.d_buf, host_layout)) != FA_OK) return st;
+        if ((st = to_device(weights_stage, speaker_weights, w_floats, s, d_weights)) != FA_OK) return st;
     }
 
     EntryMeta *meta = nullptr;
     int *chunk_count = nullptr, *slot_of = nullptr, *tallies = nullptr;   // tallies: 4 counters, then the entry count
     float *own_masks = nullptr;
-    st = carve_arena(ctx->scratch, [&](Carver &c) {
+    st = carve_arena(C.scratch, [&](Carver &c) {
         meta = c.take<EntryMeta>(pairs);
         chunk_count = c.take<int>(chunks);
         slot_of = c.take<int>(pairs);
@@ -596,20 +574,20 @@ int embedding_plan(bool on_device, const float *speaker_weights, int chunks, int
     return FA_OK;
 }
 
-int weight_resample(const float *rows, long long row_count, int in_len, int out_len, float *out) {
-    Context *ctx = nullptr;
-    int st = context(ctx);
-    if (st != FA_OK) return st;
-    const cudaStream_t s = ctx->stream;
+int weight_resample(CallContext &C, const float *rows, long long row_count, int in_len, int out_len, float *out) {
+    const cudaStream_t s = C.stream;
     const long long total = row_count * out_len;
-    DeviceBuffer<> in_buf, out_buf;
+    float *rows_stage = nullptr, *d_out = nullptr;
+    int st = carve_arena(C.d_buf, [&](Carver &c) {
+        rows_stage = c.take<float>((size_t)(row_count * in_len));
+        d_out = c.take<float>((size_t)total);
+    });
+    if (st != FA_OK) return st;
     const float *d_rows = nullptr;
-    if ((st = to_device(in_buf, rows, (size_t)(row_count * in_len), s, d_rows)) != FA_OK) return st;
-    if ((st = out_buf.grow((size_t)total * sizeof(float))) != FA_OK) return st;
+    if ((st = to_device(rows_stage, rows, (size_t)(row_count * in_len), s, d_rows)) != FA_OK) return st;
     const unsigned grid = (unsigned)std::min<long long>((total + kThreads - 1) / kThreads, 65535);
-    FA_CUDA_TRY(launch(weight_resample_kernel, dim3(grid), dim3(kThreads), 0, s, d_rows, total, in_len, out_len,
-                       static_cast<float *>(out_buf.data())));
-    FA_CUDA_TRY(cudaMemcpyAsync(out, out_buf.data(), (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, s));
+    FA_CUDA_TRY(launch(weight_resample_kernel, dim3(grid), dim3(kThreads), 0, s, d_rows, total, in_len, out_len, d_out));
+    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     return FA_OK;
 }

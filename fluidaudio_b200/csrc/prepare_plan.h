@@ -5,14 +5,17 @@
 // :321-405), Diarizer/Offline/Extraction/OfflineEmbeddingExtractor.swift (chunks and fbank windows :651-707; masks
 // :421-613; the mask-similarity skip strategy :338-351,554-585,632-639), Extraction/WeightInterpolation.swift.
 //
-// Every call runs on the calling thread's own stream and has finished when it returns.  `on_device` says whether the
-// large buffers (audio, windows, logits, log-probabilities, weights, the per-entry outputs) are device pointers; the small
-// ones (chunk offsets, chunk indices, histogram, counts) are always host memory.
+// Every call runs on the stream of the call context it is given and has finished when it returns; the host-buffer calls
+// stage their arrays in the context's workspace.  `on_device` says whether the large buffers (audio, windows, logits,
+// log-probabilities, weights, the per-entry outputs) are device pointers; the small ones (chunk offsets, chunk indices,
+// histogram, counts) are always host memory.
 #pragma once
 
 #include <cstdint>
 
 namespace fa {
+struct CallContext;   // call_context.h
+
 namespace prepare {
 
 constexpr int kMaxClasses = 16;   // logits per frame fa_seg_decode accepts
@@ -56,16 +59,16 @@ long long window_count(long long total_samples, const SegConfig &c);
 double resolve_chunk_offset(const double *offsets, int offsets_count, int c, const SegConfig &cfg);
 WindowDesc embed_window(double chunk_offset, long long total_samples, const SegConfig &cfg, int audio_sample_count);
 
-int gather_windows(bool on_device, const float *audio, long long total_samples, const WindowDesc *desc, int count,
-                   long long row_len, float *out);
-int seg_decode(bool on_device, const float *logits, int chunks, int frames, int classes, float onset, float *log_probs,
-               float *speaker_weights, int64_t histogram[8], int64_t *speech_frames);
+int gather_windows(CallContext &C, bool on_device, const float *audio, long long total_samples, const WindowDesc *desc,
+                   int count, long long row_len, float *out);
+int seg_decode(CallContext &C, bool on_device, const float *logits, int chunks, int frames, int classes, float onset,
+               float *log_probs, float *speaker_weights, int64_t histogram[8], int64_t *speech_frames);
 // counters: evaluatedMaskCount, emptyMaskCount, fallbackMaskCount, skippedEmbeddingCount
-int embedding_plan(bool on_device, const float *speaker_weights, int chunks, int frames, int speakers,
+int embedding_plan(CallContext &C, bool on_device, const float *speaker_weights, int chunks, int frames, int speakers,
                    const double *chunk_offsets, int offsets_count, double frame_duration, long long total_samples,
                    const SegConfig &seg, const PlanConfig &plan, const PlanOutputs &out, int32_t *entry_count,
                    int64_t counters[4]);
-int weight_resample(const float *rows, long long row_count, int in_len, int out_len, float *out);
+int weight_resample(CallContext &C, const float *rows, long long row_count, int in_len, int out_len, float *out);
 
 } // namespace prepare
 } // namespace fa

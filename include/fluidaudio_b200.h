@@ -415,9 +415,9 @@ fa_status fa_build_speaker_database(const int32_t *seg_cluster, int32_t segment_
  * 303,321-405; Extraction/OfflineEmbeddingExtractor.swift:338-351,381-387,421-707,807-842; Extraction/
  * WeightInterpolation.swift:19-146; Utils/VDSPOperations.swift:142-155.
  *
- * Each call runs on a stream of the calling thread and has finished when it returns.  The `_device` twins take device
- * pointers for the large buffers (audio, windows, logits, log-probabilities, weights and every per-entry output) and
- * leave them on the device; work queued on other streams that produces their inputs must have finished before the
+ * Each call runs on a context leased from the library's pool and has finished when it returns.  The `_device` twins
+ * take device pointers for the large buffers (audio, windows, logits, log-probabilities, weights and every per-entry
+ * output) and leave them on the device; work queued on other streams that produces their inputs must have finished before the
  * call.  Small arrays (chunk offsets, chunk indices, the histogram, counts) are host memory in both.
  * Weights, class histogram, entries, frames, times and both weight matrices equal the reference bit for bit for the
  * binary weights fa_seg_decode produces; log-probabilities depend on expf / logf (Apple's vvexpf is closed) and sums of

@@ -48,6 +48,55 @@ def test_cuda_resources_are_made_only_by_the_owning_types():
     assert not offenders, f"CUDA resources made or released outside the owners of fa_common.cuh: {offenders}"
 
 
+OWNER_DECL = re.compile(r"\b(DeviceBuffer|PinnedBuffer|Stream)\s*(<[^;{}()]*?>)?\s*[A-Za-z_]\w*")
+LOCAL_OWNERS_ALLOWED = {("fa_common.cuh", "grow_slots"), ("capi.cu", "fa_memcpy_probe")}
+THREAD_LOCALS_ALLOWED = {("capi.cu", "g_error"), ("capi.cu", "t_ev"), ("ahc_kernels.cu", "g_last_ms")}
+
+
+def _scopes(code):
+    """`code` without preprocessor lines and string / character literals, and for each of its characters the function
+    whose body encloses it (None at namespace and class scope)"""
+    code = re.sub(r"^[ \t]*#(?:[^\n]*\\\n)*[^\n]*", " ", code, flags=re.M)
+    code = re.sub(r'"(?:\\.|[^"\\\n])*"|\'(?:\\.|[^\'\\\n])*\'', '""', code)
+    owner, stack, start = [], [], 0   # stack: per open brace, the function whose body it opens or lies in
+    for i, ch in enumerate(code):
+        if ch == "{":
+            head = code[start:i]
+            if stack and stack[-1]:
+                stack.append(stack[-1])
+            elif re.search(r"\b(namespace|extern|struct|class|union|enum)\b", head):
+                stack.append(None)
+            else:
+                m = re.search(r"(\w+)\s*\(", head)
+                stack.append(m.group(1) if m else "?")
+        elif ch == "}" and stack:
+            stack.pop()
+        if ch in "{};":
+            start = i + 1
+        owner.append(stack[-1] if stack else None)
+    return code, owner
+
+
+def test_handle_less_calls_own_no_stream_or_buffer_of_their_own():
+    """A stream or buffer made inside a function body is made (and, for device memory, freed, which waits for the device)
+    on every call; handle-less calls lease a pooled context (call_context.h) instead, and per-thread state would bypass
+    that pool."""
+    offenders = []
+    for name in sorted(os.listdir(CSRC)):
+        if not name.endswith((".cu", ".cuh", ".h", ".cpp")):
+            continue
+        code, owner = _scopes(_code(os.path.join(CSRC, name)))
+        for m in OWNER_DECL.finditer(code):
+            fn = owner[m.start()]
+            if fn and (name, fn) not in LOCAL_OWNERS_ALLOWED:
+                offenders.append(f"{name}: {fn}: {' '.join(m.group(0).split())}")
+        for m in re.finditer(r"\bthread_local\b([^;=\[{(]*)", code):
+            var = re.findall(r"\w+", m.group(1))[-1]
+            if (name, var) not in THREAD_LOCALS_ALLOWED:
+                offenders.append(f"{name}: {owner[m.start()] or 'namespace scope'}: thread_local {var}")
+    assert not offenders, f"streams or buffers inside function bodies, or thread_local state: {offenders}"
+
+
 def test_the_owning_types_make_every_kind_of_resource():
     code = _code(os.path.join(CSRC, "fa_common.cuh"))
     for call in ("cudaMalloc", "cudaMallocHost", "cudaFree", "cudaFreeHost", "cudaStreamCreateWithFlags",

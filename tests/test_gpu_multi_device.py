@@ -2,8 +2,9 @@
 
 The kernels that take more than 48 KB of dynamic shared memory (the AHC merge kernel, the fused VBx E-step and the
 fused centroid accumulation) must be opted in on every device they run on: a function attribute holds for the device
-that was current when it was set.  Each pooled clustering context sets them on its own device when it is made, so a
-call on device 1 after one on device 0 runs the same kernels and gives the same labels.
+that was current when it was set.  Each pooled call context sets them on its own device when it is made (the pool keeps
+one context per device and concurrent caller), so a call on device 1 after one on device 0 runs the same kernels and
+gives the same labels.
 """
 import numpy as np
 import pytest

@@ -291,13 +291,30 @@ def test_plan_launch_count_does_not_depend_on_the_chunk_count():
 
 # ---- 10. determinism ----------------------------------------------------------------------------------------------------
 def test_results_are_identical_run_to_run_and_across_threads():
+    """Every handle-less call leases a pooled context, so the calls of four threads interleave on contexts whose
+    workspaces an earlier call of another kind has already grown: each result equals the first sequential run's."""
+    from fluidaudio_b200.audio_converter import Algorithm, AudioConverter
+    from fluidaudio_b200.clustering import OfflineClusterer
+    from fluidaudio_b200.mel import normalize_per_feature
+
     rng = np.random.default_rng(6)
     logits, truth = synth.segmentation_logits(120.0, seed=8)
+    chunks, frames, classes = logits.shape
     proc = OfflineSegmentationProcessor()
     planner = OfflineEmbeddingPlanner(config=EmbeddingPlanConfig(skip_threshold=0.95))
     soft = rng.uniform(0, 1, (30, 589, 3)).astype(np.float32)
+    audio = synth.tone_noise_audio(16000 * 30 + 123, seed=9)
+    mono = rng.uniform(-1, 1, 44100).astype(np.float32)
+    planar = rng.uniform(-1, 1, (3, 48000)).astype(np.float32)
+    mel = rng.standard_normal((300, 80)).astype(np.float32)
+    emb, _ = synth.speaker_embeddings(200, 256, 3, seed=10)
+    rho, psi = synth.synthetic_plda(emb)
+    per_entry = dict(chunk_index=(np.int32, 1), speaker_index=(np.int32, 1), start_frame=(np.int32, 1),
+                     end_frame=(np.int32, 1), start_time=(np.float64, 1), end_time=(np.float64, 1),
+                     mask_sum=(np.float32, 1), used_fallback=(np.int32, 1), reuse_of=(np.int32, 1),
+                     frame_weights=(np.float32, frames), model_weights=(np.float32, planner.config.weight_frames))
 
-    def run():
+    def host_decode_and_plan():
         seg = proc.decode(logits, truth["chunk_offsets"])
         plan = planner.plan(seg, truth["total_samples"])
         soft_plan = run_plan(SegmentationConfig(), EmbeddingPlanConfig(skip_threshold=0.9), soft, np.arange(30) * 2.0, 0.0,
@@ -305,14 +322,39 @@ def test_results_are_identical_run_to_run_and_across_threads():
         return [seg.log_probs, seg.speaker_weights, seg.class_histogram] + \
             [getattr(p, k) for p in (plan, soft_plan) for k in PLAN_FIELDS]
 
-    first = run()
-    results = [None, None]
+    def device_decode_and_plan():
+        d_lp, d_w = _lib.DeviceBuffer(logits.nbytes), _lib.DeviceBuffer(chunks * frames * 3 * 4)
+        hist, speech = proc.decode_device(upload(logits), chunks, frames, classes, d_lp, d_w)
+        d_out = {k: _lib.DeviceBuffer(chunks * 3 * width * np.dtype(t).itemsize) for k, (t, width) in per_entry.items()}
+        count, counters = planner.plan_device(d_w, chunks, frames, 3, truth["chunk_offsets"], 10.0 / frames,
+                                              truth["total_samples"], d_out)
+        return [d_lp.download(logits.shape, np.float32), d_w.download((chunks, frames, 3), np.float32), hist,
+                np.array([speech, count, *counters.values()])] + \
+            [d_out[k].download((count, width), t) for k, (t, width) in per_entry.items()]
+
+    steps = [
+        host_decode_and_plan,
+        device_decode_and_plan,
+        lambda: list(proc.windows(audio)),
+        lambda: [AudioConverter(algorithm=Algorithm.sinc).resample(mono, 44100)],
+        lambda: [AudioConverter(algorithm=Algorithm.linear).resample_buffer(planar, 48000)],
+        lambda: [normalize_per_feature(mel, 250)],
+        lambda: (lambda r: [r.labels, r.initial, r.centroids])(OfflineClusterer(psi=psi).cluster(emb, rho)),
+    ]
+
+    def run(shift):   # every step, starting at step `shift`; results in step order
+        order = [(k + shift) % len(steps) for k in range(len(steps))]
+        out = {k: steps[k]() for k in order}
+        return [a for k in range(len(steps)) for a in out[k]]
+
+    first = run(0)
+    results = [None] * 4
 
     def worker(i):
         _lib.set_device(0)
-        results[i] = [run() for _ in range(3)]
+        results[i] = [run(i + r) for r in range(3)]
 
-    threads = [threading.Thread(target=worker, args=(i,)) for i in range(2)]
+    threads = [threading.Thread(target=worker, args=(i,)) for i in range(4)]
     for t in threads:
         t.start()
     for t in threads:
@@ -320,7 +362,7 @@ def test_results_are_identical_run_to_run_and_across_threads():
     for runs in results:
         assert runs is not None
         for again in runs:
-            assert all(same_bits(a, b) for a, b in zip(first, again))
+            assert len(again) == len(first) and all(same_bits(a, b) for a, b in zip(first, again))
 
 
 # ---- 11. the chain ------------------------------------------------------------------------------------------------------
