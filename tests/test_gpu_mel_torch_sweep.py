@@ -237,13 +237,14 @@ def test_against_the_oracle(gpu_lib, oracle, kind):
     print(f"  Cohere columns left to the bit-exact checks for a tiny spread ({kind}): {tiny}")
 
 
-def cmvn_frac(coh, a, got, ref, valid):
+def cmvn_frac(coh, a, got, ref, valid, e=None):
     """Worst |d| / bar of two Cohere feature arrays [M x T] over the columns where the first-order CMVN bar applies
     (test_gpu_mel_adapter_sweep.py), with the handle's own log-mel for the bar's magnitudes; and the count of columns
-    left out for a tiny spread (E > 0.05 sd)."""
-    lm = _log_mel(coh.mel, a, 1 + a.size // 160)
+    left out for a tiny spread (E > 0.05 sd).  ``e`` [valid x M]: the log-mel difference budget (default: the
+    generic-kernel bar of the handle's log-mel)."""
+    lm = _log_mel(coh.mel, a, 1 + a.size // coh.config.hop_length)
     cols = np.isfinite(got[:, :valid]).all(1) & np.isfinite(ref[:, :valid]).all(1)
-    e = _bar(lm[:valid].astype(np.float64))
+    e = _bar(lm[:valid].astype(np.float64)) if e is None else np.asarray(e, np.float64)
     E = e.max(0)
     z, sd = _cmvn64(lm, valid)
     use = cols & np.isfinite(sd) & (E <= 0.05 * sd)

@@ -9,19 +9,13 @@ shim (``tests/emul/mel_tables_shim.cpp``):
 """
 import ctypes as C
 import itertools
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from mel_ex_restated import mel_tables_lib
 from oracle import oracle_torch as OT
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "fluidaudio_b200", "csrc")
-F32P = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
-I32P = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
-U8P = np.ctypeslib.ndpointer(np.uint8, flags="C_CONTIGUOUS")
 FB_AUDIO_MEL, FB_COHERE, FB_STYLETTS2, FB_LUXTTS = 0, 1, 2, 3   # FA_MEL_FB_*
 EDGE_ZERO, EDGE_REFLECT = 0, 1                                  # FA_MEL_EDGE_*
 NFFTS = [32, 64, 128, 256, 512, 1024, 2048, 4096]
@@ -31,19 +25,7 @@ MELS = [1, 2, 3, 5, 23, 40, 64, 80, 100, 128, 200, 257, 400, 512]
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("mel_tables") / "libmel_tables.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-I", CSRC, "-I",
-                           os.path.join(ROOT, "include"), "-o", out, os.path.join(ROOT, "tests", "emul", "mel_tables_shim.cpp"),
-                           os.path.join(CSRC, "mel_tables.cpp")])
-    L = C.CDLL(out)
-    i32, f32 = C.c_int32, C.c_float
-    L.mt_tables.argtypes = [i32, i32, i32, i32, i32, i32, i32, f32, f32, F32P, F32P]
-    L.mt_pack_sizes.argtypes = [F32P, i32, i32, C.POINTER(i32), C.POINTER(i32)]
-    L.mt_pack.argtypes = [F32P, i32, i32, i32, f32, I32P, I32P, I32P, F32P, I32P]
-    L.mt_place_window.argtypes = [F32P, i32, i32, i32, F32P, U8P]
-    L.mt_check.argtypes = [i32, i32, i32, f32, f32, i32, f32, f32, f32, f32]
-    L.mt_check.restype = C.c_char_p
-    return L
+    return mel_tables_lib(str(tmp_path_factory.mktemp("mel_tables")))
 
 
 def tables(L, sr, n_mels, n_fft, win, periodic, kind, filter_sr=0, f_min=0.0, f_max=0.0):
