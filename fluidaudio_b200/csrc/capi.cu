@@ -654,22 +654,19 @@ FA_API fa_status fa_audio_resample(const void *pcm, int64_t frames, const fa_aud
     }
     const size_t bytes = (size_t)frames * f.channels * (f.format == resample::kPcmI16 ? 2 : 4);
     return (fa_status)with_context(0, [&](CallContext &C) -> int {
-        char *d_pcm = nullptr;
-        float *d_tab = nullptr, *d_out = nullptr;
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_pcm = c.take<char>(bytes + 16);
-            d_tab = c.take<float>(d.table.size());
-            d_out = c.take<float>((size_t)n);
+        HostStaging H(true, C.stream);
+        const char *d_pcm;
+        const float *d_tab;
+        float *d_out;
+        int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+            d_pcm = l.in(static_cast<const char *>(pcm), bytes, 16);
+            d_tab = l.in(d.table.empty() ? nullptr : d.table.data(), d.table.size());
+            d_out = l.out(out, (size_t)n);
         });
         if (st != FA_OK) return st;
-        if (!d.table.empty())
-            FA_CUDA_TRY(cudaMemcpyAsync(d_tab, d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice,
-                                        C.stream));
-        FA_CUDA_TRY(cudaMemcpyAsync(d_pcm, pcm, bytes, cudaMemcpyHostToDevice, C.stream));
         st = resample::launch_convert(d_pcm, frames, f, d, d_tab, d_out, 0, n, C.stream);
         if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+        FA_CUDA_TRY(H.finish());
         return FA_OK;
     });
     FA_GUARD_END

@@ -51,8 +51,9 @@ struct Pipeline {
     const bool speaker_count =
         cfg.num_speakers != FA_NO_VALUE || cfg.min_speakers != FA_NO_VALUE || cfg.max_speakers != FA_NO_VALUE;
     // the arenas: device, pinned host, and VBx's gamma / pi / ELBOs with the centroids (raw and normalised)
-    float *d_emb32;
-    double *d_emb, *d_rho, *d_train, *d_train_rho, *d_norm, *d_gamma, *d_pi, *d_elbos, *d_cent, *d_cent_n, *h_Z;
+    const float *d_emb32;
+    const double *d_rho;
+    double *d_emb, *d_train, *d_train_rho, *d_norm, *d_gamma, *d_pi, *d_elbos, *d_cent, *d_cent_n, *h_Z;
     unsigned char *d_ok, *h_ok;
     int *d_idx, *d_init, *d_hard, *d_labels, *d_count, *h_idx, *h_count;
     int32_t *h_init;
@@ -79,10 +80,11 @@ struct Pipeline {
     // 1. Upload, widen to double (:286) and keep the rows with a finite embedding (:591-611); when none is finite, every
     // row trains.
     int upload_and_filter() {
-        int st = carve_arena(C.d_buf, [&](Carver &c) {
-            d_emb32 = c.take<float>(N * E);
+        HostStaging H(true, s);
+        int st = H.carve(C.d_buf, [&](HostStaging::Layout &c) {
+            d_emb32 = c.in(emb, N * E);
             d_emb = c.take<double>(N * E);
-            d_rho = c.take<double>(N * R);
+            d_rho = c.in(rho, N * R);
             d_ok = c.take<unsigned char>(N);
             d_idx = c.take<int>(N);               // train idx
             d_train = c.take<double>(N * E);
@@ -102,8 +104,6 @@ struct Pipeline {
             h_Z = c.take<double>(N > 1 ? (N - 1) * 4 : 4);
         }, 4096);
         if (st != FA_OK) return st;
-        FA_CUDA_TRY(cudaMemcpyAsync(d_emb32, emb, N * E * sizeof(float), cudaMemcpyHostToDevice, s));
-        FA_CUDA_TRY(cudaMemcpyAsync(d_rho, rho, N * R * sizeof(double), cudaMemcpyHostToDevice, s));
         st = ahc::launch_widen_rows(d_emb32, d_emb, (long long)N * E, s);
         if (st != FA_OK) return st;
         st = vbx::finite_rows_device(d_emb32, n, e, d_ok, s);
@@ -374,31 +374,32 @@ int cluster_batch(const float *emb, const double *rho, const int64_t *set_offset
 }
 
 int l2_normalize_rows(CallContext &C, const double *x, size_t rows, size_t dim, double *out) {
-    double *d_in, *d_out;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_in = c.take<double>(rows * dim);
-        d_out = c.take<double>(rows * dim);
+    HostStaging H(true, C.stream);
+    const double *d_in;
+    double *d_out;
+    int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_in = l.in(x, rows * dim);
+        d_out = l.out(out, rows * dim);
     }, 512);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_in, x, rows * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     st = ahc::launch_normalize_rows(d_in, d_out, (int)rows, (int)dim, C.stream);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, rows * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 
 // AHCClustering.cluster (AHCClustering.swift:20-67) for count >= 2 and dim >= 1
 int ahc_cluster(CallContext &C, const double *features, size_t count, size_t dim, double threshold, int32_t *labels) {
-    double *d_in, *d_norm, *h_Z;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_in = c.take<double>(count * dim);
-        d_norm = c.take<double>(count * dim);
+    HostStaging H(true, C.stream);
+    const double *d_in;
+    double *d_norm, *h_Z;
+    int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_in = l.in(features, count * dim);
+        d_norm = l.take<double>(count * dim);
     }, 512);
     if (st != FA_OK) return st;
     st = carve_arena(C.h_buf, [&](Carver &c) { h_Z = c.take<double>((count - 1) * 4); }, 512);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_in, features, count * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     st = ahc::launch_normalize_rows(d_in, d_norm, (int)count, (int)dim, C.stream);
     if (st != FA_OK) return st;
     st = C.solver.linkage_device(d_norm, (int)count, (int)dim, h_Z);
@@ -416,22 +417,23 @@ int kmeans_cluster(CallContext &C, const double *emb, size_t N, size_t D, int32_
                    int32_t n_init, uint64_t base_seed, int32_t *labels, double *centroids, int32_t *centroid_rows,
                    int32_t *best_init) {
     const size_t rows_needed = std::min<size_t>((size_t)num_clusters, N);
-    double *d_emb, *d_cent;
+    HostStaging H(true, C.stream);
+    const double *d_emb;
+    double *d_cent;
     int *d_labels;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_emb = c.take<double>(N * D);
-        d_cent = c.take<double>(rows_needed * D);
-        d_labels = c.take<int>(N);
+    int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_emb = l.in(emb, N * D);
+        d_cent = l.out(centroids, rows_needed * D);
+        d_labels = l.out(labels, N);
     }, 1024);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     int rows = 0, best = 0;
     st = kmeans::cluster_ninit_device(C.vbx_pool, d_emb, (int)N, (int)D, num_clusters, max_iterations, n_init, base_seed,
                                       d_labels, d_cent, &rows, &best, C.stream);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)rows * D * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(H.back(labels, d_labels, N));
+    FA_CUDA_TRY(H.back(centroids, d_cent, (size_t)rows * D));   // the rows K-Means returned
+    FA_CUDA_TRY(H.sync());
     if (centroid_rows) *centroid_rows = rows;
     if (best_init) *best_init = best;
     return FA_OK;
@@ -441,59 +443,55 @@ int vbx_refine(CallContext &C, const double *rho, size_t T, size_t D, const doub
                const int32_t *initial, int32_t S, const fa_vbx_config &cfg, double *gamma, double *pi, double *elbos,
                int32_t *hard, int32_t *iterations) {
     const int cap = std::max(cfg.max_iterations, 1);
-    double *d_x, *d_gamma, *d_pi, *d_elbos;
-    int *d_init, *d_hard;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_x = c.take<double>(T * D);
-        d_init = c.take<int>(T);
-        d_gamma = c.take<double>(T * (size_t)S);
-        d_pi = c.take<double>(S);
-        d_elbos = c.take<double>(cap);
-        d_hard = c.take<int>(T);
+    HostStaging H(true, C.stream);
+    const double *d_x;
+    const int *d_init;
+    double *d_gamma, *d_pi, *d_elbos;
+    int *d_hard;
+    int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_x = l.in(rho, T * D);
+        d_init = l.in(initial, T);
+        d_gamma = l.out(gamma, T * (size_t)S);
+        d_pi = l.out(pi, S);
+        d_elbos = l.out(elbos, cap);
+        d_hard = l.out(hard, T);
     }, 1024);
     if (st != FA_OK) return st;
     std::vector<double> psi_eff(D, 1.0);
     if (psi && psi_len == D) std::memcpy(psi_eff.data(), psi, D * sizeof(double));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_x, rho, T * D * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    if (initial) FA_CUDA_TRY(cudaMemcpyAsync(d_init, initial, T * sizeof(int), cudaMemcpyHostToDevice, C.stream));
     int its = 0;
-    st = vbx::refine_device(C.vbx_pool, d_x, (int)T, (int)D, psi_eff.data(), initial ? d_init : nullptr, S, to_vbx(cfg),
-                            d_gamma, d_pi, d_elbos, d_hard, &its, C.stream);
+    st = vbx::refine_device(C.vbx_pool, d_x, (int)T, (int)D, psi_eff.data(), d_init, S, to_vbx(cfg), d_gamma, d_pi, d_elbos,
+                            d_hard, &its, C.stream);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(gamma, d_gamma, T * (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(pi, d_pi, S * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(elbos, d_elbos, cap * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(hard, d_hard, T * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(H.finish());
     if (iterations) *iterations = its;
     return FA_OK;
 }
 
 int compute_centroids(CallContext &C, const double *emb, size_t T, size_t dim, const double *gamma, const double *pi,
                       int32_t S, double *centroids, int32_t *centroid_count) {
-    double *d_emb, *d_gamma, *d_pi, *d_cent, *d_cent_n;
+    HostStaging H(true, C.stream);
+    const double *d_emb, *d_gamma, *d_pi;
+    double *d_cent, *d_cent_n;
     int *d_count;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_emb = c.take<double>(T * dim);
-        d_gamma = c.take<double>(T * (size_t)S);
-        d_pi = c.take<double>(S);
-        d_cent = c.take<double>((size_t)S * dim);
-        d_cent_n = c.take<double>((size_t)S * dim);
-        d_count = c.take<int>(64);
+    int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_emb = l.in(emb, T * dim);
+        d_gamma = l.in(gamma, T * (size_t)S);
+        d_pi = l.in(pi, S);
+        d_cent = l.out(centroids, (size_t)S * dim);
+        d_cent_n = l.take<double>((size_t)S * dim);
+        d_count = l.take<int>(64);
     }, 1024);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, T * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_gamma, gamma, T * (size_t)S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_pi, pi, S * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     st = vbx::centroids_device(C.vbx_pool, d_emb, (int)T, (int)dim, d_gamma, d_pi, S, d_cent, d_cent_n, d_count, C.stream);
     if (st != FA_OK) return st;
     int K = 0;
     FA_CUDA_TRY(cudaMemcpyAsync(&K, d_count, sizeof(int), cudaMemcpyDeviceToHost, C.stream));
     FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
     *centroid_count = K;
-    if (K > 0) {
-        FA_CUDA_TRY(cudaMemcpyAsync(centroids, d_cent, (size_t)K * dim * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    if (K > 0) {   // the centroids of the K speakers kept
+        FA_CUDA_TRY(H.back(centroids, d_cent, (size_t)K * dim));
+        FA_CUDA_TRY(H.sync());
     }
     return FA_OK;
 }
@@ -501,27 +499,24 @@ int compute_centroids(CallContext &C, const double *emb, size_t T, size_t dim, c
 // OfflineDiarizerManager.assignEmbeddings (:789-883) for N >= 1 and K >= 1
 int assign_embeddings(CallContext &C, const double *emb, size_t N, size_t dim, const double *centroids, int32_t K,
                       int32_t *labels, double *scores) {
-    double *d_emb, *d_craw, *d_cn, *d_scores;
+    HostStaging H(true, C.stream);
+    const double *d_emb, *d_craw;
+    double *d_cn, *d_scores;
     int *d_labels;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        d_emb = c.take<double>(N * dim);
-        d_craw = c.take<double>((size_t)K * dim);
-        d_cn = c.take<double>((size_t)K * dim);
-        d_labels = c.take<int>(N);
-        d_scores = c.take<double>(scores ? N * (size_t)K : 1);
+    int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_emb = l.in(emb, N * dim);
+        d_craw = l.in(centroids, (size_t)K * dim);
+        d_cn = l.take<double>((size_t)K * dim);
+        d_labels = l.out(labels, N);
+        d_scores = l.out(scores, N * (size_t)K);
     }, 1024);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d_emb, emb, N * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_craw, centroids, (size_t)K * dim * sizeof(double), cudaMemcpyHostToDevice, C.stream));
     // centroid normalisation (:793, :824-860; zero rows kept) with the same kernel the pipeline uses
     st = ahc::launch_normalize_rows_keep(d_craw, d_cn, K, (int)dim, C.stream);
     if (st != FA_OK) return st;
-    st = vbx::assign_device(d_emb, (int)N, (int)dim, d_cn, nullptr, K, d_labels, scores ? d_scores : nullptr, C.stream);
+    st = vbx::assign_device(d_emb, (int)N, (int)dim, d_cn, nullptr, K, d_labels, d_scores, C.stream);
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(labels, d_labels, N * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
-    if (scores)
-        FA_CUDA_TRY(cudaMemcpyAsync(scores, d_scores, N * (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 

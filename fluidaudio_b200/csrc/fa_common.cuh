@@ -115,18 +115,96 @@ template <typename T, bool Pinned> class GrowBuffer {
 template <typename T = void> using DeviceBuffer = GrowBuffer<T, false>;
 template <typename T = void> using PinnedBuffer = GrowBuffer<T, true>;
 
-// Lays out one scratch arena in a grow-only buffer.  `layout(Carver &)` takes every array of the arena in order and
-// only assigns the pointers it gets, so it is safe to run twice: once over a null base to size the arena (plus `slack`
-// bytes), then, after the buffer has grown to that size, over the buffer itself.
+// The device twins of one call's caller arrays.  On a device-buffer call a twin is the caller's own pointer: nothing is
+// copied and the call stays asynchronous.  On a host-buffer call every twin is carved from one grow-only buffer, the
+// inputs are copied in on the call's stream, back() copies the outputs out and sync() waits for them.  A null caller
+// array has a null twin.  One per call, on the stack; it owns no memory.
+class HostStaging {
+  public:
+    HostStaging(bool host, cudaStream_t stream) : host_(host), stream_(stream) {}
+
+    // What carve()'s layout takes, in order: twins (an input's `slack` elements are carved but not copied) and scratch
+    // (Carver::take), which is carved on either kind of call.
+    class Layout : public Carver {
+      public:
+        template <typename T> const T *in(const T *p, size_t n, size_t slack = 0) {
+            return twin(const_cast<T *>(p), n, slack, kIn);
+        }
+        template <typename T> T *out(T *p, size_t n) { return twin(p, n, 0, kOut); }
+        template <typename T> T *inout(T *p, size_t n) { return twin(p, n, 0, kIn | kOut); }
+
+      private:
+        friend class HostStaging;
+        Layout(char *base, HostStaging &s, bool record) : Carver{base}, s_(s), record_(record) {}
+        template <typename T> T *twin(T *p, size_t n, size_t slack, int dir) {
+            if (!p || !s_.host_) return p;
+            T *t = take<T>(n + slack);
+            if (record_ && s_.count_++ < kMaxTwins) s_.twins_[s_.count_ - 1] = Twin{p, t, n * sizeof(T), dir};
+            return t;
+        }
+        HostStaging &s_;
+        bool record_;
+    };
+
+    // `layout(Layout &)` takes every array in order and only assigns the pointers it gets, so it is safe to run twice:
+    // once over a null base to size the arrays (plus `slack` bytes), then, after `buf` has grown to that size, over the
+    // buffer itself.  Then the inputs' copies are queued.  A device-buffer call without scratch grows nothing.
+    template <typename T, bool Pinned, typename L> int carve(GrowBuffer<T, Pinned> &buf, L &&layout, size_t slack = 0) {
+        Layout size(nullptr, *this, false);
+        layout(size);
+        const int st = buf.grow(size.off + slack);
+        if (st != FA_OK) return st;
+        Layout c(static_cast<char *>(static_cast<void *>(buf.data())), *this, true);
+        count_ = 0;
+        layout(c);
+        if (count_ > kMaxTwins) {
+            set_error("internal: a call stages %d arrays, at most %d", count_, kMaxTwins);
+            return FA_RUNTIME_ERROR;
+        }
+        for (int i = 0; i < count_; ++i)
+            if ((twins_[i].dir & kIn) && twins_[i].bytes)
+                FA_CUDA_TRY(cudaMemcpyAsync(twins_[i].dev, twins_[i].host, twins_[i].bytes, cudaMemcpyHostToDevice, stream_));
+        return FA_OK;
+    }
+    // Queues the copy of every out / inout twin to its caller array: whole, or, when each holds `of` rows, its first
+    // `rows` rows (outputs whose row count the device decides).
+    cudaError_t back(size_t rows = 1, size_t of = 1) const {
+        cudaError_t e = cudaSuccess;
+        for (int i = 0; i < count_ && e == cudaSuccess; ++i) {
+            const size_t bytes = twins_[i].bytes / of * rows;
+            if ((twins_[i].dir & kOut) && bytes)
+                e = cudaMemcpyAsync(twins_[i].host, twins_[i].dev, bytes, cudaMemcpyDeviceToHost, stream_);
+        }
+        return e;
+    }
+    // Queues the copy of the first n elements of one twin.
+    template <typename T> cudaError_t back(T *p, const T *twin, size_t n) const {
+        return host_ && p && n ? cudaMemcpyAsync(p, twin, n * sizeof(T), cudaMemcpyDeviceToHost, stream_) : cudaSuccess;
+    }
+    cudaError_t sync() const { return host_ ? cudaStreamSynchronize(stream_) : cudaSuccess; }
+    // back() then sync(): the end of a host-buffer call whose outputs return whole
+    cudaError_t finish() const {
+        const cudaError_t e = back();
+        return e != cudaSuccess ? e : sync();
+    }
+
+  private:
+    enum : int { kIn = 1, kOut = 2, kMaxTwins = 16 };
+    struct Twin {
+        void *host, *dev;
+        size_t bytes;
+        int dir;
+    };
+    bool host_;
+    cudaStream_t stream_;
+    int count_ = 0;
+    Twin twins_[kMaxTwins];
+};
+
+// Lays out one scratch arena in a grow-only buffer: a carve with Carver::take alone, which copies nothing.
 template <typename T, bool Pinned, typename Layout>
 int carve_arena(GrowBuffer<T, Pinned> &buf, Layout &&layout, size_t slack = 0) {
-    Carver size{nullptr};
-    layout(size);
-    const int st = buf.grow(size.off + slack);
-    if (st != FA_OK) return st;
-    Carver c{static_cast<char *>(static_cast<void *>(buf.data()))};
-    layout(c);
-    return FA_OK;
+    return HostStaging(false, nullptr).carve(buf, layout, slack);
 }
 
 // Moves a session set's two per-slot device arrays (a_slot and b_slot elements per slot) into buffers of `grown` slots,

@@ -79,15 +79,13 @@ __global__ void per_feature_norm_inplace_kernel(float *x, long long T, int M, lo
 
 // host buffer in, host buffer out (x: [T x M] time-major, normalised in place), staged in the context's d_buf; valid >= 1
 int normalize_per_feature_host(CallContext &C, float *x, long long T, int M, long long valid) {
-    float *d = nullptr;
-    const size_t count = (size_t)T * M;
-    const int st = carve_arena(C.d_buf, [&](Carver &c) { d = c.take<float>(count); });
+    HostStaging H(true, C.stream);
+    float *d;
+    const int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) { d = l.inout(x, (size_t)T * M); });
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(d, x, count * sizeof(float), cudaMemcpyHostToDevice, C.stream));
     FA_CUDA_TRY(fa::launch(per_feature_norm_inplace_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, C.stream, d,
                            T, M, valid));
-    FA_CUDA_TRY(cudaMemcpyAsync(x, d, count * sizeof(float), cudaMemcpyDeviceToHost, C.stream));
-    FA_CUDA_TRY(cudaStreamSynchronize(C.stream));
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 
@@ -133,13 +131,18 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
         fa::set_error("unified mel features need %lld floats, buffer has %lld", T * M, out_len);
         return FA_OUTPUT_TOO_SMALL;
     }
-    st = p.ensure_staging((size_t)n + 16, (size_t)(2 * T * M));
-    if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
-    float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
-    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), window, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    HostStaging H(true, s);
+    const float *d_audio;
+    float *d_flat, *d_pack;
+    st = H.carve(p.staging, [&](HostStaging::Layout &l) {
+        d_audio = l.in(window, (size_t)n, 16);
+        d_flat = l.take<float>((size_t)(T * M));
+        d_pack = l.out(out, (size_t)(T * M));
+    });
+    if (st != FA_OK) return st;
     long long ml = 0, nf = 0;
-    st = p.compute_device(p.d_audio.data(), n, 0.0f, FA_MEL_PAD_CENTER, T, FA_MEL_TIME_MAJOR, d_flat, T * M, &ml, &nf, s);
+    st = p.compute_device(d_audio, n, 0.0f, FA_MEL_PAD_CENTER, T, FA_MEL_TIME_MAJOR, d_flat, T * M, &ml, &nf, s);
     if (st != FA_OK) return st;
     if (valid <= 0) {
         FA_CUDA_TRY(cudaMemsetAsync(d_pack, 0, sizeof(float) * T * M, s));
@@ -147,8 +150,7 @@ int unified_features(MelPlan &p, const float *window, long long n, long long val
         FA_CUDA_TRY(fa::launch(per_feature_norm_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, s, d_flat, T, M,
                                valid, d_pack));
     }
-    FA_CUDA_TRY(cudaMemcpyAsync(out, d_pack, sizeof(float) * T * M, cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 
@@ -164,21 +166,22 @@ int lseend_features(MelPlan &p, const float *chunk, long long n, float *cmn_mean
         fa::set_error("LS-EEND features need %lld floats, buffer has %lld", T * M, out_len);
         return FA_OUTPUT_TOO_SMALL;
     }
-    st = p.ensure_staging((size_t)n + 16, (size_t)(T * M + M));
-    if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
-    float *d_flat = p.d_out.data(), *d_mean = d_flat + T * M;
-    FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), chunk, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    FA_CUDA_TRY(cudaMemcpyAsync(d_mean, cmn_mean, sizeof(float) * M, cudaMemcpyHostToDevice, s));
+    HostStaging H(true, s);
+    const float *d_audio;
+    float *d_flat, *d_mean;
+    st = H.carve(p.staging, [&](HostStaging::Layout &l) {
+        d_audio = l.in(chunk, (size_t)n, 16);
+        d_flat = l.out(out, (size_t)(T * M));
+        d_mean = l.inout(cmn_mean, (size_t)M);
+    });
+    if (st != FA_OK) return st;
     long long ml = 0, nf = 0;
-    st = p.compute_device(p.d_audio.data(), n, 0.0f, FA_MEL_PAD_PREPADDED, -1, FA_MEL_TIME_MAJOR, d_flat, T * M, &ml, &nf,
-                          s);
+    st = p.compute_device(d_audio, n, 0.0f, FA_MEL_PAD_PREPADDED, -1, FA_MEL_TIME_MAJOR, d_flat, T * M, &ml, &nf, s);
     if (st != FA_OK) return st;
     const float scale = 1.0f / logf(10.0f);   // LSEENDPreprocessor.swift:36, Float arithmetic
     FA_CUDA_TRY(fa::launch(lseend_scale_cmn_kernel, (M + 127) / 128, 128, 0, s, d_flat, T, M, d_mean, *cmn_count, scale));
-    FA_CUDA_TRY(cudaMemcpyAsync(out, d_flat, sizeof(float) * T * M, cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaMemcpyAsync(cmn_mean, d_mean, sizeof(float) * M, cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    FA_CUDA_TRY(H.finish());
     *cmn_count += T;
     return FA_OK;
 }
@@ -257,31 +260,38 @@ int cohere_features(MelPlan &p, const float *audio, long long n, long long fixed
     if (valid_frames) *valid_frames = std::min(valid, W);
     st = check_out(what, W * M, out_len);
     if (st != FA_OK) return st;
-    st = p.ensure_staging((size_t)n + 16, (size_t)((T + W) * M));
-    if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
-    float *d_flat = p.d_out.data(), *d_pack = d_flat + T * M;
-    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    st = p.launch_clip(p.d_audio.data(), n, T, FA_MEL_TIME_MAJOR, d_flat, s);
+    HostStaging H(true, s);
+    const float *d_audio;
+    float *d_flat, *d_pack;
+    st = H.carve(p.staging, [&](HostStaging::Layout &l) {
+        d_audio = l.in(audio, (size_t)n, 16);
+        d_flat = l.take<float>((size_t)(T * M));
+        d_pack = l.out(out, (size_t)(W * M));
+    });
+    if (st != FA_OK) return st;
+    st = p.launch_clip(d_audio, n, T, FA_MEL_TIME_MAJOR, d_flat, s);
     if (st != FA_OK) return st;
     FA_CUDA_TRY(fa::launch(cohere_cmvn_kernel, (M + kBinsPerCta - 1) / kBinsPerCta, kBinsPerCta, 0, s, d_flat, M, valid, W,
                            1.0e-5f, d_pack));   // Config.cmvnEpsilon
-    if (W) FA_CUDA_TRY(cudaMemcpyAsync(out, d_pack, sizeof(float) * W * M, cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 
 // host clip in, one launch of T frames in `layout`, rows out
 static int run_clip(MelPlan &p, const float *audio, long long n, long long T, int layout, float *out) {
-    const long long need = T * p.cfg.n_mels;
-    int st = p.ensure_staging((size_t)n + 16, (size_t)need);
-    if (st != FA_OK) return st;
     cudaStream_t s = p.streams[1];
-    if (n) FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio, sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    st = p.launch_clip(p.d_audio.data(), n, T, layout, p.d_out.data(), s);
+    HostStaging H(true, s);
+    const float *d_audio;
+    float *d_out;
+    int st = H.carve(p.staging, [&](HostStaging::Layout &l) {
+        d_audio = l.in(audio, (size_t)n, 16);
+        d_out = l.out(out, (size_t)(T * p.cfg.n_mels));
+    });
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpyAsync(out, p.d_out.data(), sizeof(float) * need, cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    st = p.launch_clip(d_audio, n, T, layout, d_out, s);
+    if (st != FA_OK) return st;
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 

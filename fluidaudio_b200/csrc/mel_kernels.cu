@@ -588,11 +588,6 @@ long long MelPlan::frame_count(long long n, int mode, long long expected) const 
     return expected >= 0 ? expected : computed;
 }
 
-int MelPlan::ensure_staging(size_t audio_floats, size_t out_floats) {
-    const int st = d_audio.grow(audio_floats * sizeof(float));
-    return st != FA_OK ? st : d_out.grow(out_floats * sizeof(float));
-}
-
 int MelPlan::ensure_events(size_t count) {
     while (events.size() < count) {
         Event e;

@@ -127,17 +127,17 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
     const long long need = Tp * cfg.n_mels;
     st = ensure_resampler(f.in_rate, f.out_rate);
     if (st != FA_OK) return st;
-    st = ensure_staging((size_t)n + 8, (size_t)need);
-    if (st != FA_OK) return st;
     const size_t bps = f.format == resample::kPcmI16 ? 2 : 4;
     const size_t pcm_bytes = (size_t)frames * f.channels * bps;
-    float *const d_f32 = d_audio.data(), *const d_rows = d_out.data();   // kernel input, staged output
-    char *d_in = reinterpret_cast<char *>(d_f32);   // where the input lands
-    if (!identity) {
-        st = d_pcm.grow(pcm_bytes + 16);
-        if (st != FA_OK) return st;
-        d_in = static_cast<char *>(d_pcm.data());
-    }
+    float *d_f32, *d_rows;   // kernel input, staged output
+    char *d_pcm = nullptr;   // the raw PCM of converted input
+    st = carve_arena(staging, [&](Carver &c) {
+        d_f32 = c.take<float>((size_t)n + 8);
+        d_rows = c.take<float>((size_t)need);
+        if (!identity) d_pcm = c.take<char>(pcm_bytes + 16);
+    });
+    if (st != FA_OK) return st;
+    char *const d_in = identity ? reinterpret_cast<char *>(d_f32) : d_pcm;   // where the input lands
     // Units: pipeline_chunks for identity input; converted input keeps ~10 MB of PCM per unit (the copy engines' fixed
     // cost per transfer and the host's enqueue rate make finer units slower there: int16 hour 3.08 ms at 8-12 units,
     // 3.44 at 24, 3.61 at 96).
@@ -208,7 +208,7 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
                 fa::set_error("internal: resampler window accounting (%lld < %lld)", ready, s_end);
                 return FA_RUNTIME_ERROR;
             }
-            st = resample::launch_convert(d_pcm.data(), frames, f, D, d_rs_tab.data(), d_f32, converted, s_end, s_k);
+            st = resample::launch_convert(d_pcm, frames, f, D, d_rs_tab.data(), d_f32, converted, s_end, s_k);
             if (st != FA_OK) return st;
             converted = std::max(converted, s_end);
         }
@@ -262,7 +262,11 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
     }
     doff[count] = a;
     dout[count] = o;
-    int st = ensure_staging((size_t)a + 8, (size_t)o);
+    float *d_f32, *d_rows;
+    int st = carve_arena(staging, [&](Carver &c) {
+        d_f32 = c.take<float>((size_t)a + 8);
+        d_rows = c.take<float>((size_t)o);
+    });
     if (st != FA_OK) return st;
     st = units.reserve(unit_bytes(count));
     if (st != FA_OK) return st;
@@ -286,7 +290,6 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
         st = units.upload(used * sizeof(MelUnit), s_k);
         if (st != FA_OK) return st;
     }
-    float *const d_f32 = d_audio.data(), *const d_rows = d_out.data();
     FA_CUDA_TRY(cudaMemsetAsync(d_rows, 0, (size_t)o * sizeof(float), s_k));
     for (int g = 0; g < groups; ++g) {
         const int c0 = (int)((long long)count * g / groups), c1 = (int)((long long)count * (g + 1) / groups);

@@ -96,16 +96,14 @@ struct MelPlan {
 
     // buffers grown on demand
     UploadStage<MelUnit> units;                    // unit descriptors of every launch
-    DeviceBuffer<float> d_audio, d_out;            // staging for the host-buffer entry points
-    // AudioConverter stage ahead of the kernel (fa_audio_to_mel): raw PCM staging + the polyphase table of the last ratio
-    DeviceBuffer<> d_pcm;
+    DeviceBuffer<> staging;                        // the host-buffer entry points' arrays (HostStaging, fa_common.cuh)
+    // AudioConverter stage ahead of the kernel (fa_audio_to_mel): the polyphase table of the last ratio
     resample::Design rs_design;
     double rs_in = 0.0, rs_out = 0.0;
     DeviceBuffer<float> d_rs_tab;
 
     int init(const MelConfig &c);
     long long frame_count(long long n, int mode, long long expected) const;
-    int ensure_staging(size_t audio_floats, size_t out_floats);
     int ensure_events(size_t count);
     // kernel launch over `count` units at d_u (device) whose host mirror is h_u, numbered by number_tiles (the last unit
     // gives the tile total; h_u is also read for the alignment of the audio and of the output rows).

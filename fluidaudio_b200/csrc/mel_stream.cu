@@ -12,13 +12,13 @@
 // One push, whatever the number of sessions:
 //   H2D samples (host push) + H2D descriptors -> mel_stream_ingest_kernel (one CTA per session with work) -> one
 //   MelPlan launch over the emitting sessions' units (.prePadded, time-major) -> D2H rows + synchronise (host push).
+// A host push stages its samples and rows in the plan's staging buffer (HostStaging, fa_common.cuh).
 // The ingest CTA assembles [carry | new samples | tail] contiguously at a 16-byte aligned arena offset (the mel kernel's
 // bulk-copy path), copies the session's `last` into its MelUnit, then writes back the new carry and `last`.
 #include "fa_common.cuh"
 #include "mel_plan.h"
 
 #include <algorithm>
-#include <cstring>
 #include <cuda_runtime.h>
 #include <vector>
 
@@ -200,12 +200,20 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         return FA_OUTPUT_TOO_SMALL;
     }
 
-    // ---- buffers
+    // ---- buffers: the pushed samples, from offsets[0] on, and the rows
+    cudaStream_t s = p.streams[1];
+    HostStaging H(!device, s);
+    const float *src;
+    float *k_out;
     const size_t units_bytes = (((size_t)units * sizeof(MelUnit)) + 15) & ~size_t(15);
     const size_t desc_bytes = units_bytes + (size_t)jobs * sizeof(MelStreamJob);
     st = desc.reserve(std::max<size_t>(desc_bytes, 4096));
     if (st == FA_OK) st = d_arena.grow((size_t)std::max(arena, 1024LL) * sizeof(float));
-    if (st == FA_OK && !device) st = p.ensure_staging((size_t)std::max(total_new, 0LL) + 8, (size_t)rows * M);
+    if (st == FA_OK)
+        st = H.carve(p.staging, [&](HostStaging::Layout &l) {
+            src = l.in(audio ? audio + offsets[0] : nullptr, (size_t)total_new, 8);
+            k_out = l.out(out, (size_t)(rows * M));
+        });
     if (st != FA_OK) return st;
 
     // ---- descriptors: units, then jobs
@@ -213,7 +221,6 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     MelStreamJob *hj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(desc.host.data()) + units_bytes);
     MelUnit *du = static_cast<MelUnit *>(desc.device.data());
     MelStreamJob *dj = reinterpret_cast<MelStreamJob *>(static_cast<char *>(desc.device.data()) + units_bytes);
-    const long long src0 = device ? 0 : offsets[0];   // a host push's samples land at d_audio[0]
     long long row = 0, a = 0;
     int u = 0, j = 0;
     for (int i = 0; i < count; ++i) {
@@ -222,7 +229,7 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         const long long n = offsets[i + 1] - offsets[i], emit = S.first + S.second;
         if (table[id].finished || (emit == 0 && (n == 0 || S.fin))) continue;
         MelStreamJob &J = hj[j++];
-        J = MelStreamJob{offsets[i] - src0, n, -1, -1, id, (int)table[id].carry_len, 0, 0, -1, S.fin ? 1 : 0};
+        J = MelStreamJob{offsets[i] - offsets[0], n, -1, -1, id, (int)table[id].carry_len, 0, 0, -1, S.fin ? 1 : 0};
         if (emit == 0) continue;
         const bool split = S.first > 0 && S.second > 0;
         J.consumed = (int)(S.first * hop);
@@ -244,14 +251,6 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     number_tiles(hu, units);
 
     // ---- device work, all on the compute stream
-    cudaStream_t s = p.streams[1];
-    const float *src = audio;
-    if (!device) {
-        if (total_new > 0)
-            FA_CUDA_TRY(cudaMemcpyAsync(p.d_audio.data(), audio + offsets[0], (size_t)total_new * sizeof(float),
-                                        cudaMemcpyHostToDevice, s));
-        src = p.d_audio.data();
-    }
     if (desc_bytes) {
         st = desc.upload(desc_bytes, s);
         if (st != FA_OK) return st;
@@ -260,16 +259,12 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
         FA_CUDA_TRY(fa::launch(mel_stream_ingest_kernel, jobs, kIngestThreads, 0, s, dj, src, d_carry.data(), d_last.data(),
                                d_arena.data(), du, capacity, c.preemph));
     }
-    float *k_out = device ? out : p.d_out.data();
     if (units) {
         // `last` lives in the device units (written by the ingest kernel): the launch reads them from HBM, never inline
         st = p.launch(du, hu, units, false, d_arena.data(), k_out, FA_MEL_PAD_PREPADDED, FA_MEL_TIME_MAJOR, s);
         if (st != FA_OK) return st;
     }
-    if (!device) {
-        if (rows) FA_CUDA_TRY(cudaMemcpyAsync(out, p.d_out.data(), (size_t)rows * M * sizeof(float), cudaMemcpyDeviceToHost, s));
-        FA_CUDA_TRY(cudaStreamSynchronize(s));
-    }
+    FA_CUDA_TRY(H.finish());
 
     table.commit(count, sessions, next.data());
     for (int i = 0; i < count; ++i) frames_out[i] = step[i].first + step[i].second;

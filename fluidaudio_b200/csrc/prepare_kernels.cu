@@ -19,7 +19,6 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
-#include <vector>
 
 namespace fa {
 namespace prepare {
@@ -358,16 +357,6 @@ template <typename Kernel> int allow_smem(Kernel kernel, size_t bytes, const cha
     return FA_OK;
 }
 
-// A device copy of a host array for the host-buffer calls, in its staging carved from the context's d_buf (null and
-// empty arrays stay null).
-template <typename T> int to_device(T *staging, const T *host, size_t count, cudaStream_t s, const T *&dev) {
-    dev = nullptr;
-    if (!host || !count) return FA_OK;
-    FA_CUDA_TRY(cudaMemcpyAsync(staging, host, count * sizeof(T), cudaMemcpyHostToDevice, s));
-    dev = staging;
-    return FA_OK;
-}
-
 } // namespace
 
 bool seg_config_ok(const SegConfig &c) {
@@ -399,26 +388,23 @@ WindowDesc embed_window(double chunk_offset, long long total_samples, const SegC
 int gather_windows(CallContext &C, bool on_device, const float *audio, long long total_samples, const WindowDesc *desc,
                    int count, long long row_len, float *out) {
     const cudaStream_t s = C.stream;
-    const size_t desc_bytes = (size_t)count * sizeof(WindowDesc), out_floats = (size_t)count * (size_t)row_len;
+    const size_t desc_bytes = (size_t)count * sizeof(WindowDesc);
     int st = C.stage.reserve(desc_bytes);
     if (st != FA_OK) return st;
     std::copy(desc, desc + count, static_cast<WindowDesc *>(C.stage.host.data()));
     if ((st = C.stage.upload(desc_bytes, s)) != FA_OK) return st;
-    const float *d_audio = audio;
-    float *d_out = out;
-    if (!on_device) {
-        float *audio_stage = nullptr;
-        st = carve_arena(C.d_buf, [&](Carver &c) {
-            audio_stage = c.take<float>((size_t)total_samples);
-            d_out = c.take<float>(out_floats);
-        });
-        if (st != FA_OK) return st;
-        if ((st = to_device(audio_stage, audio, (size_t)total_samples, s, d_audio)) != FA_OK) return st;
-    }
+    HostStaging H(!on_device, s);
+    const float *d_audio;
+    float *d_out;
+    st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_audio = l.in(audio, (size_t)total_samples);
+        d_out = l.out(out, (size_t)count * (size_t)row_len);
+    });
+    if (st != FA_OK) return st;
     const unsigned tiles = (unsigned)std::min<long long>(16, (row_len + 4 * kThreads - 1) / (4 * kThreads));
     FA_CUDA_TRY(launch(seg_windows_kernel, dim3((unsigned)count, std::max(1u, tiles)), dim3(kThreads), 0, s, d_audio,
                        static_cast<const WindowDesc *>(C.stage.device.data()), row_len, d_out));
-    if (!on_device) FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, out_floats * sizeof(float), cudaMemcpyDeviceToHost, s));
+    FA_CUDA_TRY(H.back());
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     return FA_OK;
 }
@@ -427,31 +413,25 @@ int seg_decode(CallContext &C, bool on_device, const float *logits, int chunks, 
                float *log_probs, float *speaker_weights, int64_t histogram[8], int64_t *speech_frames) {
     const cudaStream_t s = C.stream;
     const long long total = (long long)chunks * frames;
-    const size_t in_floats = (size_t)total * classes, w_floats = (size_t)total * kDecodeSpeakers;
+    const size_t in_floats = (size_t)total * classes;
     constexpr size_t kTallyBytes = (kPowersetClasses + 1) * sizeof(unsigned long long);
     int st = C.scratch.grow(kTallyBytes);
     if (st != FA_OK) return st;
     auto *tallies = static_cast<unsigned long long *>(C.scratch.data());
     FA_CUDA_TRY(cudaMemsetAsync(tallies, 0, kTallyBytes, s));
-    const float *d_logits = logits;
-    float *d_lp = log_probs, *d_w = speaker_weights;
-    if (!on_device) {
-        float *logits_stage = nullptr;
-        st = carve_arena(C.d_buf, [&](Carver &c) {
-            logits_stage = c.take<float>(in_floats);
-            if (log_probs) d_lp = c.take<float>(in_floats);
-            d_w = c.take<float>(w_floats);
-        });
-        if (st != FA_OK) return st;
-        if ((st = to_device(logits_stage, logits, in_floats, s, d_logits)) != FA_OK) return st;
-    }
+    HostStaging H(!on_device, s);
+    const float *d_logits;
+    float *d_lp, *d_w;
+    st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_logits = l.in(logits, in_floats);
+        d_lp = l.out(log_probs, in_floats);
+        d_w = l.out(speaker_weights, (size_t)total * kDecodeSpeakers);
+    });
+    if (st != FA_OK) return st;
     const size_t smem = sizeof(float) * kThreads * ((size_t)(classes | 1) + kDecodeSpeakers);
     FA_CUDA_TRY(launch(seg_decode_kernel, dim3((unsigned)((total + kThreads - 1) / kThreads)), dim3(kThreads), smem, s,
                        d_logits, total, classes, onset, d_lp, d_w, tallies));
-    if (!on_device) {
-        if (log_probs) FA_CUDA_TRY(cudaMemcpyAsync(log_probs, d_lp, in_floats * sizeof(float), cudaMemcpyDeviceToHost, s));
-        FA_CUDA_TRY(cudaMemcpyAsync(speaker_weights, d_w, w_floats * sizeof(float), cudaMemcpyDeviceToHost, s));
-    }
+    FA_CUDA_TRY(H.back());
     unsigned long long host_tallies[kPowersetClasses + 1];
     FA_CUDA_TRY(cudaMemcpyAsync(host_tallies, tallies, kTallyBytes, cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));
@@ -496,27 +476,24 @@ int embedding_plan(CallContext &C, bool on_device, const float *speaker_weights,
 
     // the host-buffer call stages the weights and packs into device arrays of full capacity, then copies the emitted
     // entries back
-    PlanOutputs d = out;
-    const float *d_weights = speaker_weights;
-    float *weights_stage = nullptr;
-    auto host_layout = [&](Carver &c) {
-        weights_stage = c.take<float>(w_floats);
-        if (out.chunk_index) d.chunk_index = c.take<int32_t>(pairs);
-        if (out.speaker_index) d.speaker_index = c.take<int32_t>(pairs);
-        if (out.start_frame) d.start_frame = c.take<int32_t>(pairs);
-        if (out.end_frame) d.end_frame = c.take<int32_t>(pairs);
-        if (out.start_time) d.start_time = c.take<double>(pairs);
-        if (out.end_time) d.end_time = c.take<double>(pairs);
-        if (out.mask_sum) d.mask_sum = c.take<float>(pairs);
-        if (out.used_fallback) d.used_fallback = c.take<int32_t>(pairs);
-        if (out.reuse_of) d.reuse_of = c.take<int32_t>(pairs);
-        if (out.frame_weights) d.frame_weights = c.take<float>(pairs * frames);
-        if (out.model_weights) d.model_weights = c.take<float>(pairs * plan.weight_frames);
-    };
-    if (!on_device) {
-        if ((st = carve_arena(C.d_buf, host_layout)) != FA_OK) return st;
-        if ((st = to_device(weights_stage, speaker_weights, w_floats, s, d_weights)) != FA_OK) return st;
-    }
+    HostStaging H(!on_device, s);
+    PlanOutputs d;
+    const float *d_weights;
+    st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_weights = l.in(speaker_weights, w_floats);
+        d.chunk_index = l.out(out.chunk_index, pairs);
+        d.speaker_index = l.out(out.speaker_index, pairs);
+        d.start_frame = l.out(out.start_frame, pairs);
+        d.end_frame = l.out(out.end_frame, pairs);
+        d.start_time = l.out(out.start_time, pairs);
+        d.end_time = l.out(out.end_time, pairs);
+        d.mask_sum = l.out(out.mask_sum, pairs);
+        d.used_fallback = l.out(out.used_fallback, pairs);
+        d.reuse_of = l.out(out.reuse_of, pairs);
+        d.frame_weights = l.out(out.frame_weights, pairs * frames);
+        d.model_weights = l.out(out.model_weights, pairs * plan.weight_frames);
+    });
+    if (st != FA_OK) return st;
 
     EntryMeta *meta = nullptr;
     int *chunk_count = nullptr, *slot_of = nullptr, *tallies = nullptr;   // tallies: 4 counters, then the entry count
@@ -552,22 +529,9 @@ int embedding_plan(CallContext &C, bool on_device, const float *speaker_weights,
     FA_CUDA_TRY(cudaMemcpyAsync(host_tallies, tallies, sizeof(host_tallies), cudaMemcpyDeviceToHost, s));
     FA_CUDA_TRY(cudaStreamSynchronize(s));
     const size_t n = (size_t)host_tallies[4];
-    if (!on_device && n) {
-        auto back = [&](auto *host, const auto *dev, size_t per_entry) -> cudaError_t {
-            return host ? cudaMemcpyAsync(host, dev, n * per_entry * sizeof(*host), cudaMemcpyDeviceToHost, s) : cudaSuccess;
-        };
-        FA_CUDA_TRY(back(out.chunk_index, d.chunk_index, 1));
-        FA_CUDA_TRY(back(out.speaker_index, d.speaker_index, 1));
-        FA_CUDA_TRY(back(out.start_frame, d.start_frame, 1));
-        FA_CUDA_TRY(back(out.end_frame, d.end_frame, 1));
-        FA_CUDA_TRY(back(out.start_time, d.start_time, 1));
-        FA_CUDA_TRY(back(out.end_time, d.end_time, 1));
-        FA_CUDA_TRY(back(out.mask_sum, d.mask_sum, 1));
-        FA_CUDA_TRY(back(out.used_fallback, d.used_fallback, 1));
-        FA_CUDA_TRY(back(out.reuse_of, d.reuse_of, 1));
-        FA_CUDA_TRY(back(out.frame_weights, d.frame_weights, (size_t)frames));
-        FA_CUDA_TRY(back(out.model_weights, d.model_weights, (size_t)plan.weight_frames));
-        FA_CUDA_TRY(cudaStreamSynchronize(s));
+    if (n) {   // the emitted entries alone
+        FA_CUDA_TRY(H.back(n, pairs));
+        FA_CUDA_TRY(H.sync());
     }
     *entry_count = (int32_t)n;
     for (int k = 0; counters && k < 4; ++k) counters[k] = host_tallies[k];
@@ -577,18 +541,17 @@ int embedding_plan(CallContext &C, bool on_device, const float *speaker_weights,
 int weight_resample(CallContext &C, const float *rows, long long row_count, int in_len, int out_len, float *out) {
     const cudaStream_t s = C.stream;
     const long long total = row_count * out_len;
-    float *rows_stage = nullptr, *d_out = nullptr;
-    int st = carve_arena(C.d_buf, [&](Carver &c) {
-        rows_stage = c.take<float>((size_t)(row_count * in_len));
-        d_out = c.take<float>((size_t)total);
+    HostStaging H(true, s);
+    const float *d_rows;
+    float *d_out;
+    const int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+        d_rows = l.in(rows, (size_t)(row_count * in_len));
+        d_out = l.out(out, (size_t)total);
     });
     if (st != FA_OK) return st;
-    const float *d_rows = nullptr;
-    if ((st = to_device(rows_stage, rows, (size_t)(row_count * in_len), s, d_rows)) != FA_OK) return st;
     const unsigned grid = (unsigned)std::min<long long>((total + kThreads - 1) / kThreads, 65535);
     FA_CUDA_TRY(launch(weight_resample_kernel, dim3(grid), dim3(kThreads), 0, s, d_rows, total, in_len, out_len, d_out));
-    FA_CUDA_TRY(cudaMemcpyAsync(out, d_out, (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, s));
-    FA_CUDA_TRY(cudaStreamSynchronize(s));
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 

@@ -6,7 +6,7 @@
 // :421-613; the mask-similarity skip strategy :338-351,554-585,632-639), Extraction/WeightInterpolation.swift.
 //
 // Every call runs on the stream of the call context it is given and has finished when it returns; the host-buffer calls
-// stage their arrays in the context's workspace.  `on_device` says whether the large buffers (audio, windows, logits,
+// stage their arrays in the context's workspace `d_buf` (HostStaging, fa_common.cuh).  `on_device` says whether the large buffers (audio, windows, logits,
 // log-probabilities, weights, the per-entry outputs) are device pointers; the small ones (chunk offsets, chunk indices,
 // histogram, counts) are always host memory.
 #pragma once

@@ -93,7 +93,7 @@ class SortformerSet {
     DeviceBuffer<float> d_state;
     DeviceBuffer<long long> d_silence;
     UploadStage<> update_desc, input_desc;
-    DeviceBuffer<float> d_embs, d_preds, d_out, d_inputs;   // staging of the host-buffer variants
+    DeviceBuffer<> staging;   // the host-buffer variants' arrays (HostStaging, fa_common.cuh)
 };
 
 } // namespace sortformer

@@ -4,13 +4,13 @@
 // Every length of the state follows from coreFrames and the configuration, never from values, so the host mirrors the
 // cache and FIFO lengths, whether spkcachePreds exists, the chunk count, the FIFO ring's head and which of the two cache
 // buffers is current.  A push therefore checks and plans every session before anything runs, uploads one descriptor
-// per session and issues one kernel launch (sortformer_kernels.cu); the host variant adds its copies and one
-// synchronisation.  Only the silence mean and count depend on values, and they stay on the device.
+// per session and issues one kernel launch (sortformer_kernels.cu); the host variant stages its arrays in the set's one
+// staging buffer (HostStaging, fa_common.cuh), which adds their copies and one synchronisation.  Only the silence mean
+// and count depend on values, and they stay on the device.
 #include "sortformer_plan.h"
 
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 
 namespace fa {
 namespace sortformer {
@@ -172,13 +172,18 @@ int SortformerSet::update(int count, const int *sessions, const float *embs, int
     }
 
     // ---- buffers and descriptors
+    HostStaging H(!on_device, stream);
+    const float *e, *p;
+    float *c_out, *t_out;
     const size_t desc_bytes = (size_t)count * sizeof(UpdateJob);
     st = update_desc.reserve(std::max<size_t>(desc_bytes, 4096));
-    if (st == FA_OK && !on_device) {
-        st = d_embs.grow((size_t)std::max(emb_floats, 1LL) * sizeof(float));
-        if (st == FA_OK) st = d_preds.grow((size_t)std::max(pred_floats, 1LL) * sizeof(float));
-        if (st == FA_OK) st = d_out.grow((size_t)std::max(conf + tent, 1LL) * kSpeakers * sizeof(float));
-    }
+    if (st == FA_OK)
+        st = H.carve(staging, [&](HostStaging::Layout &l) {
+            e = l.in(embs, (size_t)emb_floats);
+            p = l.in(preds, (size_t)pred_floats);
+            c_out = l.out(confirmed, (size_t)(conf * kSpeakers));
+            t_out = l.out(tentative, (size_t)(tent * kSpeakers));
+        });
     if (st != FA_OK) return st;
     UpdateJob *hj = static_cast<UpdateJob *>(update_desc.host.data());
     long long co = 0, to = 0;
@@ -194,27 +199,12 @@ int SortformerSet::update(int count, const int *sessions, const float *embs, int
     }
 
     // ---- device work, on the handle's stream
-    const float *e = embs, *p = preds;
-    float *c_out = confirmed, *t_out = tentative;
-    if (!on_device) {
-        if (emb_floats) FA_CUDA_TRY(cudaMemcpyAsync(d_embs.data(), embs, emb_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
-        if (pred_floats)
-            FA_CUDA_TRY(cudaMemcpyAsync(d_preds.data(), preds, pred_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
-        e = d_embs.data();
-        p = d_preds.data();
-        c_out = d_out.data();
-        t_out = d_out.data() + conf * kSpeakers;
-    }
     st = update_desc.upload(desc_bytes, stream);
     if (st == FA_OK)
         st = launch_update(cfg, arena, static_cast<const UpdateJob *>(update_desc.device.data()), count, e, p,
                            d_state.data(), d_silence.data(), c_out, t_out, stream);
     if (st != FA_OK) return st;
-    if (!on_device) {
-        if (conf) FA_CUDA_TRY(cudaMemcpyAsync(confirmed, c_out, conf * kSpeakers * sizeof(float), cudaMemcpyDeviceToHost, stream));
-        if (tent) FA_CUDA_TRY(cudaMemcpyAsync(tentative, t_out, tent * kSpeakers * sizeof(float), cudaMemcpyDeviceToHost, stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(stream));
-    }
+    FA_CUDA_TRY(H.finish());
 
     table.commit(count, sessions, next.data());
     for (int i = 0; i < count; ++i) {
@@ -236,8 +226,14 @@ int SortformerSet::model_inputs(int count, const int *sessions, bool on_device, 
     const size_t desc_bytes = (size_t)count * sizeof(InputJob);
     const long long cache_floats = (long long)count * cfg.spkcache_len * kDims;
     const long long fifo_floats = (long long)count * cfg.fifo_len * kDims;
+    HostStaging H(!on_device, stream);
+    float *c_out, *f_out;
     st = input_desc.reserve(std::max<size_t>(desc_bytes, 4096));
-    if (st == FA_OK && !on_device) st = d_inputs.grow((size_t)(cache_floats + fifo_floats + 1) * sizeof(float));
+    if (st == FA_OK)
+        st = H.carve(staging, [&](HostStaging::Layout &l) {
+            c_out = l.out(spkcache, (size_t)cache_floats);
+            f_out = l.out(fifo, (size_t)fifo_floats);
+        });
     if (st != FA_OK) return st;
     InputJob *hj = static_cast<InputJob *>(input_desc.host.data());
     for (int i = 0; i < count; ++i) {
@@ -246,18 +242,12 @@ int SortformerSet::model_inputs(int count, const int *sessions, bool on_device, 
         if (spkcache_lengths) spkcache_lengths[i] = m.spk_len;
         if (fifo_lengths) fifo_lengths[i] = m.fifo_len;
     }
-    float *c_out = on_device ? spkcache : d_inputs.data();
-    float *f_out = on_device ? fifo : d_inputs.data() + cache_floats;
     st = input_desc.upload(desc_bytes, stream);
     if (st == FA_OK)
         st = launch_inputs(cfg, arena, static_cast<const InputJob *>(input_desc.device.data()), count, d_state.data(), c_out,
                            f_out, stream);
     if (st != FA_OK) return st;
-    if (!on_device) {
-        FA_CUDA_TRY(cudaMemcpyAsync(spkcache, c_out, cache_floats * sizeof(float), cudaMemcpyDeviceToHost, stream));
-        if (fifo_floats) FA_CUDA_TRY(cudaMemcpyAsync(fifo, f_out, fifo_floats * sizeof(float), cudaMemcpyDeviceToHost, stream));
-        FA_CUDA_TRY(cudaStreamSynchronize(stream));
-    }
+    FA_CUDA_TRY(H.finish());
     return FA_OK;
 }
 

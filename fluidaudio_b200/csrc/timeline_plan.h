@@ -84,9 +84,7 @@ class TimelineSet {
     DeviceBuffer<Segment> d_stage;
     DeviceBuffer<int> d_lane_counts;          // [2 x lanes]: finalized, tentative
     DeviceBuffer<long long> d_lane_offsets;   // [2 x lanes]
-    DeviceBuffer<long long> d_counts;         // host variant: [2 x count]
-    DeviceBuffer<float> d_in;                 // host variant: the packed rows
-    DeviceBuffer<Segment> d_out;              // host variant: both segment lists
+    DeviceBuffer<> staging;                   // the host variant's arrays (HostStaging, fa_common.cuh)
 };
 
 } // namespace timeline

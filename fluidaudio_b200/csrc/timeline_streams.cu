@@ -5,8 +5,9 @@
 // Every length follows from the row counts alone, never from values: the host mirrors each session's finalized cursor
 // and tentative row count, and bounds the segments a push can emit (segment_bound, timeline_core.cuh).  A push therefore
 // checks and plans every session before anything runs, uploads one descriptor per session and issues two launches
-// (timeline_kernels.cu); the host variant adds its copies and two synchronisations, one for the counts and one for
-// exactly the segments.  The scratches, which depend on values, stay on the device.
+// (timeline_kernels.cu); the host variant stages its arrays in the set's one staging buffer (HostStaging,
+// fa_common.cuh) and adds their copies and two synchronisations, one for the counts and one for exactly the segments.
+// The scratches, which depend on values, stay on the device.
 #include "timeline_plan.h"
 
 #include <algorithm>
@@ -103,18 +104,25 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
         return FA_INVALID_ARGUMENT;
     }
 
-    // ---- buffers and descriptors
+    // ---- buffers and descriptors (the host variant's counts are one scratch array: one copy reads them all back)
+    HostStaging H(!on_device, stream);
+    const float *f, *t;
+    Segment *f_out, *t_out;
+    long long *d_counts = nullptr;
     const int lanes = count * S;
     const size_t desc_bytes = (size_t)count * sizeof(PushJob);
     st = push_desc.reserve(std::max<size_t>(desc_bytes, 4096));
     if (st == FA_OK) st = d_stage.grow((size_t)std::max(stage, 1LL) * sizeof(Segment));
     if (st == FA_OK) st = d_lane_counts.grow((size_t)2 * lanes * sizeof(int));
     if (st == FA_OK) st = d_lane_offsets.grow((size_t)2 * lanes * sizeof(long long));
-    if (st == FA_OK && !on_device) {
-        st = d_in.grow((size_t)std::max((nsum + msum) * S, 1LL) * sizeof(float));
-        if (st == FA_OK) st = d_out.grow((size_t)std::max(fin_bound + ten_bound, 1LL) * sizeof(Segment));
-        if (st == FA_OK) st = d_counts.grow((size_t)2 * count * sizeof(long long));
-    }
+    if (st == FA_OK)
+        st = H.carve(staging, [&](HostStaging::Layout &l) {
+            f = l.in(fin, (size_t)(nsum * S));
+            t = l.in(ten, (size_t)(msum * S));
+            f_out = l.out(fin_out, (size_t)fin_bound);
+            t_out = l.out(ten_out, (size_t)ten_bound);
+            if (!on_device) d_counts = l.take<long long>(2 * (size_t)count);
+        });
     if (st != FA_OK) return st;
     PushJob *hj = static_cast<PushJob *>(push_desc.host.data());
     long long fo = 0, to = 0, so = 0;
@@ -127,21 +135,7 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
     }
 
     // ---- device work, on the handle's stream
-    const float *f = fin, *t = ten;
-    Segment *f_out = fin_out, *t_out = ten_out;
-    long long *f_cnt = fin_counts, *t_cnt = ten_counts;
-    if (!on_device) {
-        float *in = d_in.data();
-        if (nsum) FA_CUDA_TRY(cudaMemcpyAsync(in, fin, nsum * S * sizeof(float), cudaMemcpyHostToDevice, stream));
-        if (msum)
-            FA_CUDA_TRY(cudaMemcpyAsync(in + nsum * S, ten, msum * S * sizeof(float), cudaMemcpyHostToDevice, stream));
-        f = in;
-        t = in + nsum * S;
-        f_out = d_out.data();
-        t_out = d_out.data() + fin_bound;
-        f_cnt = d_counts.data();
-        t_cnt = d_counts.data() + count;
-    }
+    long long *f_cnt = on_device ? fin_counts : d_counts, *t_cnt = on_device ? ten_counts : d_counts + count;
     st = push_desc.upload(desc_bytes, stream);
     if (st == FA_OK) {
         const PushJob *jobs = static_cast<const PushJob *>(push_desc.device.data());
@@ -163,9 +157,9 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
             nf += fin_counts[i];
             nt += ten_counts[i];
         }
-        if (nf) FA_CUDA_TRY(cudaMemcpyAsync(fin_out, f_out, nf * sizeof(Segment), cudaMemcpyDeviceToHost, stream));
-        if (nt) FA_CUDA_TRY(cudaMemcpyAsync(ten_out, t_out, nt * sizeof(Segment), cudaMemcpyDeviceToHost, stream));
-        if (nf || nt) FA_CUDA_TRY(cudaStreamSynchronize(stream));
+        FA_CUDA_TRY(H.back(fin_out, f_out, (size_t)nf));
+        FA_CUDA_TRY(H.back(ten_out, t_out, (size_t)nt));
+        if (nf || nt) FA_CUDA_TRY(H.sync());
     }
     table.commit(count, sessions, next.data());
     return FA_OK;

@@ -112,4 +112,100 @@ coh.features(a[:1000], 3500)
 coh.compute(a[:1])
 CohereMelSpectrogram(CohereMelSpectrogram.Config(mag_power=1.5)).compute(a[:5000])
 sty.mel.compute_batch([b[:3], b[:30000]])
+# host-buffer staging: the prepare stage, live mel streams, Sortformer sessions and timelines, host and device variants
+# alternating on seeded inputs (outputs of the embedding plan partly null, with and without the skip strategy)
+import ctypes as C
+from fluidaudio_b200 import _lib
+from fluidaudio_b200.diarizer_timeline import SEGMENT, DiarizerTimelineConfig, DiarizerTimelines
+from fluidaudio_b200.mel import MelStreams
+from fluidaudio_b200.segmentation import (EmbeddingPlanConfig, OfflineEmbeddingPlanner, OfflineSegmentationProcessor,
+                                          WeightInterpolation)
+from fluidaudio_b200.sortformer import SortformerConfig, SortformerStreams
+
+
+keep = []   # device buffers live until the end: the device variants return with their work queued
+
+
+def dev(x=None, nbytes=0):
+    d = _lib.DeviceBuffer(nbytes if x is None else x.nbytes)
+    if x is not None:
+        d.upload(x)
+    keep.append(d)
+    return d
+
+
+rng = np.random.default_rng(21)
+speech = (rng.standard_normal(16000 * 25 + 311) * 0.1).astype(np.float32)
+segp, planner = OfflineSegmentationProcessor(), OfflineEmbeddingPlanner()
+_, offs = segp.windows(speech, 1, 3)
+segp.windows_device(dev(speech), speech.size, _lib.DeviceBuffer(3 * 160000 * 4), 1, 3)
+planner.fbank_windows(speech, offs)
+planner.fbank_windows_device(dev(speech), speech.size, offs, np.array([2, 0], np.int32), 2,
+                             _lib.DeviceBuffer(2 * 160000 * 4))
+logits, truth = synth.segmentation_logits(30.0, seed=4)
+seg = segp.decode(logits, truth["chunk_offsets"])
+segp.decode(logits, truth["chunk_offsets"], want_log_probs=False)
+c, f, k = logits.shape
+d_logits, d_w = dev(logits), _lib.DeviceBuffer(c * f * 3 * 4)
+segp.decode_device(d_logits, c, f, k, _lib.DeviceBuffer(logits.nbytes), d_w)
+segp.decode_device(d_logits, c, f, k, None, d_w)
+planner.plan(seg, truth["total_samples"])
+for skip in (None, 0.9):
+    cfg = EmbeddingPlanConfig(skip_threshold=skip)
+    pairs, wf = c * 3, cfg.weight_frames
+    d_out = {"chunk_index": _lib.DeviceBuffer(pairs * 4), "start_time": _lib.DeviceBuffer(pairs * 8),
+             "reuse_of": _lib.DeviceBuffer(pairs * 4), "model_weights": _lib.DeviceBuffer(pairs * wf * 4)}
+    OfflineEmbeddingPlanner(config=cfg).plan_device(dev(seg.speaker_weights), c, f, 3, seg.chunk_offsets,
+                                                    seg.frame_duration, truth["total_samples"], d_out)
+    ci, st, ro, mw = np.zeros(pairs, np.int32), np.zeros(pairs), np.zeros(pairs, np.int32), np.zeros((pairs, wf), np.float32)
+    n, counters = C.c_int32(), np.zeros(4, np.int64)
+    _lib.check(_lib.load().fa_embedding_plan(
+        _lib.ptr(seg.speaker_weights), c, f, 3, _lib.ptr(seg.chunk_offsets), c, float(seg.frame_duration),
+        int(truth["total_samples"]), C.byref(segp.config._c()), C.byref(cfg._c()), _lib.ptr(ci), None, None, None,
+        _lib.ptr(st), None, None, None, _lib.ptr(ro), None, _lib.ptr(mw), C.byref(n), counters.ctypes.data),
+        "fa_embedding_plan")
+WeightInterpolation.resample_2d(rng.random((5, 589), np.float32), 293)
+mel = AudioMelSpectrogram(n_mels=80)
+ms = MelStreams(mel)
+s1, s2 = ms.open(), ms.open()
+for i, n in enumerate((700, 2500, 0, 4001)):
+    if i % 2 == 0:
+        ms.push({s1: speech[i * 5000:i * 5000 + n], s2: speech[:n + 160]})
+    else:
+        offsets = np.array([0, n, 2 * n + 160], np.int64)
+        rows = ms.pending_frames(s1, n) + ms.pending_frames(s2, n + 160)
+        ms.push_device([s1, s2], dev(np.concatenate([speech[:n], speech[:n + 160]])), offsets,
+                       dev(nbytes=max(rows, 1) * 80 * 4))
+ms.push({s1: speech[:333]}, finish=[s1, s2])
+sf = SortformerStreams(SortformerConfig.preset("default"))
+ids = [sf.open() for _ in range(3)]
+conf_d, tent_d = _lib.DeviceBuffer(3 * 6 * 4 * 4), _lib.DeviceBuffer(16)
+sc_d, ff_d = _lib.DeviceBuffer(3 * 188 * 512 * 4), _lib.DeviceBuffer(3 * 40 * 512 * 4)
+for step in range(45):   # past the speaker cache's first compression
+    e = (rng.standard_normal((3, 6, 512)) * 0.5).astype(np.float32)
+    p = rng.random((3, 240, 4), np.float32)
+    if step % 2 == 0:
+        sf.update(ids, e, p, left_context=0, right_context=0)
+        sf.model_inputs(ids[:2])
+    else:
+        sf.update_device(ids, dev(e), 6, dev(p), 240, conf_d, tent_d, left_context=0, right_context=0)
+        sf.model_inputs_device(ids[1:], sc_d, ff_d)
+_lib.synchronize()
+tl = DiarizerTimelines(DiarizerTimelineConfig.sortformer_default(), max_tentative_rows=64)
+tids = [tl.open_session() for _ in range(2)]
+for step in range(4):
+    fin = [rng.random((r, 4), np.float32) for r in (40, 17)]
+    ten = [rng.random((r, 4), np.float32) for r in (8, 0)]
+    if step % 2 == 0:
+        tl.push(tids, fin, ten)
+    else:
+        fr, tr = [40, 17], [8, 0]
+        bf, bt = tl.segment_bound(fr, tr)
+        tl.push_device(tids, dev(np.concatenate(fin)), fr, dev(np.concatenate(ten)), tr,
+                       dev(nbytes=max(bf, 1) * SEGMENT.itemsize), dev(nbytes=max(bt, 1) * SEGMENT.itemsize), dev(nbytes=16),
+                       dev(nbytes=16))
+tl.finalize(tids)
+tl.reset(tids[:1])
+tl.push(tids, [rng.random((9, 4), np.float32)] * 2)
+_lib.synchronize()
 print("sanitize target done")
