@@ -4,12 +4,14 @@
 #include "assign_host.h"
 #include "kmeans_plan.h"
 #include "vbx_plan.h"
+#include "c_abi.h"
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
+#include <cstdio>
 #include <cstring>
-#include <string>
 #include <thread>
 #include <vector>
 
@@ -320,39 +322,30 @@ int cluster_batch(const float *emb, const double *rho, const int64_t *set_offset
     const int lanes = plan.lanes, worker_limit = plan.worker_limit;
     std::atomic<int> next{0};
     std::vector<int> status(lanes, FA_OK);
-    std::vector<std::string> messages(lanes);
-    // Each lane is a plain std::thread: nothing may escape it (an exception leaving a thread function is std::terminate,
-    // and the C ABI's exception guard only covers the calling thread), so the body reports every failure through status[].
+    std::vector<std::array<char, 512>> messages(lanes);   // a failed lane's error text, empty when it set none
+    // Each lane is a plain std::thread: nothing may escape it (an exception leaving a thread function is std::terminate),
+    // so run_guarded turns every failure, exceptions included, into status[] and the lane's own error text.
     auto run = [&](int lane) noexcept {
-        try {
+        const unsigned serial = error_serial();
+        status[lane] = run_guarded([&]() -> int {
             const cudaError_t e = cudaSetDevice(dev);
-            if (e != cudaSuccess) {
-                status[lane] = cuda_failure(e, "cudaSetDevice", __FILE__, __LINE__);
-            } else {
-                status[lane] = with_context(worker_limit, [&](CallContext &C) {
-                    for (;;) {
-                        const int m = next.fetch_add(1);
-                        if (m >= set_count) return (int)FA_OK;
-                        const int64_t a = set_offsets[m], b = set_offsets[m + 1];
-                        if (b == a) continue;   // not clustered: the caller zeroed its info
-                        const int st = cluster_pipeline(C, emb + (size_t)a * emb_dim, rho + (size_t)a * rho_dim,
-                                                        (size_t)(b - a), emb_dim, rho_dim, psi, cfg, labels + a, nullptr,
-                                                        nullptr, 0, infos ? infos + m : nullptr,
-                                                        chunk_index ? chunk_index + a : nullptr);
-                        if (st != FA_OK) return st;
-                    }
-                });
-            }
-            if (status[lane] != FA_OK) messages[lane] = fa::last_error();
-        } catch (const std::bad_alloc &) {
-            status[lane] = FA_ALLOCATION_FAILURE;
-            try { messages[lane] = "host allocation failed"; } catch (...) {}
-        } catch (const std::exception &ex) {
-            status[lane] = FA_RUNTIME_ERROR;
-            try { messages[lane] = std::string("exception: ") + ex.what(); } catch (...) {}
-        } catch (...) {
-            status[lane] = FA_UNKNOWN_ERROR;
-        }
+            if (e != cudaSuccess) return cuda_failure(e, "cudaSetDevice", __FILE__, __LINE__);
+            return with_context(worker_limit, [&](CallContext &C) {
+                for (;;) {
+                    const int m = next.fetch_add(1);
+                    if (m >= set_count) return (int)FA_OK;
+                    const int64_t a = set_offsets[m], b = set_offsets[m + 1];
+                    if (b == a) continue;   // not clustered: the caller zeroed its info
+                    const int st = cluster_pipeline(C, emb + (size_t)a * emb_dim, rho + (size_t)a * rho_dim,
+                                                    (size_t)(b - a), emb_dim, rho_dim, psi, cfg, labels + a, nullptr,
+                                                    nullptr, 0, infos ? infos + m : nullptr,
+                                                    chunk_index ? chunk_index + a : nullptr);
+                    if (st != FA_OK) return st;
+                }
+            });
+        });
+        if (status[lane] != FA_OK && error_serial() != serial)
+            std::snprintf(messages[lane].data(), messages[lane].size(), "%s", fa::last_error());
         if (status[lane] != FA_OK) next.store(set_count);   // the other lanes stop taking new sets
     };
     // Lane 0 runs on the calling thread.  Every thread that starts is joined below: nothing between its start and the
@@ -367,7 +360,7 @@ int cluster_batch(const float *emb, const double *rho, const int64_t *set_offset
     for (auto &t : threads) t.join();
     for (int l = 0; l < lanes; ++l)
         if (status[l] != FA_OK) {
-            fa::set_error("%s", messages[l].c_str());
+            if (messages[l][0]) fa::set_error("%s", messages[l].data());
             return status[l];
         }
     return FA_OK;

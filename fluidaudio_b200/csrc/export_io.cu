@@ -8,15 +8,13 @@
 //
 // Host code only (no kernels): a small recursive-descent reader for exactly this schema.  Numbers are converted with
 // strtof / strtod straight from the decimal text, so a float32 written in shortest form reads back bit-identically.
-#include "../../include/fluidaudio_b200.h"
-#include "fa_common.cuh"
+#include "c_abi.h"
 
 #include <cerrno>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <new>
 #include <string>
 #include <vector>
 
@@ -285,51 +283,42 @@ int parse(const char *path, std::vector<Entry> &entries) {
 
 } // namespace
 
-#define FA_API extern "C" __attribute__((visibility("default")))
-
-
 FA_API fa_status fa_export_shape(const char *path, size_t *count, size_t *emb_dim, size_t *rho_dim) {
-    try {
-        if (!path || !count || !emb_dim || !rho_dim) return (fa_status)FA_INVALID_ARGUMENT;
+    return fa::guard(__func__, [&]() -> int {
+        if (!path || !count || !emb_dim || !rho_dim) return FA_INVALID_ARGUMENT;
         std::vector<Entry> entries;
         const int st = parse(path, entries);
-        if (st != FA_OK) return (fa_status)st;
+        if (st != FA_OK) return st;
         *count = entries.size();
         *emb_dim = entries.empty() ? 0 : entries[0].emb.size();
         *rho_dim = entries.empty() ? 0 : entries[0].rho.size();
         for (const Entry &e : entries)
             if (e.emb.size() != *emb_dim || e.rho.size() != *rho_dim) {
                 fa::set_error("%s: entries have different embedding256 / rho128 lengths", path);
-                return (fa_status)FA_INVALID_ARGUMENT;
+                return FA_INVALID_ARGUMENT;
             }
-        return (fa_status)FA_OK;
-    } catch (const std::bad_alloc &) {
-        fa::set_error("host allocation failed");
-        return (fa_status)FA_ALLOCATION_FAILURE;
-    } catch (...) {
-        fa::set_error("unexpected exception in %s", "fa_export_shape");
-        return (fa_status)FA_UNKNOWN_ERROR;
-    }
+        return FA_OK;
+    });
 }
 
 FA_API fa_status fa_export_read(const char *path, size_t count, size_t emb_dim, size_t rho_dim, int32_t *chunk_index,
                          int32_t *speaker_index, int32_t *start_frame, int32_t *end_frame, double *start_time,
                          double *end_time, float *emb, double *rho, int32_t *cluster) {
-    try {
-        if (!path) return (fa_status)FA_INVALID_ARGUMENT;
+    return fa::guard(__func__, [&]() -> int {
+        if (!path) return FA_INVALID_ARGUMENT;
         std::vector<Entry> entries;
         const int st = parse(path, entries);
-        if (st != FA_OK) return (fa_status)st;
+        if (st != FA_OK) return st;
         if (entries.size() != count) {
             fa::set_error("%s holds %zu entries, caller expected %zu", path, entries.size(), count);
-            return (fa_status)FA_INVALID_ARGUMENT;
+            return FA_INVALID_ARGUMENT;
         }
         for (size_t i = 0; i < count; ++i) {
             const Entry &e = entries[i];
             if (e.emb.size() != emb_dim || e.rho.size() != rho_dim) {
                 fa::set_error("%s: entry %zu has %zu / %zu values, expected %zu / %zu", path, i, e.emb.size(), e.rho.size(),
                               emb_dim, rho_dim);
-                return (fa_status)FA_INVALID_ARGUMENT;
+                return FA_INVALID_ARGUMENT;
             }
             if (chunk_index) chunk_index[i] = (int32_t)e.chunk;
             if (speaker_index) speaker_index[i] = (int32_t)e.speaker;
@@ -341,26 +330,20 @@ FA_API fa_status fa_export_read(const char *path, size_t count, size_t emb_dim, 
             if (emb) std::memcpy(emb + i * emb_dim, e.emb.data(), sizeof(float) * emb_dim);
             if (rho) std::memcpy(rho + i * rho_dim, e.rho.data(), sizeof(double) * rho_dim);
         }
-        return (fa_status)FA_OK;
-    } catch (const std::bad_alloc &) {
-        fa::set_error("host allocation failed");
-        return (fa_status)FA_ALLOCATION_FAILURE;
-    } catch (...) {
-        fa::set_error("unexpected exception in %s", "fa_export_read");
-        return (fa_status)FA_UNKNOWN_ERROR;
-    }
+        return FA_OK;
+    });
 }
 
 FA_API fa_status fa_export_write(const char *path, size_t count, size_t emb_dim, size_t rho_dim, const int32_t *chunk_index,
                           const int32_t *speaker_index, const int32_t *start_frame, const int32_t *end_frame,
                           const double *start_time, const double *end_time, const float *emb, const double *rho,
                           const int32_t *cluster) {
-    try {
-        if (!path || (count && (!emb || !rho))) return (fa_status)FA_INVALID_ARGUMENT;
+    return fa::guard(__func__, [&]() -> int {
+        if (!path || (count && (!emb || !rho))) return FA_INVALID_ARGUMENT;
         FILE *f = std::fopen(path, "wb");
         if (!f) {
             fa::set_error("cannot create %s: %s", path, std::strerror(errno));
-            return (fa_status)FA_INVALID_ARGUMENT;
+            return FA_INVALID_ARGUMENT;
         }
         std::fputc('[', f);
         for (size_t i = 0; i < count; ++i) {
@@ -379,15 +362,8 @@ FA_API fa_status fa_export_write(const char *path, size_t count, size_t emb_dim,
         const bool bad = std::ferror(f) != 0;
         if (std::fclose(f) != 0 || bad) {
             fa::set_error("write error on %s", path);
-            return (fa_status)FA_RUNTIME_ERROR;
+            return FA_RUNTIME_ERROR;
         }
-        return (fa_status)FA_OK;
-    } catch (const std::bad_alloc &) {
-        fa::set_error("host allocation failed");
-        return (fa_status)FA_ALLOCATION_FAILURE;
-    } catch (...) {
-        fa::set_error("unexpected exception in %s", "fa_export_write");
-        return (fa_status)FA_UNKNOWN_ERROR;
-    }
+        return FA_OK;
+    });
 }
-

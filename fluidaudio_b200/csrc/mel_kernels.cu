@@ -727,9 +727,9 @@ int MelPlan::launch_clip(const float *d_in, long long n, long long T, int layout
     return launch(units.device.data(), units.host.data(), 1, false, d_in, d_out_buf, FA_MEL_PAD_CENTER, layout, stream);
 }
 
-int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, int count, const float *last, int mode,
-                                  int layout, float *d_out_buf, const long long *out_offsets, long long *mel_lengths,
-                                  long long *num_frames, cudaStream_t stream) {
+int MelPlan::compute_batch_device(const float *d_in, const int64_t *offsets, int count, const float *last, int mode,
+                                  int layout, float *d_out_buf, const int64_t *out_offsets, int64_t *mel_lengths,
+                                  int64_t *num_frames, cudaStream_t stream) {
     int st = units.reserve(unit_bytes(count));
     if (st != FA_OK) return st;
     MelUnit *h_units = units.host.data();
@@ -737,8 +737,9 @@ int MelPlan::compute_batch_device(const float *d_in, const long long *offsets, i
     for (int i = 0; i < count; ++i) {
         const long long n = offsets[i + 1] - offsets[i];
         long long T, Tp;
-        clip_shape(*this, n, mode, -1, kUnchecked, T, Tp, mel_lengths ? mel_lengths + i : nullptr,
-                   num_frames ? num_frames + i : nullptr);
+        clip_shape(*this, n, mode, -1, kUnchecked, T, Tp, nullptr, nullptr);
+        if (mel_lengths) mel_lengths[i] = T;
+        if (num_frames) num_frames[i] = Tp;
         if (T == 0) {
             if (Tp) FA_CUDA_TRY(cudaMemsetAsync(d_out_buf + out_offsets[i], 0, cfg.n_mels * sizeof(float), stream));
             continue;

@@ -237,9 +237,9 @@ int MelPlan::compute_host(const void *pcm, long long frames, const resample::Aud
 }
 
 // Batch of clips, host buffers: clips are grouped so that copies and kernels of successive groups overlap.
-int MelPlan::compute_batch_host(const float *audio, const long long *offsets, int count, const float *last, int mode,
-                                int layout, float *out, const long long *out_offsets, long long *mel_lengths,
-                                long long *num_frames) {
+int MelPlan::compute_batch_host(const float *audio, const int64_t *offsets, int count, const float *last, int mode,
+                                int layout, float *out, const int64_t *out_offsets, int64_t *mel_lengths,
+                                int64_t *num_frames) {
     if (count <= 0) return FA_OK;
     // device-side packing: clip i starts at a 4-float aligned offset so that every tile can use the TMA path
     // When every clip already starts at a multiple of four floats in the caller's buffer, the device copy keeps the
@@ -256,8 +256,9 @@ int MelPlan::compute_batch_host(const float *audio, const long long *offsets, in
         doff[i] = same_layout ? offsets[i] - offsets[0] : a;
         a = same_layout ? ceil_to(offsets[i + 1] - offsets[0], 4) + 4 : a + ceil_to(n, 4) + 4;
         dout[i] = o;
-        clip_shape(*this, n, mode, -1, kUnchecked, Ts[i], Tps[i], mel_lengths ? mel_lengths + i : nullptr,
-                   num_frames ? num_frames + i : nullptr);
+        clip_shape(*this, n, mode, -1, kUnchecked, Ts[i], Tps[i], nullptr, nullptr);
+        if (mel_lengths) mel_lengths[i] = Ts[i];
+        if (num_frames) num_frames[i] = Tps[i];
         o += std::max<long long>(Tps[i], 1) * cfg.n_mels;   // an empty clip returns one zero row, in every mode
     }
     doff[count] = a;

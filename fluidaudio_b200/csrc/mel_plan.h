@@ -122,12 +122,12 @@ struct MelPlan {
                      long long expected, int layout, float *out, long long out_len, long long *mel_length,
                      long long *num_frames, long long *resampled);
     int ensure_resampler(double in_rate, double out_rate);
-    int compute_batch_host(const float *audio, const long long *offsets, int count, const float *last, int mode,
-                           int layout, float *out, const long long *out_offsets, long long *mel_lengths,
-                           long long *num_frames);
-    int compute_batch_device(const float *d_in, const long long *offsets, int count, const float *last, int mode,
-                             int layout, float *d_out_buf, const long long *out_offsets, long long *mel_lengths,
-                             long long *num_frames, cudaStream_t stream);
+    int compute_batch_host(const float *audio, const int64_t *offsets, int count, const float *last, int mode,
+                           int layout, float *out, const int64_t *out_offsets, int64_t *mel_lengths,
+                           int64_t *num_frames);
+    int compute_batch_device(const float *d_in, const int64_t *offsets, int count, const float *last, int mode,
+                             int layout, float *d_out_buf, const int64_t *out_offsets, int64_t *mel_lengths,
+                             int64_t *num_frames, cudaStream_t stream);
     // One .center launch of exactly T frames of one n-sample clip at d_in, whatever n (an empty clip reads zeros): the
     // torch-style frontends count their frames by their own rules (mel_adapters.cu).  last = 0.
     int launch_clip(const float *d_in, long long n, long long T, int layout, float *d_out_buf, cudaStream_t stream);
@@ -177,8 +177,8 @@ struct MelStreamSet {
     // Session sessions[i] receives audio[offsets[i] .. offsets[i+1]); its frames[i] rows start at row sum_{j<i} frames[j]
     // of out.  device: audio and out are HBM and the call is asynchronous on the compute stream; otherwise both are host
     // buffers, the samples travel in one copy, the rows in one copy, and the call returns after one synchronisation.
-    int push(MelPlan &p, int count, const int *sessions, const float *audio, const long long *offsets, const int *finish,
-             bool device, float *out, long long out_len, long long *frames);
+    int push(MelPlan &p, int count, const int *sessions, const float *audio, const int64_t *offsets, const int *finish,
+             bool device, float *out, long long out_len, int64_t *frames);
 };
 
 // mel_adapters.cu: device epilogues for the callers directly behind AudioMelSpectrogram (host buffers in and out)

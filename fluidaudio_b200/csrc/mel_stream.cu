@@ -136,8 +136,8 @@ long long MelStreamSet::frames(const MelPlan &p, int session, long long n, bool 
     return first + second;
 }
 
-int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *audio, const long long *offsets,
-                       const int *finish, bool device, float *out, long long out_len, long long *frames_out) {
+int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *audio, const int64_t *offsets,
+                       const int *finish, bool device, float *out, long long out_len, int64_t *frames_out) {
     const MelConfig &c = p.cfg;
     const int M = c.n_mels, hop = c.hop_length, half = c.n_fft / 2;
     if (count < 0 || (count > 0 && (!sessions || !offsets || !frames_out))) {
@@ -146,14 +146,15 @@ int MelStreamSet::push(MelPlan &p, int count, const int *sessions, const float *
     }
     if (count == 0) return FA_OK;
     if (offsets[0] < 0) {
-        fa::set_error("mel stream push: offsets[0] is negative (%lld)", offsets[0]);
+        fa::set_error("mel stream push: offsets[0] is negative (%lld)", (long long)offsets[0]);
         return FA_INVALID_ARGUMENT;
     }
     int st = table.check(count, sessions, "mel stream push");
     if (st != FA_OK) return st;
     for (int i = 0; i < count; ++i)
         if (offsets[i + 1] < offsets[i]) {
-            fa::set_error("mel stream push: offsets decrease at %d (%lld > %lld)", i, offsets[i], offsets[i + 1]);
+            fa::set_error("mel stream push: offsets decrease at %d (%lld > %lld)", i, (long long)offsets[i],
+                          (long long)offsets[i + 1]);
             return FA_INVALID_ARGUMENT;
         }
     const long long total_new = offsets[count] - offsets[0];

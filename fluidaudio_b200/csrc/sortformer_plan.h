@@ -79,8 +79,8 @@ class SortformerSet {
     int close(int session);
     int update(int count, const int *sessions, const float *embs, int emb_rows, const float *preds, int pred_rows,
                const int *emb_lengths, const int *left, const int *right, bool device, float *confirmed,
-               long long confirmed_len, float *tentative, long long tentative_len, long long *confirmed_rows,
-               long long *tentative_rows);
+               long long confirmed_len, float *tentative, long long tentative_len, int64_t *confirmed_rows,
+               int64_t *tentative_rows);
     int model_inputs(int count, const int *sessions, bool device, float *spkcache, float *fifo, int *spkcache_lengths,
                      int *fifo_lengths);
     int state(int session, SessionInfo *info, float *spkcache, float *spkcache_preds, float *fifo, float *fifo_preds,

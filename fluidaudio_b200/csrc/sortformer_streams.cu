@@ -128,7 +128,7 @@ int SortformerSet::close(int session) { return table.close(session, "sortformer"
 int SortformerSet::update(int count, const int *sessions, const float *embs, int emb_rows, const float *preds,
                           int pred_rows, const int *emb_lengths, const int *left, const int *right, bool on_device,
                           float *confirmed, long long confirmed_len, float *tentative, long long tentative_len,
-                          long long *confirmed_rows, long long *tentative_rows) {
+                          int64_t *confirmed_rows, int64_t *tentative_rows) {
     if (count < 0 || emb_rows < 0 || pred_rows < 0 ||
         (count > 0 && (!sessions || !emb_lengths || !confirmed_rows || !tentative_rows))) {
         fa::set_error("sortformer update: count, emb_rows and pred_rows must be >= 0; sessions, emb_lengths and the row "

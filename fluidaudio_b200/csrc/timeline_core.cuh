@@ -15,6 +15,7 @@
 // would overflow them (Swift traps there).  `.logits` is log(c / (1 - c)) with f_log = (float)log((double)x) (DESIGN §4.8).
 #pragma once
 
+#include "../../include/fluidaudio_b200.h"
 #include "fa_common.cuh"
 #include "fa_float.cuh"
 
@@ -45,12 +46,8 @@ struct Scratch {
     int speaking, has_segment;
 };
 
-// The layout of fa_diarizer_timeline_segment.
-struct Segment {
-    long long start_frame, end_frame;
-    float activity;
-    int speaker;
-};
+// A segment as the C ABI returns it: {start_frame, end_frame, activity, speaker}.
+using Segment = fa_diarizer_timeline_segment;
 
 // A scratch in HBM stores its three frames XOR 2^63, so that all-zero bytes are a fresh scratch: open, reset and
 // clearing one speaker are memsets.

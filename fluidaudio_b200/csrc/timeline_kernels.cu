@@ -44,7 +44,7 @@ __global__ void __launch_bounds__(kWarps * 32)
 timeline_scan_kernel(Params c, Layout l, const PushJob *__restrict__ jobs, int count, const float *__restrict__ fin,
                      const float *__restrict__ ten, StoredScratch *__restrict__ scratch, float *__restrict__ rows,
                      Segment *__restrict__ stage, int *__restrict__ lane_counts, int lanes,
-                     long long *__restrict__ fin_counts, long long *__restrict__ ten_counts) {
+                     int64_t *__restrict__ fin_counts, int64_t *__restrict__ ten_counts) {
     __shared__ float tiles[kWarps][kTile * 32];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int i = blockIdx.x * kWarps + warp;
@@ -177,8 +177,8 @@ __global__ void timeline_finalize_kernel(Layout l, const FinalizeJob *__restrict
 } // namespace
 
 int launch_push(const Config &c, const Layout &l, const PushJob *d_jobs, int count, const float *fin, const float *ten,
-                StoredScratch *scratch, float *rows, Segment *stage, int *lane_counts, long long *fin_counts,
-                long long *ten_counts, cudaStream_t s) {
+                StoredScratch *scratch, float *rows, Segment *stage, int *lane_counts, int64_t *fin_counts,
+                int64_t *ten_counts, cudaStream_t s) {
     const int blocks = (count + kWarps - 1) / kWarps;
     FA_CUDA_TRY(launch(timeline_scan_kernel, dim3(blocks), dim3(kWarps * 32), 0, s, c.params(), l, d_jobs, count, fin, ten,
                        scratch, rows, stage, lane_counts, count * l.speakers, fin_counts, ten_counts));

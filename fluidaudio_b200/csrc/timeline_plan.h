@@ -49,8 +49,8 @@ struct Layout {
 };
 
 int launch_push(const Config &c, const Layout &l, const PushJob *d_jobs, int count, const float *fin, const float *ten,
-                StoredScratch *scratch, float *rows, Segment *stage, int *lane_counts, long long *fin_counts,
-                long long *ten_counts, cudaStream_t s);
+                StoredScratch *scratch, float *rows, Segment *stage, int *lane_counts, int64_t *fin_counts,
+                int64_t *ten_counts, cudaStream_t s);
 int launch_pack(const Layout &l, int lanes, const PushJob *d_jobs, const Segment *stage, const int *lane_counts,
                 long long *lane_offsets, Segment *fin_out, Segment *ten_out, cudaStream_t s);
 int launch_finalize(const Layout &l, const FinalizeJob *d_jobs, int count, float *rows, cudaStream_t s);
@@ -66,9 +66,9 @@ class TimelineSet {
     int init(const Config &c, int max_tentative_rows);
     int open(int *session);
     int close(int session);
-    int push(int count, const int *sessions, const float *fin, const long long *fin_rows, const float *ten,
-             const long long *ten_rows, bool on_device, Segment *fin_out, long long fin_cap, Segment *ten_out,
-             long long ten_cap, long long *fin_counts, long long *ten_counts);
+    int push(int count, const int *sessions, const float *fin, const int64_t *fin_rows, const float *ten,
+             const int64_t *ten_rows, bool on_device, Segment *fin_out, long long fin_cap, Segment *ten_out,
+             long long ten_cap, int64_t *fin_counts, int64_t *ten_counts);
     int finalize(int count, const int *sessions);
     int reset(int count, const int *sessions);
     int clear_speaker(int session, int speaker);

@@ -67,9 +67,9 @@ int TimelineSet::open(int *session) {
 
 int TimelineSet::close(int session) { return table.close(session, "diarizer timeline"); }
 
-int TimelineSet::push(int count, const int *sessions, const float *fin, const long long *fin_rows, const float *ten,
-                      const long long *ten_rows, bool on_device, Segment *fin_out, long long fin_cap, Segment *ten_out,
-                      long long ten_cap, long long *fin_counts, long long *ten_counts) {
+int TimelineSet::push(int count, const int *sessions, const float *fin, const int64_t *fin_rows, const float *ten,
+                      const int64_t *ten_rows, bool on_device, Segment *fin_out, long long fin_cap, Segment *ten_out,
+                      long long ten_cap, int64_t *fin_counts, int64_t *ten_counts) {
     if (count < 0 || (count > 0 && (!sessions || !fin_rows || !ten_rows || !fin_counts || !ten_counts))) {
         fa::set_error("diarizer timeline push: count must be >= 0; sessions, row counts and counts non-null");
         return FA_INVALID_ARGUMENT;
@@ -108,7 +108,7 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
     HostStaging H(!on_device, stream);
     const float *f, *t;
     Segment *f_out, *t_out;
-    long long *d_counts = nullptr;
+    int64_t *d_counts = nullptr;
     const int lanes = count * S;
     const size_t desc_bytes = (size_t)count * sizeof(PushJob);
     st = push_desc.reserve(std::max<size_t>(desc_bytes, 4096));
@@ -121,7 +121,7 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
             t = l.in(ten, (size_t)(msum * S));
             f_out = l.out(fin_out, (size_t)fin_bound);
             t_out = l.out(ten_out, (size_t)ten_bound);
-            if (!on_device) d_counts = l.take<long long>(2 * (size_t)count);
+            if (!on_device) d_counts = l.take<int64_t>(2 * (size_t)count);
         });
     if (st != FA_OK) return st;
     PushJob *hj = static_cast<PushJob *>(push_desc.host.data());
@@ -135,7 +135,7 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
     }
 
     // ---- device work, on the handle's stream
-    long long *f_cnt = on_device ? fin_counts : d_counts, *t_cnt = on_device ? ten_counts : d_counts + count;
+    int64_t *f_cnt = on_device ? fin_counts : d_counts, *t_cnt = on_device ? ten_counts : d_counts + count;
     st = push_desc.upload(desc_bytes, stream);
     if (st == FA_OK) {
         const PushJob *jobs = static_cast<const PushJob *>(push_desc.device.data());
@@ -147,11 +147,11 @@ int TimelineSet::push(int count, const int *sessions, const float *fin, const lo
     }
     if (st != FA_OK) return st;
     if (!on_device) {
-        std::vector<long long> counts(2 * (size_t)count);
-        FA_CUDA_TRY(cudaMemcpyAsync(counts.data(), f_cnt, counts.size() * sizeof(long long), cudaMemcpyDeviceToHost, stream));
+        std::vector<int64_t> counts(2 * (size_t)count);
+        FA_CUDA_TRY(cudaMemcpyAsync(counts.data(), f_cnt, counts.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, stream));
         FA_CUDA_TRY(cudaStreamSynchronize(stream));
-        std::memcpy(fin_counts, counts.data(), (size_t)count * sizeof(long long));
-        std::memcpy(ten_counts, counts.data() + count, (size_t)count * sizeof(long long));
+        std::memcpy(fin_counts, counts.data(), (size_t)count * sizeof(int64_t));
+        std::memcpy(ten_counts, counts.data() + count, (size_t)count * sizeof(int64_t));
         long long nf = 0, nt = 0;
         for (int i = 0; i < count; ++i) {
             nf += fin_counts[i];

@@ -59,7 +59,9 @@ typedef enum {
 
 /* ---- runtime ------------------------------------------------------------------------------------------- */
 const char *fa_version(void);
-const char *fa_last_error(void);            /* thread-local text of the last failure */
+/* Thread-local text of the last failure.  After any call that fails (a status other than FA_STATUS_OK, or -1 from a
+ * counting call), the text describes that call's failure; a call that succeeds leaves the text unchanged. */
+const char *fa_last_error(void);
 int32_t fa_device_count(void);              /* sm_90a devices visible */
 fa_status fa_set_device(int32_t ordinal);   /* binds the calling thread; one process per GPU is the intended use */
 fa_status fa_device_synchronize(void);
