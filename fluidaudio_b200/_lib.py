@@ -1,4 +1,4 @@
-"""ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h``).
+"""ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h`` and ``include/fluidaudio_b200_lseend.h``).
 
 The library is the product: it is built in-tree by ``__graft_entry__.build()`` / ``make -C fluidaudio_b200/csrc``.
 There is no Python or CPU fallback — if the shared object is missing, or no sm_90a device is visible, every
@@ -111,6 +111,23 @@ class TimelineSessionInfo(C.Structure):
     _fields_ = [("finalized_frames", C.c_int64), ("stored_frames", C.c_int64), ("tentative_frames", C.c_int64)]
 
 
+class LSEENDStreamConfig(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("n_mels", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32),
+                ("context_size", C.c_int32), ("subsampling", C.c_int32), ("chunk_size", C.c_int32),
+                ("conv_delay", C.c_int32), ("precision", C.c_int32)]
+
+
+class LSEENDStreamSizes(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("n_fft", "mel_frames", "chunk_mels", "mel_context", "chunk_samples",
+                                         "audio_left_context", "audio_context", "flush_samples", "mask_length",
+                                         "audio_capacity")]
+
+
+class LSEENDSessionInfo(C.Structure):
+    _fields_ = [("audio_samples", C.c_int64), ("mel_rows", C.c_int64), ("cmn_count", C.c_int64),
+                ("decoder_mask_end", C.c_int32), ("has_snapshot", C.c_int32)]
+
+
 # fa_diarizer_timeline_segment as a numpy record
 TIMELINE_SEGMENT = np.dtype([("start_frame", np.int64), ("end_frame", np.int64), ("activity", np.float32),
                              ("speaker", np.int32)])
@@ -147,6 +164,14 @@ EXPORTED_SYMBOLS = [
     "fa_diarizer_timeline_push_device", "fa_diarizer_timeline_finalize", "fa_diarizer_timeline_reset",
     "fa_diarizer_timeline_clear_speaker", "fa_diarizer_timeline_session_state",
     "fastcluster_compute_centroid_linkage",
+]
+
+# every symbol include/fluidaudio_b200_lseend.h declares (the LS-EEND feature streams)
+LSEEND_SYMBOLS = [
+    "fa_lseend_stream_resolve", "fa_lseend_stream_create", "fa_lseend_stream_destroy", "fa_lseend_stream_open",
+    "fa_lseend_stream_close", "fa_lseend_stream_chunks", "fa_lseend_stream_push", "fa_lseend_stream_push_device",
+    "fa_lseend_stream_snapshot", "fa_lseend_stream_rollback", "fa_lseend_stream_reset",
+    "fa_lseend_stream_session_state",
 ]
 
 _lib = None
@@ -293,6 +318,20 @@ def load():
     L.fa_diarizer_timeline_clear_speaker.argtypes = [vp, i32, i32]
     L.fa_diarizer_timeline_session_state.argtypes = [vp, i32, C.POINTER(TimelineSessionInfo), vp, vp,
                                                      C.POINTER(TimelineScratch)]
+    LC = C.POINTER(LSEENDStreamConfig)
+    L.fa_lseend_stream_resolve.argtypes = [LC, C.POINTER(LSEENDStreamSizes)]
+    L.fa_lseend_stream_create.argtypes = [LC, C.POINTER(vp)]
+    L.fa_lseend_stream_destroy.argtypes = [vp]
+    L.fa_lseend_stream_destroy.restype = None
+    L.fa_lseend_stream_open.argtypes = [vp, C.POINTER(i32)]
+    L.fa_lseend_stream_close.argtypes = [vp, i32]
+    L.fa_lseend_stream_chunks.argtypes = [vp, i32, i64, i32]
+    L.fa_lseend_stream_chunks.restype = i64
+    L.fa_lseend_stream_push.argtypes = [vp, i32, vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, vp]
+    L.fa_lseend_stream_push_device.argtypes = L.fa_lseend_stream_push.argtypes
+    for name in ("fa_lseend_stream_snapshot", "fa_lseend_stream_rollback", "fa_lseend_stream_reset"):
+        getattr(L, name).argtypes = [vp, i32, vp]
+    L.fa_lseend_stream_session_state.argtypes = [vp, i32, C.POINTER(LSEENDSessionInfo), vp, vp, vp]
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

@@ -5,6 +5,7 @@
 #include "../../include/fluidaudio_b200.h"
 #include "fa_common.cuh"
 
+#include <cstdint>
 #include <exception>
 #include <new>
 
@@ -16,6 +17,10 @@ namespace fa {
 unsigned error_serial();
 // "FA_STATUS_INVALID_ARGUMENT" and so on.
 const char *status_name(int status);
+// FA_OK when an sm_90a device is visible, else FA_NO_DEVICE with error text (entry points that create a handle).
+int require_device();
+// A caller's buffer capacity as the library's signed lengths: one of 2^63 elements or more is as good as unlimited.
+inline long long capacity(size_t n) { return n > (size_t)INT64_MAX ? INT64_MAX : (long long)n; }
 
 // Runs `body` (returning an int status) and turns any exception it throws into a status with error text.  It throws
 // nothing, so a thread of its own can run it (cluster_batch's lanes do).

@@ -86,7 +86,7 @@ static int usable_device_count() {
     return ok;
 }
 
-static int require_device() {
+int require_device() {
     static std::atomic<int> cached{-1};
     int c = cached.load();
     if (c < 0) {
@@ -99,9 +99,6 @@ static int require_device() {
     }
     return FA_OK;
 }
-
-// A caller's buffer capacity as the library's signed lengths: one of 2^63 elements or more is as good as unlimited.
-static long long capacity(size_t n) { return (long long)std::min<size_t>(n, INT64_MAX); }
 
 // timer state for fa_timer_*, per thread
 static thread_local Event t_ev[2];

@@ -14,6 +14,7 @@
 // frames), the point is fusion with the producer, not throughput.
 #include "call_context.h"
 #include "fa_common.cuh"
+#include "lseend/lseend_plan.h"
 #include "mel_plan.h"
 
 #include <algorithm>
@@ -93,14 +94,7 @@ int normalize_per_feature_host(CallContext &C, float *x, long long T, int M, lon
 __global__ void lseend_scale_cmn_kernel(float *x, long long T, int M, float *mean_io, long long count0, float scale) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= M) return;
-    float mean = mean_io[m];
-    for (long long t = 0; t < T; ++t) {
-        const float alpha = __fdiv_rn(1.0f, (float)(count0 + t + 1));
-        const float v = __fmul_rn(x[t * M + m], scale);
-        mean = __fadd_rn(mean, __fmul_rn(alpha, __fsub_rn(v, mean)));
-        x[t * M + m] = __fsub_rn(v, mean);
-    }
-    mean_io[m] = mean;
+    mean_io[m] = lseend::scale_cmn_column(x, T, M, m, mean_io[m], count0, scale);
 }
 
 // Both adapters return exactly T rows and size their staging for T; a handle with pad_to > 1 would have the mel kernel
