@@ -1,4 +1,5 @@
-"""ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h`` and ``include/fluidaudio_b200_lseend.h``).
+"""ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h``,
+``include/fluidaudio_b200_lseend.h`` and ``include/fluidaudio_b200_ctc.h``).
 
 The library is the product: it is built in-tree by ``__graft_entry__.build()`` / ``make -C fluidaudio_b200/csrc``.
 There is no Python or CPU fallback — if the shared object is missing, or no sm_90a device is visible, every
@@ -128,6 +129,15 @@ class LSEENDSessionInfo(C.Structure):
                 ("decoder_mask_end", C.c_int32), ("has_snapshot", C.c_int32)]
 
 
+class CtcDetection(C.Structure):
+    _fields_ = [("clip", C.c_int32), ("term", C.c_int32), ("score", C.c_float), ("start_frame", C.c_int32),
+                ("end_frame", C.c_int32)]
+
+
+# fa_ctc_detection as a numpy record
+CTC_DETECTION = np.dtype([("clip", np.int32), ("term", np.int32), ("score", np.float32), ("start_frame", np.int32),
+                          ("end_frame", np.int32)])
+
 # fa_diarizer_timeline_segment as a numpy record
 TIMELINE_SEGMENT = np.dtype([("start_frame", np.int64), ("end_frame", np.int64), ("activity", np.float32),
                              ("speaker", np.int32)])
@@ -172,6 +182,13 @@ LSEEND_SYMBOLS = [
     "fa_lseend_stream_close", "fa_lseend_stream_chunks", "fa_lseend_stream_push", "fa_lseend_stream_push_device",
     "fa_lseend_stream_snapshot", "fa_lseend_stream_rollback", "fa_lseend_stream_reset",
     "fa_lseend_stream_session_state",
+]
+
+# every symbol include/fluidaudio_b200_ctc.h declares (CTC keyword spotting)
+CTC_SYMBOLS = [
+    "fa_ctc_log_softmax", "fa_ctc_log_softmax_device", "fa_ctc_merge_chunks", "fa_ctc_merge_chunks_device",
+    "fa_ctc_spotter_create", "fa_ctc_spotter_destroy", "fa_ctc_spot", "fa_ctc_spot_device", "fa_ctc_spot_constrained",
+    "fa_ctc_spot_constrained_device",
 ]
 
 _lib = None
@@ -332,6 +349,17 @@ def load():
     for name in ("fa_lseend_stream_snapshot", "fa_lseend_stream_rollback", "fa_lseend_stream_reset"):
         getattr(L, name).argtypes = [vp, i32, vp]
     L.fa_lseend_stream_session_state.argtypes = [vp, i32, C.POINTER(LSEENDSessionInfo), vp, vp, vp]
+    L.fa_ctc_log_softmax.argtypes = [vp, i32, i32, i32, f32, f32, i32, vp]
+    L.fa_ctc_log_softmax_device.argtypes = L.fa_ctc_log_softmax.argtypes
+    L.fa_ctc_merge_chunks.argtypes = [vp, vp, i32, i32, i32, vp, sz, C.POINTER(i32)]
+    L.fa_ctc_merge_chunks_device.argtypes = L.fa_ctc_merge_chunks.argtypes
+    L.fa_ctc_spotter_create.argtypes = [i32, i32, i32, vp, vp, C.POINTER(vp)]
+    L.fa_ctc_spotter_destroy.argtypes = [vp]
+    L.fa_ctc_spotter_destroy.restype = None
+    L.fa_ctc_spot.argtypes = [vp, vp, vp, i32, C.POINTER(f32), vp, C.POINTER(i64), vp, sz]
+    L.fa_ctc_spot_device.argtypes = L.fa_ctc_spot.argtypes
+    L.fa_ctc_spot_constrained.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    L.fa_ctc_spot_constrained_device.argtypes = L.fa_ctc_spot_constrained.argtypes
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]
