@@ -1,5 +1,5 @@
 """ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h``,
-``include/fluidaudio_b200_lseend.h`` and ``include/fluidaudio_b200_ctc.h``).
+``include/fluidaudio_b200_lseend.h``, ``include/fluidaudio_b200_ctc.h`` and ``include/fluidaudio_b200_ctc_decode.h``).
 
 The library is the product: it is built in-tree by ``__graft_entry__.build()`` / ``make -C fluidaudio_b200/csrc``.
 There is no Python or CPU fallback — if the shared object is missing, or no sm_90a device is visible, every
@@ -134,6 +134,11 @@ class CtcDetection(C.Structure):
                 ("end_frame", C.c_int32)]
 
 
+class CtcBeamConfig(C.Structure):
+    _fields_ = [("beam_width", C.c_int32), ("token_candidates", C.c_int32), ("lm_weight", C.c_float),
+                ("word_bonus", C.c_float)]
+
+
 # fa_ctc_detection as a numpy record
 CTC_DETECTION = np.dtype([("clip", np.int32), ("term", np.int32), ("score", np.float32), ("start_frame", np.int32),
                           ("end_frame", np.int32)])
@@ -189,6 +194,13 @@ CTC_SYMBOLS = [
     "fa_ctc_log_softmax", "fa_ctc_log_softmax_device", "fa_ctc_merge_chunks", "fa_ctc_merge_chunks_device",
     "fa_ctc_spotter_create", "fa_ctc_spotter_destroy", "fa_ctc_spot", "fa_ctc_spot_device", "fa_ctc_spot_constrained",
     "fa_ctc_spot_constrained_device",
+]
+
+# every symbol include/fluidaudio_b200_ctc_decode.h declares (CTC decoding)
+CTC_DECODE_SYMBOLS = [
+    "fa_ctc_beam_default_config", "fa_ctc_lm_create", "fa_ctc_lm_destroy", "fa_ctc_decoder_create",
+    "fa_ctc_decoder_destroy", "fa_ctc_beam_search", "fa_ctc_beam_search_device", "fa_ctc_greedy",
+    "fa_ctc_greedy_device",
 ]
 
 _lib = None
@@ -360,6 +372,18 @@ def load():
     L.fa_ctc_spot_device.argtypes = L.fa_ctc_spot.argtypes
     L.fa_ctc_spot_constrained.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     L.fa_ctc_spot_constrained_device.argtypes = L.fa_ctc_spot_constrained.argtypes
+    L.fa_ctc_beam_default_config.argtypes = [C.POINTER(CtcBeamConfig)]
+    L.fa_ctc_beam_default_config.restype = None
+    L.fa_ctc_lm_create.argtypes = [i32, vp, vp, vp, vp, vp, i64, vp, vp, vp, C.POINTER(vp)]
+    L.fa_ctc_lm_destroy.argtypes = [vp]
+    L.fa_ctc_lm_destroy.restype = None
+    L.fa_ctc_decoder_create.argtypes = [i32, i32, vp, vp, C.POINTER(vp)]
+    L.fa_ctc_decoder_destroy.argtypes = [vp]
+    L.fa_ctc_decoder_destroy.restype = None
+    L.fa_ctc_beam_search.argtypes = [vp, vp, vp, vp, i32, C.POINTER(CtcBeamConfig), vp, vp, vp, sz, C.POINTER(i64)]
+    L.fa_ctc_beam_search_device.argtypes = L.fa_ctc_beam_search.argtypes
+    L.fa_ctc_greedy.argtypes = [vp, vp, i32, i32, i32, vp, vp, sz, C.POINTER(i64)]
+    L.fa_ctc_greedy_device.argtypes = L.fa_ctc_greedy.argtypes
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

@@ -207,5 +207,25 @@ for step in range(4):
 tl.finalize(tids)
 tl.reset(tids[:1])
 tl.push(tids, [rng.random((9, 4), np.float32)] * 2)
+# CTC decoding: greedy over three clips, beam search with a small bigram LM (the radix select, the parent fold-in, the
+# trie conses, the LM walk), beam_width 0 and the NaN refusal
+from fluidaudio_b200 import ctc_decoding as CD
+crng = np.random.default_rng(21)
+cvoc = {v: ("\u2581" if v % 3 == 0 else "") + "ab"[v % 2] + "cd"[(v // 2) % 2] for v in range(16)}
+cclips = [np.round(crng.normal(0, 1, size=(T, 17)) * 2).astype(np.float32) / 2 - 3 for T in (30, 0, 11)]
+CD.greedy_ids(cclips, 17, 16)
+carpa = CD.ARPALanguageModel()
+carpa.unigrams = {w: CD.ARPALanguageModel.Entry(np.float32(-1.5), np.float32(-0.3)) for w in ("ac", "bd", "acbd")}
+carpa.bigrams = {"ac": {"bd": CD.ARPALanguageModel.Entry(np.float32(-0.2), np.float32(0.0))}}
+cdec = CD.CtcDecoder(cvoc, 17, 16)
+cdec.beam_search(cclips, carpa, 8, 0.3, 0.1, 5)
+cdec.beam_search(cclips, None, 0, 0.3, 0.0, 5)
+cbad = [cclips[0].copy()]
+cbad[0][3, 2] = np.nan
+try:
+    cdec.beam_search(cbad, carpa, 8, 0.3, 0.1, 5)
+except _lib.FluidAudioError:
+    pass
+cdec.close()
 _lib.synchronize()
 print("sanitize target done")
