@@ -1,5 +1,6 @@
 """ctypes binding of ``lib/libfluidaudio_b200.so`` (C ABI declared in ``include/fluidaudio_b200.h``,
-``include/fluidaudio_b200_lseend.h``, ``include/fluidaudio_b200_ctc.h`` and ``include/fluidaudio_b200_ctc_decode.h``).
+``include/fluidaudio_b200_lseend.h``, ``include/fluidaudio_b200_ctc.h``, ``include/fluidaudio_b200_ctc_decode.h`` and
+``include/fluidaudio_b200_vad.h``).
 
 The library is the product: it is built in-tree by ``__graft_entry__.build()`` / ``make -C fluidaudio_b200/csrc``.
 There is no Python or CPU fallback — if the shared object is missing, or no sm_90a device is visible, every
@@ -139,6 +140,28 @@ class CtcBeamConfig(C.Structure):
                 ("word_bonus", C.c_float)]
 
 
+class VadConfig(C.Structure):
+    _fields_ = [("default_threshold", C.c_float), ("min_speech_duration", C.c_double),
+                ("min_silence_duration", C.c_double), ("max_speech_duration", C.c_double),
+                ("speech_padding", C.c_double), ("silence_threshold_for_split", C.c_float),
+                ("has_negative_threshold", C.c_int32), ("negative_threshold", C.c_float),
+                ("negative_threshold_offset", C.c_float), ("min_silence_at_max_speech", C.c_double),
+                ("use_max_possible_silence_at_max_speech", C.c_int32)]
+
+
+class VadResolved(C.Structure):
+    _fields_ = [("threshold", C.c_float), ("negative_threshold", C.c_float),
+                ("silence_threshold_for_split", C.c_float), ("use_max_possible_silence_at_max_speech", C.c_int32),
+                ("min_speech_samples", C.c_int64), ("min_silence_samples", C.c_int64),
+                ("max_speech_samples", C.c_int64), ("speech_pad_samples", C.c_int64),
+                ("min_silence_at_max_speech_samples", C.c_int64)]
+
+
+class VadSessionInfo(C.Structure):
+    _fields_ = [("triggered", C.c_int32), ("has_pending", C.c_int32), ("temp_end_sample", C.c_int64),
+                ("processed_samples", C.c_int64)]
+
+
 # fa_ctc_detection as a numpy record
 CTC_DETECTION = np.dtype([("clip", np.int32), ("term", np.int32), ("score", np.float32), ("start_frame", np.int32),
                           ("end_frame", np.int32)])
@@ -201,6 +224,14 @@ CTC_DECODE_SYMBOLS = [
     "fa_ctc_beam_default_config", "fa_ctc_lm_create", "fa_ctc_lm_destroy", "fa_ctc_decoder_create",
     "fa_ctc_decoder_destroy", "fa_ctc_beam_search", "fa_ctc_beam_search_device", "fa_ctc_greedy",
     "fa_ctc_greedy_device",
+]
+
+# every symbol include/fluidaudio_b200_vad.h declares (voice activity detection)
+VAD_SYMBOLS = [
+    "fa_vad_default_config", "fa_vad_resolve", "fa_vad_stream_create", "fa_vad_stream_destroy", "fa_vad_stream_open",
+    "fa_vad_stream_close", "fa_vad_stream_model_inputs", "fa_vad_stream_model_inputs_device", "fa_vad_stream_advance",
+    "fa_vad_stream_advance_device", "fa_vad_stream_session_state", "fa_vad_segment", "fa_vad_segment_device",
+    "fa_fsmn_vad_decide", "fa_fsmn_vad_decide_device",
 ]
 
 _lib = None
@@ -384,6 +415,24 @@ def load():
     L.fa_ctc_beam_search_device.argtypes = L.fa_ctc_beam_search.argtypes
     L.fa_ctc_greedy.argtypes = [vp, vp, i32, i32, i32, vp, vp, sz, C.POINTER(i64)]
     L.fa_ctc_greedy_device.argtypes = L.fa_ctc_greedy.argtypes
+    VC = C.POINTER(VadConfig)
+    L.fa_vad_default_config.argtypes = [VC]
+    L.fa_vad_default_config.restype = None
+    L.fa_vad_resolve.argtypes = [VC, C.POINTER(VadResolved)]
+    L.fa_vad_stream_create.argtypes = [C.POINTER(vp)]
+    L.fa_vad_stream_destroy.argtypes = [vp]
+    L.fa_vad_stream_destroy.restype = None
+    L.fa_vad_stream_open.argtypes = [vp, C.POINTER(i32)]
+    L.fa_vad_stream_close.argtypes = [vp, i32]
+    L.fa_vad_stream_model_inputs.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]
+    L.fa_vad_stream_model_inputs_device.argtypes = L.fa_vad_stream_model_inputs.argtypes
+    L.fa_vad_stream_advance.argtypes = [vp, i32, vp, vp, vp, vp, VC, vp]
+    L.fa_vad_stream_advance_device.argtypes = L.fa_vad_stream_advance.argtypes
+    L.fa_vad_stream_session_state.argtypes = [vp, i32, C.POINTER(VadSessionInfo), vp, vp, vp]
+    L.fa_vad_segment.argtypes = [vp, vp, i32, vp, VC, vp, vp, sz, C.POINTER(i64)]
+    L.fa_vad_segment_device.argtypes = L.fa_vad_segment.argtypes
+    L.fa_fsmn_vad_decide.argtypes = [vp, vp, i32, vp, vp, sz, C.POINTER(i64)]
+    L.fa_fsmn_vad_decide_device.argtypes = L.fa_fsmn_vad_decide.argtypes
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

@@ -227,5 +227,27 @@ try:
 except _lib.FluidAudioError:
     pass
 cdec.close()
+# VAD: Silero sessions with chunks of 0, 1, 63, 64, 4096 and 5000 samples (host and device), a refused advance,
+# segmentation of clips with split corners, and the FSMN decision
+from fluidaudio_b200 import vad as VD
+vrng = np.random.default_rng(22)
+vst = VD.SileroVadStreams()
+vids = [vst.open() for _ in range(6)]
+for _ in range(3):
+    vin, vh, vc = vst.model_inputs(vids, [vrng.normal(size=n).astype(np.float32) for n in (0, 1, 63, 64, 4096, 5000)])
+    vst.advance(vids, vrng.uniform(size=6).astype(np.float32), vh + 1, vc - 1,
+                seg=VD.VadSegmentationConfig(min_silence_duration=0.0))
+try:
+    vst.advance(vids[:1], [0.5], vh[:1], vc[:1])
+except _lib.FluidAudioError:
+    pass
+vaud = _lib.DeviceBuffer(4096 * 4)
+vbuf = [_lib.DeviceBuffer(n) for n in (4160 * 4, 128 * 4, 128 * 4)]
+vst.model_inputs_device(vids[:1], vaud, np.array([0, 4096], np.int64), *vbuf)
+vst.state(vids[0])
+vst.close_handle()
+vprobs = [np.repeat(vrng.choice(np.array([0.1, 0.5, 0.9], np.float32), size=n), 4)[:4 * n] for n in (0, 5, 300)]
+VD.segment_sample_ranges(vprobs, [0, 20000, 300 * 4096], seg=VD.VadSegmentationConfig(max_speech_duration=2.0))
+VD.fsmn_vad_decide([np.repeat(vrng.choice(np.array([0.05, 0.9], np.float32), size=50), 90) for _ in range(3)])
 _lib.synchronize()
 print("sanitize target done")
