@@ -226,12 +226,41 @@ CTC_DECODE_SYMBOLS = [
     "fa_ctc_greedy_device",
 ]
 
+class OnlineDiarConfig(C.Structure):
+    """fa_od_config's layout"""
+    _fields_ = [("clustering_threshold", C.c_float), ("min_speech_duration", C.c_float),
+                ("min_embedding_update_duration", C.c_float), ("min_silence_gap", C.c_float),
+                ("num_clusters", C.c_int32), ("min_active_frames_count", C.c_float), ("chunk_duration", C.c_float),
+                ("chunk_overlap", C.c_float)]
+
+
+class OnlineDiarResolved(C.Structure):
+    """fa_od_resolved's layout"""
+    _fields_ = [("speaker_threshold", C.c_float), ("embedding_threshold", C.c_float),
+                ("min_speech_duration", C.c_float), ("min_active_frames_count", C.c_float),
+                ("chunk_size", C.c_int64), ("step_size", C.c_int64)]
+
+
+ONLINE_DIAR_SPEAKER = np.dtype([("key", "<i8"), ("numeric", "<i8"), ("update_count", "<i8"), ("duration", "<f4"),
+                                ("named", "<i4"), ("has_numeric", "<i4"), ("permanent", "<i4"),
+                                ("raw_count", "<i4")], align=True)   # fa_od_speaker's layout
+
+
 # every symbol include/fluidaudio_b200_vad.h declares (voice activity detection)
 VAD_SYMBOLS = [
     "fa_vad_default_config", "fa_vad_resolve", "fa_vad_stream_create", "fa_vad_stream_destroy", "fa_vad_stream_open",
     "fa_vad_stream_close", "fa_vad_stream_model_inputs", "fa_vad_stream_model_inputs_device", "fa_vad_stream_advance",
     "fa_vad_stream_advance_device", "fa_vad_stream_session_state", "fa_vad_segment", "fa_vad_segment_device",
     "fa_fsmn_vad_decide", "fa_fsmn_vad_decide_device",
+]
+
+# every symbol include/fluidaudio_b200_online_diar.h declares (streaming speaker tracking)
+ONLINE_DIAR_SYMBOLS = [
+    "fa_od_default_config", "fa_od_resolve", "fa_od_chunk_inputs", "fa_od_chunk_inputs_device",
+    "fa_od_enrollment_inputs", "fa_od_enrollment_inputs_device", "fa_od_create", "fa_od_destroy", "fa_od_open",
+    "fa_od_close", "fa_od_embedding_inputs", "fa_od_embedding_inputs_device", "fa_od_advance", "fa_od_advance_device",
+    "fa_od_query", "fa_od_query_device", "fa_od_speaker_count", "fa_od_read", "fa_od_initialize", "fa_od_remove",
+    "fa_od_merge", "fa_od_set_permanent", "fa_od_reset", "fa_od_upsert",
 ]
 
 _lib = None
@@ -433,6 +462,33 @@ def load():
     L.fa_vad_segment_device.argtypes = L.fa_vad_segment.argtypes
     L.fa_fsmn_vad_decide.argtypes = [vp, vp, i32, vp, vp, sz, C.POINTER(i64)]
     L.fa_fsmn_vad_decide_device.argtypes = L.fa_fsmn_vad_decide.argtypes
+    OC = C.POINTER(OnlineDiarConfig)
+    L.fa_od_default_config.argtypes = [OC]
+    L.fa_od_default_config.restype = None
+    L.fa_od_resolve.argtypes = [OC, C.POINTER(OnlineDiarResolved)]
+    L.fa_od_chunk_inputs.argtypes = [vp, vp, i32, i64, vp, vp]
+    L.fa_od_chunk_inputs_device.argtypes = L.fa_od_chunk_inputs.argtypes
+    L.fa_od_enrollment_inputs.argtypes = [vp, vp, i32, i32, vp, vp]
+    L.fa_od_enrollment_inputs_device.argtypes = L.fa_od_enrollment_inputs.argtypes
+    L.fa_od_create.argtypes = [i32, C.POINTER(vp)]
+    L.fa_od_destroy.argtypes = [vp]
+    L.fa_od_destroy.restype = None
+    L.fa_od_open.argtypes = [vp, C.POINTER(i32)]
+    L.fa_od_close.argtypes = [vp, i32]
+    L.fa_od_embedding_inputs.argtypes = [vp, i32, vp, vp, OC, vp, vp]
+    L.fa_od_embedding_inputs_device.argtypes = L.fa_od_embedding_inputs.argtypes
+    L.fa_od_advance.argtypes = [vp, i32, vp, vp, vp, OC, vp, vp, vp, vp]
+    L.fa_od_advance_device.argtypes = L.fa_od_advance.argtypes
+    L.fa_od_query.argtypes = [vp, i32, i32, vp, vp]
+    L.fa_od_query_device.argtypes = L.fa_od_query.argtypes
+    L.fa_od_speaker_count.argtypes = [vp, i32, C.POINTER(i64), C.POINTER(i64)]
+    L.fa_od_read.argtypes = [vp, i32, vp, vp, vp]
+    L.fa_od_initialize.argtypes = [vp, i32, i32, vp, vp, vp, i32, i32]
+    L.fa_od_remove.argtypes = [vp, i32, i32, i64, i32, C.POINTER(i32)]
+    L.fa_od_merge.argtypes = [vp, i32, i32, i64, i32, i64, i32, C.POINTER(i32)]
+    L.fa_od_set_permanent.argtypes = [vp, i32, i32, i64, i32, C.POINTER(i32)]
+    L.fa_od_reset.argtypes = [vp, i32, i32]
+    L.fa_od_upsert.argtypes = [vp, i32, vp, vp, vp]
     L.fa_ahc_last_stage_ms.argtypes = [vp]
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]

@@ -249,5 +249,32 @@ vst.close_handle()
 vprobs = [np.repeat(vrng.choice(np.array([0.1, 0.5, 0.9], np.float32), size=n), 4)[:4 * n] for n in (0, 5, 300)]
 VD.segment_sample_ranges(vprobs, [0, 20000, 300 * 4096], seg=VD.VadSegmentationConfig(max_speech_duration=2.0))
 VD.fsmn_vad_decide([np.repeat(vrng.choice(np.array([0.05, 0.9], np.float32), size=50), 90) for _ in range(3)])
+# online diarization: model inputs (chunks of 0 to 200 000 samples, enrollment), two sessions over four chunks with
+# databases grown past a reallocation, the database operations, queries, a refused advance and the device variants
+from fluidaudio_b200 import online_diarizer as ODZ
+orng = np.random.default_rng(23)
+ODZ.chunk_inputs([orng.normal(size=n).astype(np.float32) for n in (0, 1, 80000, 200000)])
+ODZ.enrollment_inputs([orng.normal(size=n).astype(np.float32) for n in (0, 100, 170000)], 589)
+odb = ODZ.SpeakerDatabases(589, ODZ.DiarizerConfig(min_speech_duration=0.1))
+oids = [odb.open() for _ in range(2)]
+odb.initialize_known_speakers(oids[0], [ODZ.Speaker(str(k), orng.normal(size=256).astype(np.float32), 1.0, 1,
+                                                    orng.normal(size=(3, 256)).astype(np.float32)) for k in range(6)])
+for t in range(4):
+    olg = np.repeat(np.eye(7, dtype=np.float32)[orng.integers(0, 7, size=(2, 31))], 19, axis=1)[:, :589] * 4
+    odb.embedding_inputs(oids, olg)
+    odb.advance(oids, orng.normal(size=(2, 3, 256)).astype(np.float32), [10.0 * t] * 2)
+odb.upsert_speaker(oids[1], ODZ.Speaker("alice", orng.normal(size=256).astype(np.float32), 2.0))
+odb.merge_speaker(oids[0], "1", "2")
+odb.set_permanent(oids[0], "3")
+odb.remove_speaker(oids[0], "4")
+odb.find_mergeable_pairs(oids[0], 2.0)
+odb.find_matching_speakers(oids[1], orng.normal(size=256).astype(np.float32), 2.0)
+try:
+    odb.advance(oids, np.zeros((2, 3, 256), np.float32), [0.0, 0.0])
+except _lib.FluidAudioError:
+    pass
+odb.reset(oids[0], True)
+odb.speakers(oids[0])
+odb.close_handle()
 _lib.synchronize()
 print("sanitize target done")
