@@ -304,8 +304,10 @@ int Spotter::init(int vocab_, int blank_, int terms_, const int32_t *tokens, con
     st = d_terms.grow(desc_bytes + tok_bytes + 1);
     if (st != FA_OK) return st;
     char *d = static_cast<char *>(d_terms.data());
-    if (desc_bytes) FA_CUDA_TRY(cudaMemcpy(d, desc.data(), desc_bytes, cudaMemcpyHostToDevice));
-    if (tok_bytes) FA_CUDA_TRY(cudaMemcpy(d + desc_bytes, tokens, tok_bytes, cudaMemcpyHostToDevice));
+    // on the stream the kernels read them on, complete before `desc` and the caller's tokens go
+    if (desc_bytes) FA_CUDA_TRY(cudaMemcpyAsync(d, desc.data(), desc_bytes, cudaMemcpyHostToDevice, stream));
+    if (tok_bytes) FA_CUDA_TRY(cudaMemcpyAsync(d + desc_bytes, tokens, tok_bytes, cudaMemcpyHostToDevice, stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(stream));
     return FA_OK;
 }
 

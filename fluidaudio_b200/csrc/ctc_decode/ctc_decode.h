@@ -30,6 +30,7 @@ struct LmTables {
 // An ARPALanguageModel in HBM (fa_ctc_lm): read-only once made.
 struct Lm {
     int device = 0;
+    Stream stream;   // the upload's; declared first, so destroyed last
     DeviceBuffer<> d;
     LmView view{};                 // device pointers, on the host
     const LmView *d_view = nullptr;   // the same in HBM, for the kernels

@@ -487,6 +487,8 @@ int gather(UploadStage<> &stage, DeviceBuffer<> &d_buf, cudaStream_t stream, boo
 // ------------------------------------------------------------------------------------------------ host
 int Lm::init(const LmTables &t) {
     FA_CUDA_TRY(cudaGetDevice(&device));
+    int st = stream.create();
+    if (st != FA_OK) return st;
     const unsigned long long *ck, *bk;
     const int *cn, *nw;
     const float *ulp, *ubo, *blp;
@@ -501,11 +503,12 @@ int Lm::init(const LmTables &t) {
         ubo = c.take<float>(t.uni_backoff.size() + 1);
         blp = c.take<float>(t.bigram_log_prob.size());
     };
-    const int st = carve_arena(d, layout);
+    st = carve_arena(d, layout);
     if (st != FA_OK) return st;
-    auto put = [](const void *dst, const auto &v) {
+    auto put = [&](const void *dst, const auto &v) {
         return v.empty() ? cudaSuccess
-                         : cudaMemcpy(const_cast<void *>(dst), v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
+                         : cudaMemcpyAsync(const_cast<void *>(dst), v.data(), v.size() * sizeof(v[0]),
+                                           cudaMemcpyHostToDevice, stream);
     };
     FA_CUDA_TRY(put(ck, t.child_key));
     FA_CUDA_TRY(put(bk, t.bigram_key));
@@ -515,7 +518,9 @@ int Lm::init(const LmTables &t) {
     FA_CUDA_TRY(put(ubo, t.uni_backoff));
     FA_CUDA_TRY(put(blp, t.bigram_log_prob));
     view = LmView{ck, cn, (long long)t.child_key.size(), nw, ulp, ubo, bk, blp, (long long)t.bigram_key.size()};
-    FA_CUDA_TRY(cudaMemcpy(dv, &view, sizeof(view), cudaMemcpyHostToDevice));
+    FA_CUDA_TRY(cudaMemcpyAsync(dv, &view, sizeof(view), cudaMemcpyHostToDevice, stream));
+    // complete before fa_ctc_lm_create returns: a decoder's stream is not ordered after this one
+    FA_CUDA_TRY(cudaStreamSynchronize(stream));
     d_view = dv;
     return FA_OK;
 }
@@ -540,9 +545,10 @@ int Decoder::init(int vocab_, int blank_, const char *bytes, const int64_t *offs
         d_bytes = c.take<unsigned char>((size_t)n_bytes + 1);
     });
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpy(d_off, offsets, ((size_t)vocab + 1) * sizeof(long long), cudaMemcpyHostToDevice));
-    FA_CUDA_TRY(cudaMemcpy(d_bound, boundary.data(), (size_t)vocab, cudaMemcpyHostToDevice));
-    if (n_bytes) FA_CUDA_TRY(cudaMemcpy(d_bytes, bytes, (size_t)n_bytes, cudaMemcpyHostToDevice));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_off, offsets, ((size_t)vocab + 1) * sizeof(long long), cudaMemcpyHostToDevice, stream));
+    FA_CUDA_TRY(cudaMemcpyAsync(d_bound, boundary.data(), (size_t)vocab, cudaMemcpyHostToDevice, stream));
+    if (n_bytes) FA_CUDA_TRY(cudaMemcpyAsync(d_bytes, bytes, (size_t)n_bytes, cudaMemcpyHostToDevice, stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(stream));
     pieces = Pieces{d_bytes, d_off, d_bound};
     return FA_OK;
 }

@@ -459,11 +459,15 @@ static int window_offset(const MelConfig &c, int placement) { return placement =
 
 static_assert(sizeof(MelSlot) == sizeof(int4) && offsetof(MelSlot, mel) == offsetof(int4, w), "MelSlot is an int4");
 
-// Device copy of a host table (at least one element, so that an empty table still has an address).
-template <typename T, typename U> static int upload_table(DeviceBuffer<T> &b, const std::vector<U> &v) {
+// Device copy of a host table (at least one element, so that an empty table still has an address), complete on return:
+// `v` may be a temporary, and the kernels that read the table run on `stream`.
+template <typename T, typename U>
+static int upload_table(DeviceBuffer<T> &b, const std::vector<U> &v, cudaStream_t stream) {
     const int st = b.grow(std::max<size_t>(1, v.size()) * sizeof(U));
     if (st != FA_OK) return st;
-    if (!v.empty()) FA_CUDA_TRY(cudaMemcpy(b.data(), v.data(), v.size() * sizeof(U), cudaMemcpyHostToDevice));
+    if (v.empty()) return FA_OK;
+    FA_CUDA_TRY(cudaMemcpyAsync(b.data(), v.data(), v.size() * sizeof(U), cudaMemcpyHostToDevice, stream));
+    FA_CUDA_TRY(cudaStreamSynchronize(stream));
     return FA_OK;
 }
 
@@ -520,12 +524,15 @@ int MelPlan::init(const MelConfig &c) {
         }
     }
 
+    for (auto &s : streams)
+        if (st == FA_OK) st = s.create();
+    if (st != FA_OK) return st;
     std::vector<float> win_tab;
     std::vector<uint8_t> in_tab;
     for (int pl = 0; pl < 2; ++pl) {
         place_window(window, n_fft, window_offset(cfg, pl), win_tab, in_tab);
-        st = upload_table(d_win_tab_mode[pl], win_tab);
-        if (st == FA_OK) st = upload_table(d_in_tab_mode[pl], in_tab);
+        st = upload_table(d_win_tab_mode[pl], win_tab, streams[1]);
+        if (st == FA_OK) st = upload_table(d_in_tab_mode[pl], in_tab, streams[1]);
         if (st != FA_OK) return st;
         if (!generic) {
             std::vector<LaneTables<double>> t64(32);
@@ -534,26 +541,25 @@ int MelPlan::init(const MelConfig &c) {
                 load_lane_tables(l, win_tab.data(), in_tab.data(), t64[l]);
                 load_lane_tables(l, win_tab.data(), in_tab.data(), t32[l]);
             }
-            st = upload_table(d_lane_tab[pl][FA_MEL_PRECISION_F64], t64);
-            if (st == FA_OK) st = upload_table(d_lane_tab[pl][FA_MEL_PRECISION_F32], t32);
+            st = upload_table(d_lane_tab[pl][FA_MEL_PRECISION_F64], t64, streams[1]);
+            if (st == FA_OK) st = upload_table(d_lane_tab[pl][FA_MEL_PRECISION_F32], t32, streams[1]);
             if (st != FA_OK) return st;
         }
     }
     // mel512_kernel finds the bins of a quad swizzled in its power tile, the any-nFFT kernel in natural order; the
     // weights carry 1/4 where the tile holds 4|X|^2
-    st = upload_table(d_fb_w, pack_weights(filterbank, bands, bins, !generic, spectrum == kSpecPower ? 0.25f : 1.0f));
-    if (st == FA_OK) st = upload_table(d_fb_slots, bands.slots);
-    if (st == FA_OK) st = upload_table(d_fb_lo, bands.lo);
-    if (st == FA_OK) st = upload_table(d_fb_hi, bands.hi);
-    if (st == FA_OK) st = upload_table(d_fb_off, bands.off);
-    for (auto &s : streams)
-        if (st == FA_OK) st = s.create();
+    st = upload_table(d_fb_w, pack_weights(filterbank, bands, bins, !generic, spectrum == kSpecPower ? 0.25f : 1.0f),
+                      streams[1]);
+    if (st == FA_OK) st = upload_table(d_fb_slots, bands.slots, streams[1]);
+    if (st == FA_OK) st = upload_table(d_fb_lo, bands.lo, streams[1]);
+    if (st == FA_OK) st = upload_table(d_fb_hi, bands.hi, streams[1]);
+    if (st == FA_OK) st = upload_table(d_fb_off, bands.off, streams[1]);
     if (st != FA_OK) return st;
     if (generic) {
         // FP64 twiddle table W_n^k and the shared-memory budget: as many warps per CTA as fit beside it
         std::vector<cpxd> tw(n_fft / 2);
         for (int k = 0; k < n_fft / 2; ++k) tw[k] = unit_root(k, n_fft);
-        st = upload_table(d_generic_tw, tw);
+        st = upload_table(d_generic_tw, tw, streams[1]);
         if (st != FA_OK) return st;
         generic_prow = ((bins + 3) & ~3) + 4;
         int log2n = 0;

@@ -98,7 +98,10 @@ int MelPlan::ensure_resampler(double in_rate, double out_rate) {
     rs_in = rs_out = 0.0;   // the table is being replaced
     st = d_rs_tab.grow(d.table.size() * sizeof(float));
     if (st != FA_OK) return st;
-    FA_CUDA_TRY(cudaMemcpy(d_rs_tab.data(), d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice));
+    // on the compute stream, which runs the conversion; complete before `d` is moved
+    FA_CUDA_TRY(cudaMemcpyAsync(d_rs_tab.data(), d.table.data(), d.table.size() * sizeof(float), cudaMemcpyHostToDevice,
+                                streams[1]));
+    FA_CUDA_TRY(cudaStreamSynchronize(streams[1]));
     rs_design = std::move(d);
     rs_in = in_rate;
     rs_out = out_rate;

@@ -1,4 +1,5 @@
-"""Seeded inputs of the CTC decoding tests: log-prob rows (random, tie-heavy quantised, constant, with -inf columns),
+"""Seeded inputs of the CTC decoding tests: log-prob rows (random, tie-heavy quantised, constant, with -inf columns,
+and peaky log-softmax rows like a model's),
 SentencePiece-like vocabularies over a small alphabet (word starts, continuations, the bare U+2581, empty and missing
 pieces) and synthetic bigram LMs whose words those pieces spell."""
 import numpy as np
@@ -49,3 +50,24 @@ def synthetic_lm(rng, words=400, bigrams=2000, letters="abcdefgh", max_len=4):
         c, w = vocab[int(rng.integers(words))], vocab[int(rng.integers(words))]
         bi.setdefault(c, {})[w] = np.float32(-rng.uniform(0.1, 5))
     return uni, bi
+
+
+def peaky(rng, T, V, sharpness=8.0, blank=None):
+    """[T x V] float32 log-softmax of logits shaped like a CTC model's output: runs of blank frames between tokens held
+    for one to three frames, each frame's mass almost all on its dominant column (logit lead `sharpness` over unit
+    normal noise).  With the blank outside [0, V) a blank run has no dominant column."""
+    blank = V - 1 if blank is None else blank
+    tokens = [v for v in range(V) if v != blank]
+    x = rng.normal(0, 1, size=(T, V))
+    t = 0
+    while t < T:
+        n = int(rng.geometric(0.3))
+        if 0 <= blank < V:
+            x[t:t + n, blank] += sharpness
+        t += n
+        if tokens:
+            n = int(rng.integers(1, 4))
+            x[t:t + n, tokens[int(rng.integers(len(tokens)))]] += sharpness
+            t += n
+    x -= x.max(1, keepdims=True)
+    return (x - np.log(np.exp(x).sum(1, keepdims=True))).astype(np.float32)

@@ -9,12 +9,14 @@ the counter's delta (the VBx formula follows ``tests/test_gpu_cluster_sweep.py``
 import ctypes as C
 import os
 import re
+import sys
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "fluidaudio_b200", "csrc")
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+
+from csrc_sources import path, sources  # noqa: E402
 
 
 def _code(path):
@@ -27,10 +29,10 @@ def _code(path):
 
 def test_every_launch_goes_through_the_counting_helpers():
     offenders = []
-    for name in sorted(os.listdir(CSRC)):
-        if not name.endswith((".cu", ".cuh", ".h", ".cpp")) or name == "fa_common.cuh":
+    for name in sources():
+        if name == "fa_common.cuh":
             continue
-        code = _code(os.path.join(CSRC, name))
+        code = _code(path(name))
         for token in ("<<<", "cudaLaunchCooperativeKernel", "cudaLaunchKernel"):
             if token in code:
                 offenders.append(f"{name}: {token}")
