@@ -263,6 +263,23 @@ ONLINE_DIAR_SYMBOLS = [
     "fa_od_merge", "fa_od_set_permanent", "fa_od_reset", "fa_od_upsert",
 ]
 
+# every symbol include/fluidaudio_b200_luxtts.h declares (LuxTTS synthesis around the caller's models)
+LUXTTS_SYMBOLS = [
+    "fa_luxtts_plan", "fa_luxtts_create", "fa_luxtts_destroy", "fa_luxtts_begin", "fa_luxtts_begin_device",
+    "fa_luxtts_text_condition", "fa_luxtts_text_condition_device", "fa_luxtts_model_inputs",
+    "fa_luxtts_model_inputs_device", "fa_luxtts_advance", "fa_luxtts_advance_device", "fa_luxtts_vocoder_input",
+    "fa_luxtts_vocoder_input_device", "fa_luxtts_finish", "fa_luxtts_finish_device", "fa_luxtts_close",
+    "fa_luxtts_request_state",
+]
+
+
+class LuxTtsPlanInfo(C.Structure):
+    """fa_luxtts_plan_info's layout"""
+    _fields_ = [("reason", C.c_int32), ("prompt_samples", C.c_int32), ("prompt_frames", C.c_int32),
+                ("token_count", C.c_int32), ("features_length", C.c_int32), ("gen_frames", C.c_int32),
+                ("bucket", C.c_int32), ("boosted", C.c_int32), ("prompt_rms", C.c_float), ("step", C.c_int32)]
+
+
 _lib = None
 
 
@@ -493,6 +510,28 @@ def load():
     L.fa_ahc_last_stage_ms.restype = None
     L.fastcluster_compute_centroid_linkage.argtypes = [vp, sz, sz, vp, sz]
     L.fastcluster_compute_centroid_linkage.restype = C.c_int
+    LP = C.POINTER(LuxTtsPlanInfo)
+    L.fa_luxtts_plan.argtypes = [i64, i32, i32, f32, LP]
+    L.fa_luxtts_create.argtypes = [C.POINTER(vp)]
+    L.fa_luxtts_destroy.argtypes = [vp]
+    L.fa_luxtts_destroy.restype = None
+    for name in ("fa_luxtts_begin", "fa_luxtts_begin_device"):
+        getattr(L, name).argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, LP, vp, vp]
+    for name in ("fa_luxtts_text_condition", "fa_luxtts_text_condition_device"):
+        getattr(L, name).argtypes = [vp, i32, vp, vp, i64, i64, vp]
+    for name in ("fa_luxtts_model_inputs", "fa_luxtts_model_inputs_device"):
+        getattr(L, name).argtypes = [vp, i32, vp, vp, vp]
+    for name in ("fa_luxtts_advance", "fa_luxtts_advance_device"):
+        getattr(L, name).argtypes = [vp, i32, vp, vp, i64, i64]
+    for name in ("fa_luxtts_vocoder_input", "fa_luxtts_vocoder_input_device"):
+        getattr(L, name).argtypes = [vp, i32, vp, i32, vp]
+    for name in ("fa_luxtts_finish", "fa_luxtts_finish_device"):
+        getattr(L, name).argtypes = [vp, i32, vp, vp, i64, i64, vp, sz, vp, C.POINTER(i64)]
+    L.fa_luxtts_close.argtypes = [vp, i32]
+    L.fa_luxtts_request_state.argtypes = [vp, i32, LP, vp]
+    for name in LUXTTS_SYMBOLS:
+        if name != "fa_luxtts_destroy":
+            getattr(L, name).restype = C.c_int
     _lib = L
     return L
 

@@ -276,5 +276,27 @@ except _lib.FluidAudioError:
 odb.reset(oids[0], True)
 odb.speakers(oids[0])
 odb.close_handle()
+# LuxTTS: begin with boosted and unboosted prompts (one capped) and a refused call, a text condition at row stride 112,
+# four interleaved steps, the vocoder input at both buckets and finish with its capacity refusal
+from fluidaudio_b200 import luxtts as LX
+lrng = np.random.default_rng(24)
+lreq = LX.LuxTtsRequests()
+lprompts = [(lrng.normal(size=n) * s).astype(np.float32) for n, s in ((30000, 0.02), (130000, 0.3), (5000, 0.2))]
+lids, lplans, _, _ = lreq.begin(lprompts, [40, 60, 10], [50, 120, 30], [1.0, 1.0, 1.0], [0, 1, 2])
+try:
+    lreq.begin([lprompts[0], np.zeros(3000, np.float32)], [5, 5], [5, 5], [1.0, 1.0], [3, 4])
+except LX.LuxTtsError:
+    pass
+lreq.text_condition(lids, lrng.normal(size=(3, 256, 112)).astype(np.float32))
+for k in range(4):
+    lsel = lids if k % 2 == 0 else lids[::-1]
+    lreq.model_inputs(lsel)
+    lreq.advance(lsel, lrng.normal(size=(3, 1024, 100)).astype(np.float32))
+for lb in (282, 555):
+    lsel = np.array([r for r, p in zip(lids, lplans) if p.bucket == lb], np.int32)
+    if lsel.size:
+        lreq.vocoder_input(lsel, lb)
+        lreq.finish(lsel, lrng.normal(size=(lsel.size, (lb - 1) * 512)).astype(np.float32))
+lreq.close_handle()
 _lib.synchronize()
 print("sanitize target done")
