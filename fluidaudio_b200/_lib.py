@@ -273,6 +273,13 @@ LUXTTS_SYMBOLS = [
 ]
 
 
+# every symbol include/fluidaudio_b200_styletts2.h declares (StyleTTS2 synthesis glue around the caller's models)
+STYLETTS2_SYMBOLS = [
+    "fa_styletts2_plan", "fa_styletts2_sampler_inputs", "fa_styletts2_sampler_inputs_device", "fa_styletts2_style",
+    "fa_styletts2_style_device", "fa_styletts2_align", "fa_styletts2_align_device",
+]
+
+
 class LuxTtsPlanInfo(C.Structure):
     """fa_luxtts_plan_info's layout"""
     _fields_ = [("reason", C.c_int32), ("prompt_samples", C.c_int32), ("prompt_frames", C.c_int32),
@@ -532,6 +539,16 @@ def load():
     for name in LUXTTS_SYMBOLS:
         if name != "fa_luxtts_destroy":
             getattr(L, name).restype = C.c_int
+    L.fa_styletts2_plan.argtypes = [i32, C.POINTER(i32), C.POINTER(i32)]
+    for name in ("fa_styletts2_sampler_inputs", "fa_styletts2_sampler_inputs_device"):
+        getattr(L, name).argtypes = [i32, vp, vp, vp, i32, vp, vp, vp, vp]
+    for name in ("fa_styletts2_style", "fa_styletts2_style_device"):
+        getattr(L, name).argtypes = [i32, vp, vp, vp, vp, vp, vp]
+    for name in ("fa_styletts2_align", "fa_styletts2_align_device"):
+        getattr(L, name).argtypes = [i32, vp, vp, i32, i64, i64, vp, i32, i64, i64, vp, i32, i64, i64, i64, vp, vp, vp,
+                                     vp, vp]
+    for name in STYLETTS2_SYMBOLS:
+        getattr(L, name).restype = C.c_int
     _lib = L
     return L
 

@@ -298,5 +298,31 @@ for lb in (282, 555):
         lreq.vocoder_input(lsel, lb)
         lreq.finish(lsel, lrng.normal(size=(lsel.size, (lb - 1) * 512)).astype(np.float32))
 lreq.close_handle()
+# StyleTTS2 glue: sampler inputs for two buckets and a refusal, the blend, align at odd widths and its too-small and
+# NaN refusals
+from fluidaudio_b200 import styletts2 as ST
+srng = np.random.default_rng(25)
+sglue = ST.StyleTTS2Glue()
+sglue.sampler_inputs([srng.integers(0, 178, size=k) for k in (3, 57)], [0, 1], 57)
+sglue.sampler_inputs([srng.integers(0, 178, size=k) for k in (65, 128)], [2, 3], 128)
+try:
+    sglue.sampler_inputs([np.zeros(3, np.int32), np.zeros(64, np.int32)], [0, 0], 57)
+except _lib.FluidAudioError:
+    pass
+sglue.blend_style(srng.normal(size=(3, 256)), srng.normal(size=(3, 256)), [0.3, 1.0, 0.0], [0.7, 0.0, 1.0])
+scounts = (1, 40, 256)
+slog = [srng.normal(size=(k, 4)).astype(np.float32) * 3 for k in scounts]
+sd = [srng.normal(size=(k, 33)).astype(np.float32) for k in scounts]
+st_en = [srng.normal(size=(3, k)).astype(np.float32) for k in scounts]
+sglue.align(slog, sd, st_en)
+try:
+    sglue.align(slog, sd, st_en, frame_stride=2)
+except _lib.FluidAudioError:
+    pass
+slog[1][5, 2] = np.nan
+try:
+    sglue.align(slog, sd, st_en, frame_stride=2000)
+except ST.StyleTTS2Error:
+    pass
 _lib.synchronize()
 print("sanitize target done")
