@@ -280,6 +280,14 @@ STYLETTS2_SYMBOLS = [
 ]
 
 
+# every symbol include/fluidaudio_b200_offline_sortformer.h declares (offline Sortformer windows around the caller's
+# model)
+OFFLINE_SORTFORMER_SYMBOLS = [
+    "fa_offline_sortformer_plan", "fa_offline_sortformer_model_inputs", "fa_offline_sortformer_model_inputs_device",
+    "fa_offline_sortformer_stitch", "fa_offline_sortformer_stitch_device",
+]
+
+
 class LuxTtsPlanInfo(C.Structure):
     """fa_luxtts_plan_info's layout"""
     _fields_ = [("reason", C.c_int32), ("prompt_samples", C.c_int32), ("prompt_frames", C.c_int32),
@@ -548,6 +556,13 @@ def load():
         getattr(L, name).argtypes = [i32, vp, vp, i32, i64, i64, vp, i32, i64, i64, vp, i32, i64, i64, i64, vp, vp, vp,
                                      vp, vp]
     for name in STYLETTS2_SYMBOLS:
+        getattr(L, name).restype = C.c_int
+    L.fa_offline_sortformer_plan.argtypes = [i32, i32, vp, vp, vp]
+    for name in ("fa_offline_sortformer_model_inputs", "fa_offline_sortformer_model_inputs_device"):
+        getattr(L, name).argtypes = [i32, i32, vp, vp, vp, i64, vp, vp]
+    for name in ("fa_offline_sortformer_stitch", "fa_offline_sortformer_stitch_device"):
+        getattr(L, name).argtypes = [i32, i32, vp, vp, vp, vp]
+    for name in OFFLINE_SORTFORMER_SYMBOLS:
         getattr(L, name).restype = C.c_int
     _lib = L
     return L

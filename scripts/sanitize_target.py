@@ -324,5 +324,19 @@ try:
     sglue.align(slog, sd, st_en, frame_stride=2000)
 except ST.StyleTTS2Error:
     pass
+# offline Sortformer windows: model inputs and the stitch at three overlaps, an empty file and a refusal
+from fluidaudio_b200 import offline_sortformer as OSF
+orng = np.random.default_rng(26)
+owin = OSF.OfflineSortformerWindows()
+for oov in (0, 100, 383):
+    oframes = [1, 3072, 0, 5344]
+    omel = orng.normal(size=sum(oframes) * 128).astype(np.float32)
+    ooff = np.concatenate([[0], np.cumsum(oframes)])[:-1] * 128
+    oin, olen = owin.model_inputs(omel, ooff, oframes, oov)
+    owin.stitch(orng.random((olen.size, 384, 4), np.float32), oframes, oov, mappings=True)
+try:
+    owin.stitch(np.zeros(384 * 4, np.float32), [3, -1], 100)
+except _lib.FluidAudioError:
+    pass
 _lib.synchronize()
 print("sanitize target done")
