@@ -23,8 +23,6 @@ constexpr float kDefaultMinScore = -15.0f;          // ContextBiasingConstants.d
 constexpr float kNeg = -FLT_MAX;                    // -Float.greatestFiniteMagnitude
 constexpr float kLog2 = 0.69314718f;
 
-FA_HD float f_exp(float x) { return (float)exp((double)x); }
-
 // ------------------------------------------------------------------------------------------------ log-softmax
 // One row of applyLogSoftmax: x(v) reads logit v, out(v, value) writes log-prob v.  Temperature division only when it
 // is not 1, the max as Sequence.max() finds it (a later element replaces the running max only when it is greater), the

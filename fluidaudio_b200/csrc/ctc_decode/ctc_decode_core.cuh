@@ -35,7 +35,7 @@ FA_HD float log_add_exp(float a, float b) {
     if (a == -INFINITY) return b;
     if (b == -INFINITY) return a;
     const float m = swift_max(a, b);
-    return f_add(m, f_log(f_add(ctc::f_exp(f_sub(a, m)), ctc::f_exp(f_sub(b, m)))));
+    return f_add(m, f_log(f_add(f_exp(f_sub(a, m)), f_exp(f_sub(b, m)))));
 }
 
 // CtcBeam.total: totalAcoustic + lmScore

@@ -42,7 +42,8 @@ struct FrameDecision {
 };
 
 // One frame: x[classes] logits in, logp[classes] = x + (-logSumExp(x)) out (:337-346); logp may alias x.  The sum of the
-// shifted exponentials runs in class order (vDSP_sve's order is closed; so are vvexpf's bits, see DESIGN §2).
+// shifted exponentials runs in class order (vDSP_sve's order is closed; so are vvexpf's bits, see DESIGN §2), and exp
+// and log are the correctly rounded f_exp / f_log.
 FA_HD FrameDecision decode_frame(const float *x, int classes, float onset, float *logp) {
     FrameDecision d;
     d.best = 0;
@@ -57,9 +58,9 @@ FA_HD FrameDecision decode_frame(const float *x, int classes, float onset, float
         if (m < x[c]) m = x[c];
     const float shift = -m;
     float sum = 0.0f;
-    for (int c = 0; c < classes; ++c) sum = f_add(sum, expf(f_add(x[c], shift)));
-    const float neg_lse = -f_add(logf(sum), m);
-    const float empty = expf(f_add(x[0], neg_lse));  // probabilityBuffer[emptyClassIndex]
+    for (int c = 0; c < classes; ++c) sum = f_add(sum, f_exp(f_add(x[c], shift)));
+    const float neg_lse = -f_add(f_log(sum), m);
+    const float empty = f_exp(f_add(x[0], neg_lse));  // probabilityBuffer[emptyClassIndex]
     for (int c = 0; c < classes; ++c) logp[c] = f_add(x[c], neg_lse);
     const float speech = swift_max(0.0f, swift_min(1.0f, f_sub(1.0f, empty)));
     d.speech = speech >= onset ? 1 : 0;

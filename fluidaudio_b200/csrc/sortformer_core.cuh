@@ -13,7 +13,7 @@
 //
 // Every float32 operation the reference states is one round-to-nearest operation here (__f*_rn on the device, plain
 // operators on the host, whose build keeps contraction off).  vForce.log / log1p are Accelerate's and closed: both
-// sides compute (float)log((double)x) and (float)log1p((double)x) instead (DESIGN §4.7).
+// sides compute the correctly rounded float32 log and log1p instead (fa_float.cuh, DESIGN §4.7).
 //
 // Both selections (the per-speaker boosts and the global top-k) are insertion sorts in the reference.  Each keeps the
 // first k elements of a strict total order on (value, index) for non-NaN input, so an element is kept exactly when

@@ -5,6 +5,7 @@
 // StyleTTS2NoiseSource itself.
 #pragma once
 
+#include "../fa_float.cuh"
 #include "../luxtts/luxtts_core.cuh"
 
 #include <cmath>
@@ -28,14 +29,11 @@ FA_HD float fmul(float a, float b) { return __fmul_rn(a, b); }
 FA_HD float fadd(float a, float b) { return __fadd_rn(a, b); }
 FA_HD float fsub(float a, float b) { return __fsub_rn(a, b); }
 FA_HD float fdiv(float a, float b) { return __fdiv_rn(a, b); }
-// expf(v) as float64 exp rounded once to float32
-FA_HD float exp_f32(float v) { return __double2float_rn(exp((double)v)); }
 #else
 FA_HD float fmul(float a, float b) { return a * b; }
 FA_HD float fadd(float a, float b) { return a + b; }
 FA_HD float fsub(float a, float b) { return a - b; }
 FA_HD float fdiv(float a, float b) { return a / b; }
-FA_HD float exp_f32(float v) { return (float)std::exp((double)v); }
 #endif
 
 // resolveBucket with the default 57-token model in front: 57, 64, 128 or 256 (0 with a reason otherwise)
@@ -55,11 +53,11 @@ FA_HD float noise_at(uint64_t seed, int j) { return luxtts::gaussian_at(luxtts::
 // blendStyle, one element: w * p + (1 - w) * r, 1 - w in float32, each product and sum rounded separately
 FA_HD float blend(float w, float p, float r) { return fadd(fmul(w, p), fmul(fsub(1.0f, w), r)); }
 
-// roundDurations for one token: the float32 sum of 1 / (1 + expf(-x)) over its C logits in channel order, rounded
-// half away from zero, at least 1.  A NaN sum (any NaN logit) returns -1: Swift's Int(NaN) traps.
+// roundDurations for one token: the float32 sum of 1 / (1 + expf(-x)) over its C logits in channel order, expf the
+// correctly rounded f_exp, rounded half away from zero, at least 1.  A NaN sum (any NaN logit) returns -1: Swift's Int(NaN) traps.
 FA_HD int duration_of(const float *logits, int channels) {
     float sum = 0.0f;
-    for (int c = 0; c < channels; ++c) sum = fadd(sum, fdiv(1.0f, fadd(1.0f, exp_f32(-logits[c]))));
+    for (int c = 0; c < channels; ++c) sum = fadd(sum, fdiv(1.0f, fadd(1.0f, fp::f_exp(-logits[c]))));
     if (sum != sum) return -1;
     const int r = (int)roundf(sum);
     return r < 1 ? 1 : r;

@@ -12,7 +12,7 @@
 //
 // Every float32 operation the reference states is one round-to-nearest operation (fa_float.cuh).  Frame indices are
 // int64 (Swift's Int) and the `.min` sentinels are INT64_MIN; create rejects negative pads and minimum durations, which
-// would overflow them (Swift traps there).  `.logits` is log(c / (1 - c)) with f_log = (float)log((double)x) (DESIGN §4.8).
+// would overflow them (Swift traps there).  `.logits` is log(c / (1 - c)) with f_log the correctly rounded float32 log (DESIGN §4.8).
 #pragma once
 
 #include "../../include/fluidaudio_b200.h"

@@ -5,21 +5,23 @@
 // (+Inference.swift:96-126, :329-346) and CtcDPAlgorithm (CtcDPAlgorithm.swift:121-392): fillDPTable with its full
 // (T+1) x (2N+1) tables, ctcWordSpotConstrained and ctcWordSpotMultiple, written from the reference's description and
 // not from the kernels' rolling formulation.  Built with -O2 -ffp-contract=off (oracle_ctc.py), so every float
-// operation is one IEEE operation; exp and log are (float)exp((double)x) and (float)log((double)x), the library's
-// stand-ins for Apple's closed libm.
+// operation is one IEEE operation; exp and log are the correctly rounded float32 functions of oracle_float.h, the
+// library's definition in place of Apple's closed libm.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
 #include <vector>
 
+#include "oracle_float.h"
+
 namespace {
 
 const float kNegMax = -FLT_MAX;
 const int kWildcard = -1;
 
-float fexp(float x) { return (float)std::exp((double)x); }
-float flog(float x) { return (float)std::log((double)x); }
+float fexp(float x) { return oracle_float::exp32(x); }
+float flog(float x) { return oracle_float::log32(x); }
 
 enum Kind { kBlank, kToken, kWild };
 struct Sym {

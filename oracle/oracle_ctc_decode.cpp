@@ -2,7 +2,7 @@
 // ARPALanguageModel.swift): ctcGreedyDecode, ctcBeamSearch with its LM terms, ARPALanguageModel.score and logAddExp.
 // Prefixes are ids of a consed trie ((parent, token) -> id), beams an insertion-ordered map (a vector with an index by
 // prefix id), the prune a stable sort: the reference's code with insertion-ordered dictionaries.  Words are byte
-// strings.  exp and log are (float)exp((double)x) and (float)log((double)x); built with -ffp-contract=off.
+// strings.  exp and log are the correctly rounded float32 functions of oracle_float.h; built with -ffp-contract=off.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -11,13 +11,15 @@
 #include <unordered_map>
 #include <vector>
 
+#include "oracle_float.h"
+
 namespace {
 
 const float kUnk = -23.026f;
 const std::string kBoundary = "\xE2\x96\x81";
 
-float f_exp(float x) { return (float)std::exp((double)x); }
-float f_log(float x) { return (float)std::log((double)x); }
+float f_exp(float x) { return oracle_float::exp32(x); }
+float f_log(float x) { return oracle_float::log32(x); }
 
 float log_add_exp(float a, float b) {
     if (a == -INFINITY) return b;

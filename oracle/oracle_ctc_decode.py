@@ -26,7 +26,8 @@ _lib = None
 
 def build(force: bool = False) -> None:
     """Compile liboracle_ctc_decode.so when it is missing or older than a source."""
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(s) > os.path.getmtime(_LIB) for s in _SRCS):
+    deps = _SRCS + [os.path.join(_HERE, "oracle_float.h")]
+    if force or not os.path.exists(_LIB) or any(os.path.getmtime(s) > os.path.getmtime(_LIB) for s in deps):
         cxx = os.environ.get("CXX", "g++")
         subprocess.check_call([cxx, *_FLAGS, "-o", _LIB, *_SRCS])
 

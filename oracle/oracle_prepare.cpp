@@ -7,14 +7,16 @@
 //   Utils/VDSPOperations.swift:142-155                                   logSumExp
 //   Extraction/WeightInterpolation.swift:19-146                          resample
 //   Extraction/OfflineEmbeddingExtractor.swift:338-351,381-387,421-707,807-842   the embedding stage's bookkeeping
-// Built with -O2 -ffp-contract=off on baseline x86-64: every operation is rounded as written.  expf / logf are the host
-// libm's (Apple's vvexpf is closed) and every vDSP sum runs in index order (vDSP's order is closed).
+// Built with -O2 -ffp-contract=off on baseline x86-64: every operation is rounded as written.  expf / logf are the correctly
+// rounded float32 exp / log of oracle_float.h (Apple's vvexpf is closed) and every vDSP sum runs in index order (vDSP's order is closed).
 #include <algorithm>
 #include <cfloat>
 #include <climits>
 #include <cmath>
 #include <cstdint>
 #include <vector>
+
+#include "oracle_float.h"
 
 namespace {
 
@@ -31,10 +33,10 @@ float log_sum_exp(const float *x, int n) {
     const float shift = -max_element;
     std::vector<float> shifted(n);
     for (int i = 0; i < n; ++i) shifted[i] = x[i] + shift;
-    for (int i = 0; i < n; ++i) shifted[i] = expf(shifted[i]);
+    for (int i = 0; i < n; ++i) shifted[i] = oracle_float::exp32(shifted[i]);
     float sum = 0;
     for (int i = 0; i < n; ++i) sum += shifted[i];
-    return logf(sum) + max_element;
+    return oracle_float::log32(sum) + max_element;
 }
 
 std::vector<float> resample(const std::vector<float> &input, int output_length) {
@@ -129,7 +131,7 @@ void oracle_seg_decode(const float *logits, int chunks, int frames, int classes,
             }
         const float shift = -log_sum_exp(x, classes);
         for (int cls = 0; cls < classes; ++cls) lp[cls] = x[cls] + shift;
-        for (int cls = 0; cls < classes; ++cls) probability[cls] = expf(lp[cls]);
+        for (int cls = 0; cls < classes; ++cls) probability[cls] = oracle_float::exp32(lp[cls]);
         if (best_index < 8) histogram[best_index] += 1;
         const int winning = std::min(best_index, 7);
         float *w = weights + frame * speaker_count;

@@ -6,7 +6,7 @@
 //   SortformerStateUpdater.swift:31-578       streamingUpdate, updateSilenceProfile, compressSpkcache and its helpers
 // The state is held as the reference holds it (growing arrays, optional prediction arrays), and both top-k selections
 // are the reference's insertion sorts as written, so this file shares nothing with the GPU's rank counting.
-// vForce.log / log1p (Accelerate, closed) are computed as (float)log((double)x) / (float)log1p((double)x).
+// vForce.log / log1p (Accelerate, closed) are the correctly rounded float32 log / log1p of oracle_float.h.
 // Compiled with -O2 -ffp-contract=off on baseline x86-64: every float32 operation is rounded as written.
 //
 // C interface (one session per handle):
@@ -26,6 +26,8 @@
 #include <cstring>
 #include <limits>
 #include <vector>
+
+#include "oracle_float.h"
 
 namespace {
 
@@ -62,8 +64,8 @@ struct Session {
     std::vector<float> lastPopEmbs, lastPopPreds;   // the rows the last update popped (none: empty)
 };
 
-float vlog(float x) { return (float)std::log((double)x); }
-float vlog1p(float x) { return (float)std::log1p((double)x); }
+float vlog(float x) { return oracle_float::log32(x); }
+float vlog1p(float x) { return oracle_float::log1p32(x); }
 float clipf(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
 int swiftInt(float v) { return (int)v; }
 

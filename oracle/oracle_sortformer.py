@@ -31,7 +31,8 @@ _lib = None
 
 def build(force: bool = False) -> None:
     """Compile liboracle_sortformer.so when it is missing or older than its source."""
-    if force or not os.path.exists(_LIB) or os.path.getmtime(_SRC) > os.path.getmtime(_LIB):
+    deps = (_SRC, os.path.join(_HERE, "oracle_float.h"))
+    if force or not os.path.exists(_LIB) or any(os.path.getmtime(s) > os.path.getmtime(_LIB) for s in deps):
         cxx = os.environ.get("CXX", "g++")
         subprocess.check_call([cxx, *_FLAGS, "-o", _LIB, _SRC])
 

@@ -3,13 +3,15 @@
 // A sequential CPU restatement of StyleTTS2Synthesizer.synthesize's glue between its models (Sources/FluidAudio/TTS/
 // StyleTTS2/Pipeline/Synthesize/StyleTTS2Synthesizer.swift:33-133 and StyleTTS2GlueOps.swift:23-161) and of
 // StyleTTS2NoiseSource (Pipeline/Sampler/StyleTTS2DiffusionSchedule.swift:45-81), line by line in the reference's
-// order.  Where the reference calls a closed library this file takes a stated reading: expf is float64 exp rounded
-// once to float32; cblas_sgemm is netlib's loop (C zeroed for beta = 0, then for each column j and each l with
+// order.  Where the reference calls a closed library this file takes a stated reading: expf is the correctly rounded
+// float32 exp of oracle_float.h; cblas_sgemm is netlib's loop (C zeroed for beta = 0, then for each column j and each l with
 // B(l, j) != 0, C(:, j) += (alpha B(l, j)) A(:, l)); vDSP_mtrans is the plain copy.  Built with -O2
 // -ffp-contract=off on baseline x86-64.
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
+
+#include "oracle_float.h"
 
 namespace {
 
@@ -37,7 +39,7 @@ struct Noise {
     }
 };
 
-float expf_pinned(float x) { return float(std::exp(double(x))); }
+float expf_pinned(float x) { return oracle_float::exp32(x); }
 
 } // namespace
 

@@ -7,12 +7,14 @@
 // commitSegment (:1297-1336) are stated as the Swift states them; the speakers' segment storage is left to the caller.
 //
 // Built with the pinned flags (-O2 -ffp-contract=off, baseline x86-64): every float operation is one IEEE single
-// operation in the order written.  Swift's Int is int64_t, `.min` is INT64_MIN, and `log` on Float is computed as
-// (float)log((double)x) (the library does the same; DESIGN §4.8).  maxStoredFrames < 0 stands for nil (unlimited).
+// operation in the order written.  Swift's Int is int64_t, `.min` is INT64_MIN, and `log` on Float is the correctly
+// rounded float32 log of oracle_float.h (the library's definition; DESIGN §4.8).  maxStoredFrames < 0 stands for nil (unlimited).
 #include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <vector>
+
+#include "oracle_float.h"
 
 namespace {
 
@@ -43,7 +45,7 @@ float evaluate(const Config &c, float p) {
     if (!c.logits) return p;
     const float eps = 1e-6f;
     const float clamped = swiftMin(swiftMax(p, eps), 1 - eps);
-    return (float)std::log((double)(clamped / (1 - clamped)));
+    return oracle_float::log32(clamped / (1 - clamped));
 }
 
 struct Timeline {

@@ -1,11 +1,11 @@
 """A literal pure-Python restatement of ctcGreedyDecode, ctcBeamSearch, logAddExp and ARPALanguageModel.score
 (CtcDecoder.swift, ARPALanguageModel.swift), independent of ``oracle/oracle_ctc_decode.cpp``: beams in a ``dict`` keyed
 by the prefix tuple (insertion-ordered, as the contract fixes the reference's hash order), the prune a stable
-``sorted(..., reverse=True)``, word pieces as lists of strings, float32 arithmetic through numpy, and exp / log as
-``float32(exp(float64(x)))`` / ``float32(log(float64(x)))``, the library's libm policy."""
-import math
-
+``sorted(..., reverse=True)``, word pieces as lists of strings, float32 arithmetic through numpy, and exp / log the
+correctly rounded float32 functions of ``tests/float_exact.py``, the library's definition."""
 import numpy as np
+
+import float_exact
 
 F = np.float32
 NEG_INF = F(-np.inf)
@@ -13,12 +13,8 @@ BOUNDARY = "▁"
 UNK = F(-23.026)
 
 
-def f_exp(x):
-    return F(math.exp(float(x)))
-
-
-def f_log(x):
-    return F(math.log(float(x)))
+f_exp = float_exact.exp
+f_log = float_exact.log
 
 
 def log_add_exp(a, b):

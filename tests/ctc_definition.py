@@ -4,7 +4,7 @@ as a maximum over explicitly enumerated alignments.  Written from the definition
 so that a misreading the kernels and the oracles share shows up as a disagreement here.
 
 Rounding bars.  The decoder's float32 arithmetic is `log_add_exp(a, b) = m + f_log(f_exp(a - m) + f_exp(b - m))` with
-f_exp / f_log the correctly rounded (float)exp((double)x) / (float)log((double)x) of fa_float.cuh, plus one float32 add
+f_exp / f_log the correctly rounded float32 exp / log of fa_float.cuh (checked on every input by test_float_rounding.py), plus one float32 add
 per emission.  With u = 2^-24, one log_add_exp whose exact result is r is off by at most u * (|r| + 3) to first order:
 the subtraction inside exp perturbs the smaller term by a relative u * |d| * e^d / (1 + e^d) <= 0.28 u, exp and the
 add of 1 + e each round once (together <= 2 u relative on the sum, so <= 2 u absolute after the log), the log rounds

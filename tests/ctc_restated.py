@@ -1,32 +1,22 @@
 """Pure-Python restatement of CTC keyword spotting (test infrastructure): applyLogSoftmax, mergeOverlapFrame and the
 chunk concatenation (CtcKeywordSpotter.swift:268-306, +Inference.swift:96-126, :329-346) and CtcDPAlgorithm
-(CtcDPAlgorithm.swift:121-392), every float operation a numpy float32 scalar operation and exp / log the double
-functions rounded to float32.  It holds the C++ oracle (oracle/oracle_ctc.cpp) to the reference's description on small
+(CtcDPAlgorithm.swift:121-392), every float operation a numpy float32 scalar operation and exp / log the correctly
+rounded float32 functions (tests/float_exact.py).  It holds the C++ oracle (oracle/oracle_ctc.cpp) to the reference's description on small
 cases; it is slow and written for clarity.
 """
 from __future__ import annotations
 
-import math
-
 import numpy as np
+
+import float_exact
 
 F = np.float32
 NEG = F(-np.finfo(np.float32).max)
 WILDCARD = -1
 
 
-def fexp(x):
-    try:
-        return F(math.exp(float(x)))
-    except OverflowError:
-        return F(np.inf)
-
-
-def flog(x):
-    x = float(x)
-    if x == 0.0:
-        return F(-np.inf)
-    return F(math.log(x)) if x > 0 else F(np.nan)
+fexp = float_exact.exp
+flog = float_exact.log
 
 
 def log_softmax(logits, temperature=1.0, blank_bias=0.0, blank_id=1024):

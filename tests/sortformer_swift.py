@@ -5,14 +5,16 @@ It is meant to be read beside the Swift: line numbers in the comments are Sortfo
 comment names SortformerTypes.swift.  The state is held as the Swift holds it: flat Python lists that grow by
 ``append(contentsOf:)`` and shrink by ``removeFirst``, and optional prediction arrays (None for nil).  Both top-k
 selections are the Swift's insertion sorts as written.  Every arithmetic step is one np.float32 scalar operation in the
-Swift's order.  The one deviation is the documented one (DESIGN §4.7): vForce.log / log1p are (float)log((double)x) and
-(float)log1p((double)x).
+Swift's order.  The one deviation is the documented one (DESIGN §4.7): vForce.log / log1p are the correctly rounded float32
+log and log1p (tests/float_exact.py).
 """
 from __future__ import annotations
 
 from types import SimpleNamespace
 
 import numpy as np
+
+import float_exact
 
 F32 = np.float32
 S, D = 4, 512                  # numSpeakers, preEncoderDims (SortformerTypes.swift:23-26)
@@ -23,14 +25,8 @@ LOGF_2 = F32(np.log(2.0))      # logf(2), correctly rounded
 LOGF_HALF = F32(np.log(0.5))   # logf(0.5) = -logf(2)
 
 
-def vlog(x):
-    with np.errstate(all="ignore"):
-        return F32(np.log(np.float64(x)))
-
-
-def vlog1p(x):
-    with np.errstate(all="ignore"):
-        return F32(np.log1p(np.float64(x)))
+vlog = float_exact.log
+vlog1p = float_exact.log1p
 
 
 def clip(x, lo, hi):

@@ -1,12 +1,13 @@
 """A literal Python restatement of StyleTTS2Synthesizer.synthesize's glue (test infrastructure), written from the Swift
 source independently of oracle_styletts2.cpp: the bucket choice, bert's padding and mask, StyleTTS2NoiseSource
-(luxtts_restated.Noise, the same Swift struct), roundDurations with numpy float32 scalars and expf as float64 exp
-rounded to float32, buildAlignmentMatrix, matmulAligned as netlib's loop, transposeLast2D, hifiganShift, blendStyle
+(luxtts_restated.Noise, the same Swift struct), roundDurations with numpy float32 scalars and expf the correctly
+rounded float32 exp (float_exact.py), buildAlignmentMatrix, matmulAligned as netlib's loop, transposeLast2D, hifiganShift, blendStyle
 and the tail trim."""
 import math
 
 import numpy as np
 
+import float_exact
 from luxtts_restated import Noise
 
 F = np.float32
@@ -33,11 +34,7 @@ def sampler_inputs(ids, padded_t, seed):
     return tokens, mask, noise_init, noises_aux
 
 
-def _expf(x):
-    try:
-        return F(math.exp(float(x)))
-    except OverflowError:
-        return F(np.inf)
+_expf = float_exact.exp
 
 
 def round_durations(logits):

@@ -19,6 +19,7 @@ import zlib
 import numpy as np
 import pytest
 
+import float_exact
 from fluidaudio_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -95,7 +96,7 @@ class PyTimeline:
         lo = eps if eps >= p else p                     # Swift.max(p, eps) = eps >= p ? eps : p
         hi = F(1) - eps
         c = hi if hi < lo else lo                       # Swift.min(lo, hi) = hi < lo ? hi : lo
-        return F(math.log(float(F(c / (F(1) - c)))))
+        return float_exact.log(F(c / (F(1) - c)))
 
     def commit(self, a, spk, finalized, out):
         if not a.has_segment:
