@@ -1,5 +1,6 @@
-// The guard every status-returning C ABI entry point returns through (capi.cu, export_io.cu).  No exception crosses
-// the extern "C" boundary, and a failing call leaves fa_last_error() text that describes its own failure.
+// The guard every status-returning C ABI entry point returns through (capi.cu, the *_abi.cu files, export_io.cu).  No
+// exception crosses the extern "C" boundary, and a failing call leaves fa_last_error() text that describes its own
+// failure.
 #pragma once
 
 #include "../../include/fluidaudio_b200.h"

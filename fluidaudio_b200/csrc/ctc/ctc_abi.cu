@@ -27,11 +27,6 @@ bool offsets_ok(const int64_t *off, int count, long long max_span) {
     return true;
 }
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 // The first term or query longer than the kernels support, or -1
 int too_long(const int64_t *off, int count) {
     for (int i = 0; i < count; ++i)

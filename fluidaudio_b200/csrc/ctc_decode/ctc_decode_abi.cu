@@ -35,11 +35,6 @@ bool offsets_ok(const int64_t *off, long long count, long long max_span) {
     return true;
 }
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 // An open-addressing table of `keys` (none kEmpty) with their values, probed as ctc_decode_core.cuh probes it
 template <typename V>
 void hash_table(const std::vector<std::pair<unsigned long long, V>> &kv, std::vector<unsigned long long> &keys,

@@ -36,6 +36,11 @@ namespace fa {
 // thread-local last-error text, set by the C ABI on every failure
 void set_error(const char *fmt, ...);
 const char *last_error();
+// An argument check's refusal: sets the text and returns FA_INVALID_ARGUMENT (= FA_STATUS_INVALID_ARGUMENT).
+template <typename... A> int refuse(const char *fmt, A... args) {
+    set_error(fmt, args...);
+    return FA_INVALID_ARGUMENT;
+}
 
 // Slices one allocation into 256-byte aligned arrays.  Carver{nullptr} is a dry run: `off` then holds the bytes the
 // arrays need (carve_arena below runs a layout both ways).
@@ -253,6 +258,13 @@ struct Event : std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDestroy>
         return FA_OK;
     }
 };
+// Creates both timer events, or neither: a failed creation leaves the timer unset, so the next start tries again.
+inline int create_timer(Event (&ev)[2]) {
+    int st = ev[0].create();
+    if (st == FA_OK) st = ev[1].create();
+    if (st != FA_OK) ev[0].reset();
+    return st;
+}
 
 // Launch descriptors written in a pinned buffer and uploaded to its device twin.  An asynchronous call returns with its
 // upload still queued, so the pinned copy may be rewritten (or replaced) only once that upload has read it: reserve()

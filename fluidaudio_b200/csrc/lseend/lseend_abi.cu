@@ -1,6 +1,6 @@
 // C ABI of the LS-EEND feature streams (declared in include/fluidaudio_b200_lseend.h): LSEENDFeatureProvider
 // (LSEENDPreprocessor.swift:46-384) for many live sessions in HBM, lseend_plan.h and lseend_streams.cu.  Every entry point
-// that returns a status returns through guard() (c_abi.h), as in capi.cu.
+// that returns a status returns through guard() (c_abi.h), as in every family's C ABI file.
 #include "../../../include/fluidaudio_b200_lseend.h"
 #include "c_abi.h"
 #include "lseend_streams.h"

@@ -22,11 +22,6 @@ using namespace fa::luxtts;
 
 namespace {
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 fa_luxtts_plan_info info_of(const Mirror &m) {
     const Plan &p = m.plan;
     return fa_luxtts_plan_info{p.reason,     p.prompt_samples, p.prompt_frames,  p.token_count, p.features_length,

@@ -156,11 +156,6 @@ __global__ void __launch_bounds__(kThreads)
     out[J.out + k] = s;
 }
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_INVALID_ARGUMENT;
-}
-
 unsigned tiles(long long n, long long per) { return (unsigned)std::max(1LL, (n + per - 1) / per); }
 
 } // namespace

@@ -1,6 +1,7 @@
 // Host-buffer pipelines of the log-mel plan: host samples in, host rows out, with the copies of one unit overlapping the
 // kernels of the next (MelPlan::compute_host: one clip, any AudioFormat, through the converter stage; compute_batch_host:
-// a batch of float32 clips in groups).  The launches themselves are MelPlan::launch (mel_kernels.cu).
+// a batch of float32 clips in groups).  The launches themselves are MelPlan::launch (mel_kernels.cu).  Also the plan's
+// event timer on its compute stream (fa_mel_timer_*).
 #include "mel_core.cuh"
 #include "mel_plan.h"
 
@@ -329,6 +330,24 @@ int MelPlan::compute_batch_host(const float *audio, const int64_t *offsets, int 
     }
     FA_CUDA_TRY(cudaStreamSynchronize(s_out));
     FA_CUDA_TRY(cudaStreamSynchronize(s_k));
+    return FA_OK;
+}
+
+int MelPlan::timer_start() {
+    if (!timer[0]) {
+        const int st = create_timer(timer);
+        if (st != FA_OK) return st;
+    }
+    FA_CUDA_TRY(cudaStreamSynchronize(streams[1]));
+    FA_CUDA_TRY(cudaEventRecord(timer[0], streams[1]));
+    return FA_OK;
+}
+
+int MelPlan::timer_stop_ms(float *elapsed_ms) {
+    if (!timer[0]) return FA_INVALID_ARGUMENT;
+    FA_CUDA_TRY(cudaEventRecord(timer[1], streams[1]));
+    FA_CUDA_TRY(cudaEventSynchronize(timer[1]));
+    FA_CUDA_TRY(cudaEventElapsedTime(elapsed_ms, timer[0], timer[1]));
     return FA_OK;
 }
 

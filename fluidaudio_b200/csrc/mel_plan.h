@@ -131,6 +131,10 @@ struct MelPlan {
     // One .center launch of exactly T frames of one n-sample clip at d_in, whatever n (an empty clip reads zeros): the
     // torch-style frontends count their frames by their own rules (mel_adapters.cu).  last = 0.
     int launch_clip(const float *d_in, long long n, long long T, int layout, float *d_out_buf, cudaStream_t stream);
+    // CUDA-event timing on the stream the mel kernels are launched on (device-resident entry points are asynchronous).
+    // timer_stop_ms refuses a timer that was never started.
+    int timer_start();
+    int timer_stop_ms(float *elapsed_ms);
 };
 
 // Numbers a run of units that one launch covers: sets each unit's tile_begin and returns the run's tile total.

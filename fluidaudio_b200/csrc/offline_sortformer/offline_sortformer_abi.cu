@@ -18,11 +18,6 @@ namespace {
 constexpr long long kMaxFrames = 1LL << 40;
 constexpr long long kMaxWindows = 1LL << 24;
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 // Checks the frame counts and sums the files' windows and output rows
 int count_files(const char *where, int count, const int64_t *mel_frames, int overlap, long long *windows,
                 long long *rows) {

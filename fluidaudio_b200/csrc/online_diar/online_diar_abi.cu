@@ -23,11 +23,6 @@ using namespace fa::od;
 
 namespace {
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 // 16000 * Int(x.rounded()), where it stays below 2^40 samples
 bool samples_of(float x, long long *out) {
     const double r = std::round((double)x);

@@ -2,6 +2,7 @@
 // mono float32 at the model rate, written straight into the buffer the log-mel kernel reads (no host round trip).
 // See resample_plan.h for the reference lines and the filter design.
 #include "resample_plan.h"
+#include "call_context.h"
 #include "resample_core.cuh"
 
 #include <algorithm>
@@ -258,6 +259,31 @@ int launch_convert(const void *d_pcm, long long frames, const AudioFormat &f, co
                                            : launch_sinc<unsigned long long>(s, d, d_tab, d_out, o_begin, o_end, grid, stream);
     }
     return FA_OK;
+}
+
+int convert_host(const void *pcm, long long frames, const AudioFormat &f, float *out, long long n) {
+    Design d;
+    if (f.in_rate != f.out_rate) {
+        const int st = make_design(f.in_rate, f.out_rate, d);
+        if (st != FA_OK) return st;
+    }
+    const size_t bytes = (size_t)frames * f.channels * (f.format == kPcmI16 ? 2 : 4);
+    return with_context(0, [&](CallContext &C) -> int {
+        HostStaging H(true, C.stream);
+        const char *d_pcm;
+        const float *d_tab;
+        float *d_out;
+        int st = H.carve(C.d_buf, [&](HostStaging::Layout &l) {
+            d_pcm = l.in(static_cast<const char *>(pcm), bytes, 16);
+            d_tab = l.in(d.table.empty() ? nullptr : d.table.data(), d.table.size());
+            d_out = l.out(out, (size_t)n);
+        });
+        if (st != FA_OK) return st;
+        st = launch_convert(d_pcm, frames, f, d, d_tab, d_out, 0, n, C.stream);
+        if (st != FA_OK) return st;
+        FA_CUDA_TRY(H.finish());
+        return FA_OK;
+    });
 }
 
 } // namespace resample

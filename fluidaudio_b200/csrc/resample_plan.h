@@ -34,6 +34,7 @@
 //     |g_{p,k}| + |g_{p+1,k}| where two rows are blended (four FMA chains, two adds, float32 taps, the blend).
 #pragma once
 
+#include "../../include/fluidaudio_b200.h"
 #include "fa_common.cuh"
 #include <cuda_runtime.h>
 #include <vector>
@@ -85,6 +86,14 @@ int launch_convert(const void *d_pcm, long long frames, const AudioFormat &f, co
 // number of leading outputs computable when only the first `frames_avail` input frames are resident
 long long outputs_ready(const AudioFormat &f, const Design &d, long long frames, long long frames_avail,
                         long long out_total);
+// The converter stage on host buffers, on a leased call context: frames [0, frames) of `pcm` (layout per `f`) into the
+// n = output_count(frames, f.in_rate, f.out_rate) > 0 samples of `out`.  Returns once `out` holds them.
+int convert_host(const void *pcm, long long frames, const AudioFormat &f, float *out, long long n);
+
+// The C ABI's check of a caller's fa_audio_format, with error text when it fails, and its conversion (resample_abi.cu):
+// shared by fa_audio_resample and fa_audio_to_mel.
+bool audio_format_ok(const fa_audio_format *f);
+AudioFormat to_format(const fa_audio_format *f);
 
 } // namespace resample
 } // namespace fa

@@ -15,11 +15,6 @@ using namespace fa::styletts2;
 
 namespace {
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 int sampler_call(int count, const int32_t *ids, const int64_t *offsets, const uint64_t *seeds, int bucket,
                  int32_t *tokens, int32_t *mask, float *noise, int32_t *reasons, bool device) {
     const char *where = device ? "fa_styletts2_sampler_inputs_device" : "fa_styletts2_sampler_inputs";

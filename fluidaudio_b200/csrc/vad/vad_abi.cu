@@ -18,11 +18,6 @@ using namespace fa::vad;
 
 namespace {
 
-template <typename... A> int refuse(const char *fmt, A... args) {
-    set_error(fmt, args...);
-    return FA_STATUS_INVALID_ARGUMENT;
-}
-
 // Int(seconds * 16000.0) for a finite, non-negative duration whose count is below 2^62, so that 2 * count and every
 // sample position plus or minus a count stay inside int64
 bool samples_of(double seconds, long long *out) {
